@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- the hot path's headline metric on B200: generated audio samples per second
+"""bench.py -- the hot path's headline metric on an H100: generated audio samples per second
 (22.05 kHz) of batched MoL WaveRNN.generate(), BASELINE.json configs[1]:
 a 10-second 80-bin mel (T=800 frames) folded with target=11000 / overlap=550 into 19 folds x
 12,100 steps, rnn_dims=512, random-init weights, synthetic mel.
@@ -16,6 +16,9 @@ One "step" = one full pass of the hot path over the workload (all folds x all st
            the kernel, D2H of the samples and the host epilogue (xfade/unfold), wall clock.
 N > 1    : weak scaling -- the mel is lengthened so every rank owns 19 folds; one NCCL
            all-gather of the sample blocks is inside the timed region.
+--dump-outputs DIR : after the timed steps, rank 0 writes what the timed calls returned in their last step as
+           DIR/<name>.npy (float32 / float64; a fixed sample of the folds when the block exceeds 64 MB), so that two
+           builds can be compared output for output on identical seeded inputs.
 """
 from __future__ import annotations
 
@@ -75,27 +78,37 @@ def build_model(device, mode="MOL"):
     return m.to(device)
 
 
-def measured_traffic(args, model):
-    """dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the dominant kernel on this workload, taken from
-    the committed ncu --set full capture (profiles/r02_tc_traffic.json, else round 1's); None when no capture matches."""
-    if args.workload != "cfg2" or args.seg_steps:
-        return None
-    for name in ("r02_tc_traffic.json", "r01_tc_traffic.json"):
-        p = ROOT / "profiles" / name
-        if p.is_file():
-            d = json.loads(p.read_text())
-            if str(d.get("engine", "")).startswith("tcgen05"):
-                return d.get("dram_bytes_per_launch")
-    return None
+DUMP_LIMIT = 64 << 20                    # bytes written by --dump-outputs in all
+
+
+def dump_outputs(directory, arrays: dict):
+    """Writes each array as <directory>/<name>.npy.  An array larger than its share of DUMP_LIMIT is cut to a fixed,
+    seeded sample of its rows (the folds of a 2-D block, the samples of a waveform), whose indices are stored next to it
+    as <name>_rows.npy."""
+    d = Path(directory)
+    d.mkdir(parents=True, exist_ok=True)
+    share = DUMP_LIMIT // (2 * max(1, len(arrays)))          # half of the share for the values, half for the indices
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        if a.nbytes > share:
+            row_bytes = a.itemsize * (a.shape[1] if a.ndim == 2 else 1)
+            keep = max(1, min(a.shape[0], share // row_bytes))
+            rows = np.sort(np.random.RandomState(0).choice(a.shape[0], keep, replace=False))
+            np.save(d / f"{name}_rows.npy", rows.astype(np.float64))
+            a = a[rows]
+        np.save(d / f"{name}.npy", np.ascontiguousarray(a))
 
 
 def measured_peaks():
+    """Peaks the roofline fractions divide by: MEASURED_PEAKS.json when present, else NVIDIA's data sheet for the H100 SXM
+    (dense FP16 / BF16 989 TFLOP/s, HBM3 3.35 TB/s, at up to 700 W) -- a ceiling, not a rate this card reached."""
     p = ROOT / "MEASURED_PEAKS.json"
     if p.is_file():
         d = json.loads(p.read_text())
         return dict(tflops=float(d["bf16_tflops"]), tflops_sustained=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
                     hbm_gbs=float(d["hbm_gbs"]), src="measured")
-    return dict(tflops=1590.0, tflops_sustained=1400.0, hbm_gbs=6650.0, src="fallback")
+    return dict(tflops=989.0, tflops_sustained=989.0, hbm_gbs=3350.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -231,6 +244,7 @@ def run_reference_arm(args):
             if i >= args.warmup:
                 times.append(dt)
         assert len(wav) == (frames_for(world) - 1) * HOP
+        dumps = {"wav": np.asarray(wav, dtype=np.float64)}
         kind = "reference"
         how = ("UNMODIFIED reference WaveRNN.generate() (oracle/_ref, " + ("eager torch CUDA operators on this GPU" if on_cuda else "CPU") +
                ", fp32), whole call: upsample network + fold + 12100-step loop + xfade")
@@ -238,9 +252,10 @@ def run_reference_arm(args):
         from oracle import torch_port
         for i in range(args.warmup + args.steps):
             torch.manual_seed(1234)
-            _, dt = torch_port.generate_segments_torch(sd, mels_f, aux_f, steps=sample_steps)
+            samples, dt = torch_port.generate_segments_torch(sd, mels_f, aux_f, steps=sample_steps)
             if i >= args.warmup:
                 times.append(dt)
+        dumps = {"samples": np.asarray(samples, dtype=np.float32)}
         kind = "port"
         how = "torch-operator port of the reference loop (oracle/torch_port.py; bit-identical samples), loop only"
     per_step = float(np.mean(times))
@@ -254,6 +269,8 @@ def run_reference_arm(args):
             "cpu_baseline": {"value": value, "unit": "samples/s", "cores": threads, "kind": kind, "sample": sample},
             "e2e": {"value": value, "unit": "samples/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
             "x_realtime": value / 22050.0}
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dumps)
     emit(line)
 
 
@@ -330,14 +347,16 @@ def run_ours(args):
     barrier(); engine.check()
     launches0 = engine.launch_count
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+    samples = None
     with ClockSampler(local) as clk:
         barrier()
         ev[0].record(stream)
         for _ in range(args.steps):
-            device_step()
+            samples = device_step()
         ev[1].record(stream)
         barrier()
     engine.check()
+    dumps = {"samples": samples.float().cpu().numpy()} if samples is not None else {}
     t_dev = ev[0].elapsed_time(ev[1]) / 1e3
     gpu_launches = engine.launch_count - launches0
     clocks = clk.summary()
@@ -359,6 +378,7 @@ def run_ours(args):
         barrier()
         t_e2e = time.perf_counter() - t0
         assert np.isfinite(wav).all()
+        dumps["wav"] = np.asarray(wav, dtype=np.float64)
 
     times = torch.tensor([t_dev, t_e2e], dtype=torch.float64, device=device)
     if world > 1:
@@ -397,7 +417,7 @@ def run_ours(args):
             "e2e": {"value": e2e_value, "unit": "samples/s", "h2d_bytes_per_step": int(world * mel_host.numel() * 4 + h2d_rng),
                     "d2h_bytes_per_step": int(world * (T - 1) * HOP * 8), "ms_per_step": t_e2e / args.steps * 1e3},
             "roofline": {"bound": "tensor", "achieved": ach_tf, "peak": peak_tf, "unit": "TFLOP/s",
-                         "frac": ach_tf / peak_tf, "traffic": measured_traffic(args, model), "peak_source": peaks["src"],
+                         "frac": ach_tf / peak_tf, "traffic": None, "peak_source": peaks["src"],
                          "note": ("stream engine: one pass over the fp16 weights per step through each SM's shared memory; bounded by the MMA "
                                   "front end (~40 cycles per M=128 MMA with A from shared memory) and the ring depth, DESIGN.md 3.2") if cfg5 else
                                  ("latency/sync-bound at 19 folds per GPU (four L2 exchanges per step, DESIGN.md 3.1): fraction of the "
@@ -410,6 +430,8 @@ def run_ours(args):
             line["cpu_baseline"] = cpu
         if args.seg_steps or args.skip_e2e:
             line["partial"] = "profiling run (--seg-steps/--skip-e2e): NOT a bench value"
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, dumps)
         emit(line)
     if world > 1:
         dist.destroy_process_group()
@@ -459,6 +481,8 @@ def run_cfg4(args, device, rank, world, local):
         barrier()
         t = time.perf_counter() - t0
     assert all(np.isfinite(w).all() for w in wavs)
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, {f"wav_{i:02d}": np.asarray(w, dtype=np.float64) for i, w in enumerate(wavs)})
     tt = torch.tensor([t], dtype=torch.float64, device=device)
     if world > 1:
         dist.all_reduce(tt, op=dist.ReduceOp.MAX)
@@ -527,6 +551,8 @@ def main():
                     help="PROFILING ONLY: generate just the first N steps of every fold in the device-timed region "
                          "(keeps ncu captures short); the printed line is then marked partial and is not a bench value")
     ap.add_argument("--skip-e2e", action="store_true", help="PROFILING ONLY: skip the end-to-end leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed calls returned in their last step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference_arm(args)

@@ -1,4 +1,4 @@
-/* wavernn_b200.h -- C ABI of the Blackwell-native WaveRNN generate() engine.
+/* wavernn_b200.h -- C ABI of the Hopper-native (sm_90a) WaveRNN generate() engine.
  *
  * Drop-in boundary (SURVEY.md section 8b).  The reference (fatchord/WaveRNN) has no
  * native interface of its own: its hot path is the Python loop
@@ -32,7 +32,7 @@ enum {
   WRNN_OK = 0,
   WRNN_E_INVALID = -1,      /* bad argument / unsupported configuration            */
   WRNN_E_CUDA = -2,         /* a CUDA runtime call failed (see wrnn_last_error)     */
-  WRNN_E_NO_DEVICE = -3,    /* no sm_100 device: there is NO CPU fallback           */
+  WRNN_E_NO_DEVICE = -3,    /* no sm_90 device: there is NO CPU fallback            */
   WRNN_E_WATCHDOG = -4,     /* the persistent kernel aborted on its spin watchdog   */
   WRNN_E_BUSY = -5
 };
@@ -127,7 +127,7 @@ typedef struct {
    * (WaveRNN.generate_many; the reference vocodes sentences one at a time, gen_tacotron.py:139-163). */
   const int64_t *fold_row0;
   const int64_t *fold_row_end;
-  /* Optional frame-rate conditioning (device; tcgen05 engine).  When mel_frames != NULL the library builds the
+  /* Optional frame-rate conditioning (device; tensor-core engines).  When mel_frames != NULL the library builds the
    * conditioning rows itself and mels_up / aux are ignored (may be NULL; L stays the stream length in samples):
    *   aux row n  = aux_frames[n / hop]                      (Stretch2d is a nearest-neighbour repeat, :57-61)
    *   mel row n  = sum_{d<5} up_taps[n % hop][d] * mel_frames[n / hop + d]

@@ -24,8 +24,12 @@ FILES = ("models/__init__.py", "models/fatchord_version.py", "utils/__init__.py"
 
 
 def main() -> int:
-    if not (SRC / "models" / "fatchord_version.py").is_file():
-        print(f"oracle/make_ref.py: no reference checkout at {SRC}; keeping whatever oracle/_ref already holds")
+    try:
+        present = (SRC / "models" / "fatchord_version.py").is_file()
+    except OSError:                       # e.g. a checkout under a directory this user may not enter
+        present = False
+    if not present:
+        print(f"oracle/make_ref.py: no readable reference checkout at {SRC}; keeping whatever oracle/_ref already holds")
         return 0
     manifest = {}
     for rel in FILES:

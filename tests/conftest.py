@@ -11,7 +11,7 @@ os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_100a) device; run on the GPU box with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_90a) device; select with -m gpu")
 
 
 @pytest.fixture(scope="session")

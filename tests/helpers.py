@@ -72,6 +72,11 @@ def first_exceed(diff, thr):
     return int(np.argmax(bad)) if bad.any() else None
 
 
+def sample_index(n, k, seed):
+    """Fixed, seeded sample of min(n, k) indices into a flattened array (the reference pins store values only)."""
+    return np.sort(np.random.RandomState(seed).choice(n, min(n, k), replace=False))
+
+
 def load_golden(name):
     return np.load(GOLDEN / name, allow_pickle=False)
 

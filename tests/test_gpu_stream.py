@@ -1,7 +1,7 @@
 """The STREAM engine (wavernn_b200/csrc/wrnn_stream.cu: activation-stationary, weights streamed from L2, one independent
 CTA per 16/32 folds) through the C ABI, against the engine-arithmetic emulation, the reference fixtures and the
 persistent tcgen05 engine.  Its packing and step program are checked on the CPU (tests/test_stream_plan.py); this file
-covers what only hardware can: descriptors, TMEM, the mbarrier protocol, the ring.  Run on the GPU box: pytest -m gpu."""
+covers what only hardware can: descriptors, wgmma fragments, the mbarrier protocol, the ring.  Run on a GPU: pytest -m gpu."""
 import numpy as np
 import pytest
 import torch
@@ -63,7 +63,7 @@ def test_stream_engine_tiles_of_16_ragged_and_zero_padded_tail(n_seg):
 
 
 def test_stream_engine_tiles_of_32_and_auto_selection():
-    """More folds than 16 x 148: tiles of 32 folds (the other instantiation).  ENGINE_AUTO must route the job to the
+    """More folds than 16 per SM: tiles of 32 folds (the other instantiation).  ENGINE_AUTO must route the job to the
     stream engine, and every tile must equal the same folds generated on their own (fold-keyed Philox)."""
     model = helpers.make_model(0, "MOL", "cuda")
     w = O.hot_weights(helpers.state_numpy(model))

@@ -67,7 +67,7 @@ def test_trained_free_running_prefix_and_statistics(trained, taco):
     first2 = [helpers.first_exceed(d[i], 1e-2) for i in range(4)]
     print(f"{name} trained free run: first step off by 1e-3 per fold {first3}, by 1e-2 {first2}")
     # chaotic system: WHERE a fold leaves the reference depends on the accumulation order (CPU emulation of the same
-    # contract: [1618, 511, 180, never]; B200 round 2: [3541, 965, 42, 3138]), so the bound is on the ensemble
+    # contract: [1618, 511, 180, never]; one engine build: [3541, 965, 42, 3138]), so the bound is on the ensemble
     big = 12100
     assert d[:, :25].max() <= 1e-3
     assert np.median([big if f is None else f for f in first3]) >= 300

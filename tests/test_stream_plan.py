@@ -3,7 +3,7 @@ WITHOUT a GPU: the library exports the plan for host-resident weights (wrnn_debu
 with numpy exactly the way the kernel's issuer / epilogue warps do -- chunk by chunk, accumulator by accumulator,
 the h1 ping-pong buffers, in-place h2, the barrier fields as ordering assertions -- and compares samples and logits with
 the engine-arithmetic emulation oracle/contract.py (which tests/test_contract.py pins to the fp32 oracle, which
-tests/test_oracle_golden.py pins to the reference's fixtures).  What remains GPU-only is the PTX (descriptors, TMEM,
+tests/test_oracle_golden.py pins to the reference's fixtures).  What remains GPU-only is the PTX (descriptors, wgmma,
 mbarriers), covered by tests/test_gpu_stream.py."""
 import ctypes as C
 
@@ -482,25 +482,3 @@ def test_cluster_form_exchange_protocol_under_adversarial_schedules():
             simulate_cluster(plans, m_up, aux, U, pick=schedules[name], h2_in_place=True, **kw)
     print(f"{len(schedules)} schedules: identical to the one-CTA program; vs contract {np.abs(ref_out[:, :steps] - emu[:, :steps]).max():.2e}")
     assert np.abs(ref_lg[:steps] - lemu[:steps]).max() <= 1e-3
-
-
-@pytest.mark.skipif(not cabi.is_built(), reason="library not built")
-def test_one_cta_form_in_place_updates_are_separated_from_their_last_readers_by_more_than_the_ring():
-    """One-CTA form: h2 is updated IN PLACE and y1 goes over the previous h1 -- by epilogues that run while issuing warps
-    other than the committing ones may still be working.  What makes that safe is the in-order ring: the block-full commit
-    that releases an epilogue sits at ring position p_full; a chunk at position p <= p_full - STAGES has released its slot
-    -- its MMAs have COMPLETED -- before the chunk at p_full could even be loaded.  So every reader of the old content must
-    precede the overwriting block's last commit by more than the deepest ring the kernel can be built with (MAX_STAGES = 9
-    slots; the one-CTA layouts have 3 and 5)."""
-    sd = helpers.state_numpy(helpers.make_model(0, "MOL"))
-    _, prog, _ = get_plan(sd)
-    pair = np.arange(len(prog)) // 2
-    last_commit = {}
-    for i, c in enumerate(prog):
-        if c["commit"]:
-            last_commit[(int(c["phase"]), int(c["commit"]) - 1)] = i
-    MAX_STAGES = 9
-    h2 = [pair[last_commit[(1, int(c["k0"]) // 128)]] - pair[i] for i, c in enumerate(prog) if int(c["phase"]) == 1 and int(c["b_buf"]) == B_H2]
-    y1 = [pair[last_commit[(2, int(c["k0"]) // 128)]] - pair[i] for i, c in enumerate(prog) if int(c["phase"]) == 0 and int(c["b_buf"]) == B_H1PREV]
-    print("ring positions between the last reader of the old content and the block-full that lets it be overwritten: h2", min(h2), " y1 over h1", min(y1))
-    assert len(h2) == 3 * 4 * 8 and min(h2) > MAX_STAGES and min(y1) > MAX_STAGES

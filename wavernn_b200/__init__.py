@@ -1,4 +1,4 @@
-"""wavernn_b200 -- Blackwell (sm_100a) native WaveRNN batched vocoder.
+"""wavernn_b200 -- Hopper (sm_90a) native WaveRNN batched vocoder.
 
 One hot path, behind the reference's own Python surface:
 

@@ -50,9 +50,9 @@ int wrnn_create(wrnn_t** out, const wrnn_cfg* cfg, const wrnn_weights* w, int de
   WRNN_CUDA_OK(cudaSetDevice(device));
   cudaDeviceProp prop;
   WRNN_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10 || prop.minor != 0) {        // only an sm_100a cubin is built: sm_101 / sm_103 would fail at launch
+  if (prop.major != 9 || prop.minor != 0) {         // only an sm_90a cubin is built (wgmma and TMA of Hopper)
     set_error(std::string("device '") + prop.name + "' is sm_" + std::to_string(prop.major * 10 + prop.minor) +
-              "; this library is built for sm_100a only");
+              "; this library is built for sm_90a only");
     return WRNN_E_NO_DEVICE;
   }
   HostWeights hw;
@@ -99,11 +99,11 @@ int wrnn_create(wrnn_t** out, const wrnn_cfg* cfg, const wrnn_weights* w, int de
 }
 
 // Folds from which ENGINE_AUTO hands a job to the stream engine: the persistent engine serves tiles of 64 folds one
-// after the other at 15.5 us per step each; the stream engine's cluster form serves up to 33 x 16 folds at once at
-// 24.9 us per step (33 x 32 at 37 us, then the one-CTA forms: 66 us for up to 148 x 16, 94 us per 148 x 32;
-// profiles/r02_stream.md): from the second tile on the stream engine is faster (cfg4, 104 folds: 3.71 vs 3.20 M samples/s).  WRNN_STREAM_MIN_FOLDS overrides (experiments).
+// after the other, the stream engine all tiles at once.  Measured on an H100 SXM (400 W limit), end to end: a persistent
+// tile costs ~15.5 us per step, the stream engine's cluster form ~64 us per step for up to a few hundred folds, so the
+// stream engine wins from the fifth tile on.  WRNN_STREAM_MIN_FOLDS overrides (experiments).
 static int stream_min_folds() {
-  static const int v = [] { const char* e = getenv("WRNN_STREAM_MIN_FOLDS"); return e ? atoi(e) : 65; }();
+  static const int v = [] { const char* e = getenv("WRNN_STREAM_MIN_FOLDS"); return e ? atoi(e) : 4 * 64 + 1; }();
   return v;
 }
 

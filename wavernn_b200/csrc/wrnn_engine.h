@@ -20,6 +20,15 @@ void set_error(const std::string& msg);          // thread-local last error (wrn
     }                                                                                         \
   } while (0)
 
+// Grid of a grid-stride kernel: `blocks`, capped at 8 blocks per SM of the current device.
+inline int grid_stride_blocks(long long blocks) {
+  int dev = 0, n_sm = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+  const long long cap = 8ll * (n_sm > 0 ? n_sm : 1);
+  return (int)(blocks < cap ? blocks : cap);
+}
+
 class Engine {
  public:
   virtual ~Engine() {}
@@ -35,7 +44,7 @@ class Engine {
 
 // SIMT engine: CUDA-core FMA contractions, fp32-strict or bf16-operand arithmetic.
 int make_simt_engine(const wrnn_cfg& cfg, const HostWeights& w, int device, Engine** out);
-// tcgen05 engine: 5th-gen tensor-core contractions with TMEM accumulators (bf16 operands).
+// persistent tensor-core engine (wrnn_tc.cu): weights stationary in 128 SMs, wgmma contractions (fp16 / bf16 operands).
 int make_tc_engine(const wrnn_cfg& cfg, const HostWeights& w, int device, Engine** out);
 // stream engine (wrnn_stream.cu): activation-stationary, weights streamed from L2; the throughput form for many folds
 int make_stream_engine(const wrnn_cfg& cfg, const HostWeights& w, int device, Engine** out);

@@ -69,7 +69,7 @@ extern "C" int wrnn_epilogue(const float* samples, int32_t n_seg, int32_t seg_le
   if (mu_table && n_classes < 2) { set_error("wrnn_epilogue: n_classes"); return WRNN_E_INVALID; }
   EpParams p{samples, n_seg, seg_len, seg_stride, overlap, fade_in, fade_out, mu_table, n_classes, tail, tail_len, wave_len, wav};
   const long long blocks = (wave_len + 255) / 256;
-  const int grid = (int)(blocks < 148 * 8 ? blocks : 148 * 8);
+  const int grid = grid_stride_blocks(blocks);
   wrnn_epilogue_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
   WRNN_CUDA_OK(cudaGetLastError());
   return WRNN_OK;

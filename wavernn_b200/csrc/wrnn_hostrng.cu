@@ -4,7 +4,7 @@
 // generate() call (fatchord_version.py:178-179 -> :266-271; reset_parameters() draws one uniform per parameter
 // element, 3.2 M values that are thrown away) and then 11 uniforms per fold and step inside the loop
 // (utils/distribution.py:106,118).  Reproducing that stream with torch operators costs ~30 ms of single-thread CPU
-// time per call -- a fifth of the whole B200 job.  Here the discarded part is skipped with bare state twists (no
+// time per call -- a large share of the whole GPU job.  Here the discarded part is skipped with bare state twists (no
 // tempering, no stores) and the used part is written straight into the caller's (pinned) staging buffer.
 //
 // The caller (wavernn_b200/vocoder.py) reads / writes the generator state through torch.get_rng_state() /
@@ -54,7 +54,7 @@ inline uint32_t temper(uint32_t y) {
   return y;
 }
 
-// One body, two instantiations: with the FMA unit (every x86-64 host a B200 sits in) the conversion is one
+// One body, two instantiations: with the FMA unit (every x86-64 host an H100 sits in) the conversion is one
 // instruction per draw; otherwise libm's correctly rounded fmaf gives the same bits.
 template <bool HW>
 inline __attribute__((always_inline)) void convert_body(const uint32_t* s, float* o, uint64_t take, float range, float lo) {

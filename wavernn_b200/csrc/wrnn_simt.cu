@@ -6,7 +6,7 @@
 // re-association error (weights, activations and accumulation all fp32), which proves the
 // folded algebra (wrnn_fold.h), the exchange protocol, the fold indexing and the samplers
 // independently of tensor-core rounding; in BF16 mode it applies exactly the rounding
-// contract of the tcgen05 engine (operands rounded to bf16, fp32 accumulate).
+// contract of the tensor-core engines (operands rounded to bf16, fp32 accumulate).
 //
 // Decomposition: P = 128 CTAs; CTA c owns hidden units [4c, 4c+4) of every layer and keeps
 // its slice of all matrices resident in shared memory for the whole launch.  Per step the

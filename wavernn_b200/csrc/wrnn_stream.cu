@@ -8,28 +8,25 @@
 // TMA bulk copies -- no inter-SM synchronisation at all, one independent CTA per fold tile, any number of tiles.
 // The step is the static program of wrnn_stream_plan.h (chunk list with accumulator / operand / barrier fields).
 //
-// Swap-AB tcgen05: D[128 weight rows, NF folds] (+)= W[128, 16] * act[NF, 16]^T, kind::f16, fp32 accumulators in
-// TMEM (16 accumulators of NF columns).  TMEM lane == weight row == hidden unit, so the r / z / n pre-activations of a
-// unit are in the same lane of different accumulators and the gate math is thread-local: thread u of the four
-// epilogue warps owns unit 128 b + u of block b for all NF folds.  The fp32 hidden state lives in L2-resident global
-// scratch ([2][512][NF] per tile); the fp16 operand images of h1', h2', y1, y2 live in shared memory.
+// Swap-AB wgmma: D[128 weight rows, NF folds] (+)= W[128, 16] * act[NF, 16]^T, fp32 accumulators in registers.  Two
+// consumer warpgroups split every 128-row chunk (rows 0-63 / 64-127) and walk the program grouped by (phase, unit
+// block): each holds the four accumulators of the current group (r / z / in / hn of a GRU block, or the four K
+// partials of an fc block) and runs the group's epilogue itself when its last chunk is done.  The r / z / n
+// pre-activations of a unit sit in the same fragment position of different accumulators, so the gate math is
+// thread-local.  The fp32 hidden state lives in L2-resident global scratch ([2][512][NF] per tile); the fp16 operand
+// images of h1', h2', y1, y2 live in shared memory.
 //
-// Warp roles (320 threads, no CTA-wide barrier inside the loop):
-//   warp 0     producer : walks the chunk list, one cp.async.bulk per chunk into the ring (full/empty mbarriers)
-//   warps 1-4  issuers  : every accumulator chain belongs to one of them (GRU phases: r / z / in / hn; fc phases: a K
-//                         quarter into a partial accumulator).  Each walks its own chunk list: waits for operands /
-//                         accumulators / its ring slots, issues the MMAs, commits slot-empty, block-full and cond-free
-//                         with tcgen05.commit.  One warp alone sustains ~1 MMA per 100 cycles (measured, r02 first
-//                         version: 214 us per step); the tensor pipe wants one per ~40.
-//   warp 5     staging  : conditioning row of step t+1 for the NF folds (stream or frame-rate form) -> fp16 image
-//   warps 6-9  epilogue : TMEM -> registers, gates / relu / MoL sampler (SFU), state, operand images, output
+// Warp roles (320 threads):
+//   warps 0-7  consumers : two warpgroups; per chunk: operand readiness, ring slot, wgmma, slot release; epilogues
+//   warp 8     producer  : walks the chunk list, one cp.async.bulk per chunk into the ring (full/empty mbarriers)
+//   warp 9     staging   : conditioning row of step t+1 for the NF folds (stream or frame-rate form) -> fp16 image
 //
-// Cluster form (template CL = 4; jobs of <= 33 tiles): a tile belongs to a thread-block cluster of four CTAs.  CTA r runs
-// the program of unit block r of every layer (a quarter of the weight stream and of the MMAs; fc3 + sampling in rank 0,
-// which hands the sample to its peers), keeps all four K = 512 operand images, and pushes the block it has just computed
-// into the peers' images with cp.async.bulk.shared::cluster.shared::cta (complete_tx on the PEER's readiness barrier,
-// arrive.expect_tx by the sender), so that a peer's block arrives exactly like a TMA load.  Same MMAs in the same order:
-// results are bit-identical to the one-CTA form.
+// Cluster form (template CL = 4; jobs whose clusters are co-resident): a tile belongs to a thread-block cluster of four
+// CTAs.  CTA r runs the program of unit block r of every layer (a quarter of the weight stream and of the MMAs; fc3 +
+// sampling in rank 0, which hands the sample to its peers), keeps all four K = 512 operand images, and pushes the block
+// it has just computed into the peers' images with cp.async.bulk.shared::cluster.shared::cta (complete_tx on the PEER's
+// readiness barrier, arrive.expect_tx by the sender), so that a peer's block arrives exactly like a TMA load.  Same MMAs
+// in the same order: results are bit-identical to the one-CTA form.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -49,51 +46,45 @@ using namespace tc;
 using namespace stream;
 
 constexpr int NT = 320;
-constexpr int EPI_WARP0 = 6, EPI_TID0 = EPI_WARP0 * 32;     // first epilogue warp / thread
+constexpr int N_CONSUMERS = 256;             // warps 0-7
+constexpr int PRODUCER_WARP = 8, STAGING_WARP = 9;
 constexpr int KQ = CDIM / 8;                 // 26 16-byte chunks per conditioning row
 constexpr int SBO_Q = KQ * 128;              // 3328: stride between 8-fold groups of the conditioning image
 constexpr int SBO_H = (H / 8) * 128;         // 8192: same for the K = 512 images
-constexpr int TMEM_COLS = 512;
 constexpr int NBAR = 48;
-constexpr int MAX_STAGES = 9;               // ring slots (one or two chunks each)
+constexpr int MAX_STAGES = 9;               // ring slots (one chunk each)
 
-template <int NF, int CL> struct Smem {
+template <int NF> struct Smem {
   static constexpr int GROUPS = NF / 8;
   static constexpr int ACT = GROUPS * SBO_H;                 // one K = 512 activation image
   static constexpr int COND = GROUPS * SBO_Q;                // one conditioning image
-  // Three K = 512 operand images: X0 / X1 = h1 ping-pong (this step's h1 is X[cur], h1' goes to X[cur^1]); y1 and then y2
-  // reuse X[cur] once its readers are done (y2 is written only after ALL fc2 MMAs have completed); h2 is updated in place.
-  // Cluster form (CL = 4, rows of every layer split over four CTAs that push their blocks into each other's images): h2 ping-pongs
-  // too (H0 / H1; a peer cannot know when this CTA's W2h MMAs are done), y1 -> X[cur], y2 -> H[cur], nothing deferred.
-  static constexpr int OFF_X0 = 0, OFF_X1 = ACT, OFF_H2 = 2 * ACT, OFF_H2B = (CL == 1) ? 2 * ACT : 3 * ACT;
-  static constexpr int OFF_COND = (CL == 1 ? 3 : 4) * ACT;   // two conditioning images (double buffer)
+  // Four K = 512 operand images: X0 / X1 = h1 ping-pong (this step's h1 is X[cur], h1' goes to X[cur^1]), H0 / H1 = h2
+  // ping-pong likewise; y1 goes to X[cur] and y2 to H[cur] once their old contents have been read.
+  static constexpr int OFF_X0 = 0, OFF_X1 = ACT, OFF_H2 = 2 * ACT, OFF_H2B = 3 * ACT;
+  static constexpr int OFF_COND = 4 * ACT;                   // two conditioning images (double buffer)
   static constexpr int OFF_RING = (OFF_COND + 2 * COND + 1023) / 1024 * 1024;
-  // chunks per ring slot / TMA / full-empty barrier pair.  Two is better for both layouts (measured at NF = 32, 96 KB of
-  // ring: three 32 KB slots 95 us per step, six 16 KB slots 107 us -- the hand-shakes cost more than the coarser refill)
-  static constexpr int CPS = (CL == 1) ? 2 : 1;          // (one-block programs have odd chunk groups: one chunk per slot)
-  static constexpr int SLOT_BYTES = CPS * CHUNK_BYTES;
+  static constexpr int SLOT_BYTES = CHUNK_BYTES;
   static constexpr int LOGP = 33;                                            // padded row of the logits transpose (conflict-free both ways)
-  static constexpr int MISC = LOGP * NF * 4 + NF * 4 + NBAR * 8 + 64;        // logits transpose, x, barriers, tmem slot
+  static constexpr int MISC = LOGP * NF * 4 + NF * 4 + NBAR * 8 + 64 + 256;  // logits transpose, x, barriers, flags, zero block
   static constexpr int STAGES = (227 * 1024 - OFF_RING - MISC) / SLOT_BYTES > MAX_STAGES ? MAX_STAGES : (227 * 1024 - OFF_RING - MISC) / SLOT_BYTES;
   static constexpr int OFF_LOG = OFF_RING + STAGES * SLOT_BYTES;             // [NF][LOGP] fp32
   static constexpr int OFF_XS = OFF_LOG + LOGP * NF * 4;                       // [NF] fp32: previous sample per fold
   static constexpr int OFF_BAR = OFF_XS + NF * 4;
-  static constexpr int BYTES = OFF_BAR + NBAR * 8 + 64;
+  static constexpr int OFF_ZERO = OFF_BAR + NBAR * 8 + 64;                  // 256 B of zeros: B operand of padding MMAs
+  static constexpr int BYTES = OFF_ZERO + 256;
   static_assert(STAGES >= 3, "ring too shallow");
   static_assert(BYTES <= 227 * 1024, "shared memory budget");
 };
 // barrier indices
-constexpr int BAR_FULL = 0, BAR_EMPTY = MAX_STAGES, BAR_ACC_FULL = 2 * MAX_STAGES, BAR_ACC_EMPTY = BAR_ACC_FULL + 4,
-              BAR_READY = BAR_ACC_EMPTY + 4 /* + {0, 1: cond[parity]; 2..5: h1' block b; 6..9: h2' block b; 10..13: y1 block b; 14..17: y2 block b} */,
+constexpr int BAR_FULL = 0, BAR_EMPTY = MAX_STAGES,
+              BAR_READY = 2 * MAX_STAGES /* + {0, 1: cond[parity]; 2..5: h1' block b; 6..9: h2' block b; 10..13: y1 block b; 14..17: y2 block b} */,
               BAR_COND_FREE = BAR_READY + 18;
 constexpr int BAR_X = BAR_COND_FREE + 2;    // cluster form: "the sample of this step has been written into this CTA's x_s"
 static_assert(BAR_X + 1 <= NBAR, "barrier table");
 
 struct StreamParams {
-  // per cluster rank (one-CTA form: rank 0 only): the weight stream, the TMA size (>> 4) of each ring-slot load, loads per step,
-  // and per issuing warp its DevChunk records
-  const unsigned char* blob[4]; const unsigned short* slot_size16[4]; int n_slots[4];
-  const uint4* mine[4 * N_ISSUERS]; int n_mine[4 * N_ISSUERS];
+  // per cluster rank (one-CTA form: rank 0 only): the weight stream and the chunk list of one step
+  const unsigned char* blob[4]; const uint4* prog[4]; int n_prog[4];
   const float* qk; const float* vq; const float* b1h; const float* b2h; const float* b3;
   const float* mels_up; const float* aux; long long L; long long seg_stride; long long row_base;
   int n_total, steps, out_pitch, seg_first;
@@ -116,12 +107,10 @@ __device__ __forceinline__ uint32_t map_to_rank(uint32_t addr, uint32_t rank) {
 
 template <int NF, int FMT, bool FRAMES, bool PROF, int CL>
 __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p) {
-  using SM = Smem<NF, CL>;
+  using SM = Smem<NF>;
   extern __shared__ __align__(1024) unsigned char smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM::OFF_BAR);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SM::OFF_BAR + NBAR * 8);
   volatile int* s_abort = reinterpret_cast<volatile int*>(smem + SM::OFF_BAR + NBAR * 8 + 16);   // CTA-local copy of the abort flag
-  volatile unsigned* issued_s = reinterpret_cast<volatile unsigned*>(smem + SM::OFF_BAR + NBAR * 8 + 32);   // chunk PAIRS the producer has issued
   float* x_s = reinterpret_cast<float*>(smem + SM::OFF_XS);
   float* log_s = reinterpret_cast<float*>(smem + SM::OFF_LOG);
   auto bar = [&](int i) -> uint32_t { return smem_u32(&bars[i]); };
@@ -131,43 +120,36 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
   const int tile = blockIdx.x / CL, f0 = tile * NF;
   const int B = (p.n_total - f0 < NF) ? (p.n_total - f0) : NF;          // real folds of this tile
   const int S = p.steps;
+  const uint4* prog = p.prog[rank];
+  const int n_prog = p.n_prog[rank];
 
   // ---- setup ----------------------------------------------------------------------------------------------------
   {
     int4* z = reinterpret_cast<int4*>(smem);
-    for (int i = tid; i < SM::OFF_RING / 16; i += NT) z[i] = make_int4(0, 0, 0, 0);       // all operand images start as zeros
+    // operand images start as zeros; the ring too, so that the padding MMAs of a K = 16 chunk (ring bytes x 0) add exact zeros
+    for (int i = tid; i < SM::OFF_LOG / 16; i += NT) z[i] = make_int4(0, 0, 0, 0);
+    for (int i = tid; i < 256 / 16; i += NT) z[SM::OFF_ZERO / 16 + i] = make_int4(0, 0, 0, 0);
     if (tid < NF) x_s[tid] = 0.f;
-    if (tid == 0) { *s_abort = 0; *issued_s = 0; }
+    if (tid == 0) *s_abort = 0;
   }
   if (tid == 0) {
     for (int i = 0; i < SM::STAGES; ++i) {
       asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar(BAR_FULL + i)));
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar(BAR_EMPTY + i)));            // one commit by the pair's issuer
-    }
-    for (int i = 0; i < 4; ++i) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar(BAR_ACC_FULL + i)), "n"(N_ISSUERS));   // one commit per issuing warp
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 128;" :: "r"(bar(BAR_ACC_EMPTY + i)));
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], 8;" :: "r"(bar(BAR_EMPTY + i)));            // one arrival per consumer warp
     }
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 32;" :: "r"(bar(BAR_READY + 0)));
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 32;" :: "r"(bar(BAR_READY + 1)));
-    // operand blocks: written here by the 128 epilogue threads (one arrival each), or -- cluster form, a peer's block --
+    // operand blocks: written here by the 256 consumer threads (one arrival each), or -- cluster form, a peer's block --
     // delivered by the peer's bulk copies (one arrive.expect_tx by the sender + the bytes)
     for (int i = 2; i < 18; ++i)
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar(BAR_READY + i)), "r"((CL == 1 || ((i - 2) & 3) == rank) ? 128 : 1));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar(BAR_COND_FREE + 0)), "n"(N_ISSUERS));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar(BAR_COND_FREE + 1)), "n"(N_ISSUERS));
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar(BAR_READY + i)), "r"((CL == 1 || ((i - 2) & 3) == rank) ? N_CONSUMERS : 1));
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 8;" :: "r"(bar(BAR_COND_FREE + 0)));
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 8;" :: "r"(bar(BAR_COND_FREE + 1)));
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar(BAR_X)));
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(tmem_slot)), "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   proxy_fence_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   if constexpr (CL > 1) cluster_sync_all();                  // every peer's barriers and zeroed images exist before anyone writes into them
   // Bounded wait (a protocol bug must end in WRNN_E_WATCHDOG, never in a hung GPU): once any wait of this CTA has given
   // up, or another CTA has raised the global flag, every later wait returns at once and the role loops end.
@@ -207,137 +189,23 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
     }
   };
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ===================================================================================================== producer
-    // one TMA (and one full / empty barrier) per ring slot = CPS consecutive chunks
-    unsigned g = 0;                                           // slot loads issued so far (ring position)
+    // one TMA (and one full / empty barrier) per chunk, in the order the consumers take them
+    unsigned g = 0;                                           // chunk loads issued so far (ring position)
     for (int t = 0; t < S && !*s_abort; ++t) {
-      size_t off = 0;
-      const unsigned short* sizes = p.slot_size16[rank];
-      const int n_slots = p.n_slots[rank];
-      uint32_t sz = __ldg(sizes);
-      for (int c = 0; c < n_slots; ++c, ++g) {
-        const uint32_t bytes = sz * 16u;
-        if (c + 1 < n_slots) sz = __ldg(sizes + c + 1);
+      for (int c = 0; c < n_prog; ++c) {
+        const uint4 r = __ldg(prog + c);
+        const uint32_t flags = (r.z >> 8) & 0xffu;
+        if (flags & DF_SAME_SLOT) continue;                   // operand of the previous record's chunk
+        const uint32_t bytes = (flags & DF_NK1) ? (uint32_t)(CHUNK_BYTES / 4) : (uint32_t)CHUNK_BYTES;
         const int slot = g % SM::STAGES;
-        wait(bar(BAR_EMPTY + slot), ((g / SM::STAGES) & 1) ^ 1);      // slot drained by the MMAs of its chunk(s)
-        tma_bulk_g2s(smem_u32(smem + SM::OFF_RING + slot * SM::SLOT_BYTES), p.blob[rank] + off, bytes, bar(BAR_FULL + slot));
-        __syncwarp();
-        if (lane == 0) *issued_s = g + 1;                      // see the issuers: parity waits need "this phase is armed"
-        off += bytes;
+        wait(bar(BAR_EMPTY + slot), ((g / SM::STAGES) & 1) ^ 1);      // slot drained by the MMAs of its chunk
+        tma_bulk_g2s(smem_u32(smem + SM::OFF_RING + slot * SM::SLOT_BYTES), p.blob[rank] + (size_t)r.x * 16, bytes, bar(BAR_FULL + slot));
+        ++g;
       }
     }
-  } else if (warp <= N_ISSUERS) {
-    // ====================================================================================================== issuers
-    // Lean by construction: the records are pre-digested (wrnn_stream_plan.h::DevChunk), a pair of chunks (eight MMAs)
-    // costs one ring hand-shake, and the four MMAs of a chunk go out under one elect.  (First multi-warp version: ~1800
-    // cycles per chunk, two thirds of it plain instruction issue -- ncu source view, profiles/r02_stream.md.)
-    const int q = warp - 1;
-    const uint32_t idesc = umma_idesc(MROWS, NF, FMT);
-    const uint4* my = p.mine[rank * N_ISSUERS + q];
-    const int n_my = p.n_mine[rank * N_ISSUERS + q];
-    const bool profiling = PROF && blockIdx.x == 0 && q == 0;
-    long long t_ring = 0, t_b = 0, t_acc = 0, t_issue = 0;
-    constexpr uint32_t LBO = (128u >> 4) << 16, VER = 1u << 14;       // descriptor: LBO field (low word), version bit (high word)
-    constexpr uint32_t HI_A4 = (1024u >> 4) | VER, HI_A1 = (256u >> 4) | VER, HI_BH = ((uint32_t)SBO_H >> 4) | VER, HI_BQ = ((uint32_t)SBO_Q >> 4) | VER;
-    const uint32_t s0_lo = smem_u32(smem) >> 4, ring_lo = smem_u32(smem + SM::OFF_RING) >> 4;
-    unsigned issued_seen = 0;
-    // four (or one) MMAs of one chunk: D[tmem] (+)= A[ring] * B[image]^T, K advancing by 16 (+16 in the address field)
-    auto mma4 = [&](uint32_t d_col, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t acc_first, bool one) {
-      if (one) {
-        asm volatile("{\n\t.reg .pred e, p;\n\t.reg .b64 da, db;\n\t"
-                     "elect.sync _|e, 0xffffffff;\n\tsetp.ne.b32 p, %6, 0;\n\t"
-                     "mov.b64 da, {%1, %2};\n\tmov.b64 db, {%3, %4};\n\t"
-                     "@e tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}\n"
-                     :: "r"(d_col), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(acc_first) : "memory");
-      } else {
-        asm volatile("{\n\t.reg .pred e, p, pt;\n\t.reg .b64 da, db;\n\t.reg .b32 al, bl;\n\t"
-                     "elect.sync _|e, 0xffffffff;\n\tsetp.ne.b32 p, %6, 0;\n\tsetp.eq.b32 pt, %6, %6;\n\t"
-                     "mov.b64 da, {%1, %2};\n\tmov.b64 db, {%3, %4};\n\t"
-                     "@e tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t"
-                     "add.u32 al, %1, 16;\n\tadd.u32 bl, %3, 16;\n\tmov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-                     "@e tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, pt;\n\t"
-                     "add.u32 al, %1, 32;\n\tadd.u32 bl, %3, 32;\n\tmov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-                     "@e tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, pt;\n\t"
-                     "add.u32 al, %1, 48;\n\tadd.u32 bl, %3, 48;\n\tmov.b64 da, {al, %2};\n\tmov.b64 db, {bl, %4};\n\t"
-                     "@e tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, pt;\n\t}\n"
-                     :: "r"(d_col), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(acc_first) : "memory");
-      }
-    };
-    for (int t = 0; t < S && !*s_abort; ++t) {
-      const int cur = t & 1;
-      const unsigned gbase = (unsigned)t * (unsigned)p.n_slots[rank];   // ring position of this step's first slot load
-      uint4 nx0 = __ldg(my), nx1 = __ldg(my + 1);
-      for (int i = 0; i < n_my; i += 2) {
-        const uint4 rec[2] = {nx0, nx1};
-        if (i + 2 < n_my) { nx0 = __ldg(my + i + 2); nx1 = __ldg(my + i + 3); }      // next pair's records: plain sequential loads
-        unsigned g = 0; int slot = 0; uint32_t slot_lo = 0;
-#pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const uint4 r = rec[j];
-          if (j == 0 || SM::CPS == 1) {                         // ring slot of this chunk (CPS == 2: of the pair)
-            g = gbase + (r.w >> 16);
-            slot = g % SM::STAGES;
-            slot_lo = ring_lo + (uint32_t)slot * (SM::SLOT_BYTES >> 4);
-          }
-          const uint32_t flags = r.z >> 24, acc = (r.z >> 16) & 0xf, phase = (r.z >> 20) & 0xf;
-          const uint32_t wait_b = r.w & 7u, wait_acc = (r.w >> 3) & 7u, commit = (r.w >> 6) & 7u, wait_blk = (r.w >> 9) & 3u;
-          long long c0 = 0, c1 = 0, c2 = 0, c3 = 0;
-          if (profiling) c0 = clock64();
-          if (wait_acc) {
-            // the epilogue of the previous (phase, block) use must have drained the block: its arrivals on acc_empty[blk] are
-            // numbered A*t + phase (A = 5 for block 0, which also serves fc3; 4 otherwise); we need number A*t + phase - 1
-            // (cluster form: one accumulator set per phase, drained once per step; set 0 also serves fc3 in rank 0)
-            const int blk = wait_acc - 1;
-            const int idx = (CL == 1) ? ((blk == 0 ? N_PHASES : N_PHASES - 1) * t + (int)phase - 1)
-                                      : ((blk == 0 && rank == 0) ? (2 * t + (phase == 4u ? 0 : -1)) : (t - 1));
-            if (idx >= 0) wait(bar(BAR_ACC_EMPTY + blk), (uint32_t)idx & 1u);
-          }
-          if (profiling) c1 = clock64();
-          if (wait_b == W_COND) wait(bar(BAR_READY + cur), (uint32_t)(t >> 1) & 1);
-          else if (wait_b != W_NONE) {
-            // the block this K range reads: written here through the generic proxy (fenced by its writers), or a peer's
-            // block that arrived by bulk copy (async proxy, complete_tx on this barrier) -- like a TMA load, no fence
-            // (so the plain CTA-scope wait: an acquire.cluster poll costs an L1 invalidate -- CCTL.IVALL -- per iteration)
-            wait(bar(BAR_READY + 2 + (wait_b - W_H1NEW) * 4 + wait_blk), (uint32_t)t & 1);
-          }
-          if (profiling) c2 = clock64();
-          if (j == 0 || SM::CPS == 1) {
-            // The ring is filled in stream order but drained by four warps: this warp may get here while the slot still
-            // holds (or waits for) the pair STAGES positions earlier, owned by another warp -- a parity wait would then
-            // alias "previous phase" with "this phase".  The producer publishes how many pairs it has issued; once ours
-            // is issued the slot's barrier is in OUR phase and the parity wait is exact.
-            if (issued_seen <= g) {
-              const long long tw = clock64();
-              unsigned spins = 0;
-              while ((issued_seen = *issued_s) <= g) {
-                if ((++spins & 255u) == 0) {
-                  if (*s_abort) break;
-                  if (ld_relaxed_s32(p.abort_flag) != 0) { *s_abort = 1; break; }
-                  if (clock64() - tw > kWatchdogCycles) { atomicExch(p.abort_flag, 2); *s_abort = 1; break; }
-                }
-              }
-            }
-            wait(bar(BAR_FULL + slot), (g / SM::STAGES) & 1);
-            tc_fence_after();
-          }
-          if (profiling) c3 = clock64();
-          // (address field: 14 bits of byte address >> 4 -- masked, because in a cluster launch the shared::cta window of
-          //  ranks > 0 does not start at 0)
-          const uint32_t a_lo = ((slot_lo + (SM::CPS == 2 ? (r.x & 0xffffu) : 0u)) & 0x3fffu) | LBO, a_hi = (flags & DF_NK1) ? HI_A1 : HI_A4;
-          const uint32_t b_lo = ((s0_lo + (cur ? (r.y & 0xffffu) : (r.x >> 16))) & 0x3fffu) | LBO, b_hi = (flags & DF_B_COND) ? HI_BQ : HI_BH;
-          const uint32_t d_col = tmem + acc * NF;
-          mma4(d_col, a_lo, a_hi, b_lo, b_hi, (flags & DF_FIRST) ? 0u : 1u, (flags & DF_NK1) != 0);
-          if (flags & DF_HAS_B2) mma4(d_col, a_lo, a_hi, ((s0_lo + (cur ? (r.z & 0xffffu) : (r.y >> 16))) & 0x3fffu) | LBO, HI_BH, 1u, false);
-          if (commit) umma_commit(bar(BAR_ACC_FULL + commit - 1));
-          if (flags & DF_COND_RELEASE) umma_commit(bar(BAR_COND_FREE + cur));
-          if (j == 1 || SM::CPS == 1) umma_commit(bar(BAR_EMPTY + slot));
-          if (profiling) { const long long c4 = clock64(); t_acc += c1 - c0; t_b += c2 - c1; t_ring += c3 - c2; t_issue += c4 - c3; }
-        }
-      }
-    }
-    if (profiling && lane == 0) { p.prof[0] = t_acc; p.prof[1] = t_b; p.prof[2] = t_ring; p.prof[3] = t_issue; }
-  } else if (warp == N_ISSUERS + 1) {
+  } else if (warp == STAGING_WARP) {
     // ====================================================================================================== staging
     // cond_s (fp32 rows of the per-sample conditioning stream, or built from frame-rate tensors) -> fp16 image of step s,
     // one step ahead of the MMAs.  (fold, 8-column chunk) tasks, 32 threads.
@@ -350,7 +218,6 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
       const int par = s & 1;
       if (s >= 2) wait(bar(BAR_COND_FREE + par), (uint32_t)((s >> 1) - 1) & 1);   // step s-2 has consumed this buffer
       unsigned char* img = smem + SM::OFF_COND + par * SM::COND;
-      // a rolled loop on purpose: this warp shares its instruction caches with an issuing warp
 #pragma unroll 2
       for (int task = st; task < NF * KQ; task += 32) {
         const int f = task / KQ, c8 = task - f * KQ;
@@ -383,44 +250,38 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
         *reinterpret_cast<uint4*>(img + (f >> 3) * SBO_Q + c8 * 128 + (f & 7) * 16) = v;
       }
       proxy_fence_smem();                                      // generic-proxy stores -> async-proxy (MMA) reads
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(bar(BAR_READY + par)) : "memory");
+      mbar_arrive(bar(BAR_READY + par));
     }
-  } else {
-    // ===================================================================================================== epilogue
-    const int row = (warp & 3) * 32 + lane;                   // TMEM lane == weight row within the 128-row tile
-    const uint32_t tlane = tmem + ((uint32_t)((warp & 3) * 32) << 16);
+  } else if (warp < PRODUCER_WARP) {
+    // ===================================================================================================== consumers
+    const int wg = warp >> 2;                                  // rows [64 wg, 64 wg + 64) of every 128-row chunk
+    // this thread's fragment: rows rw and rw + 8 of the chunk, folds 8j + fc (+1), j < NF / 8
+    const int rw = 64 * wg + 16 * (warp & 3) + (lane >> 2), fc = 2 * (lane & 3);
     float* st_h1 = p.state + ((size_t)tile * 2 + 0) * H * NF;
     float* st_h2 = p.state + ((size_t)tile * 2 + 1) * H * NF;
-    unsigned full_par = 0;                                    // per block: parity of the accumulator-full waits so far
     unsigned rows_known = p.uniforms_ready ? 0u : 0xffffffffu;   // rows of p.uniforms known to have landed (streamed draws)
-    const bool profiling = PROF && blockIdx.x == 0 && tid == EPI_TID0;
-    long long t_wait = 0, t_work = 0;
-    auto wait_full = [&](int blk) {
-      long long c0 = 0;
-      if (profiling) c0 = clock64();
-      wait(bar(BAR_ACC_FULL + blk), (full_par >> blk) & 1u); full_par ^= 1u << blk;
-      tc_fence_after();
-      if (profiling) t_wait += clock64() - c0;
-    };
-    auto release_acc = [&](int blk) {                         // this thread's tcgen05.ld of the block are complete
-      tc_fence_before();
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(bar(BAR_ACC_EMPTY + blk)) : "memory");
-    };
-    // This thread's part of operand `kind`, unit block `blk` (GLOBAL block id) of the image at `off` is written.  Cluster
+    const bool profiling = PROF && blockIdx.x == 0 && tid == 0;
+    long long t_ring = 0, t_b = 0, t_issue = 0, t_epi = 0;
+    const uint32_t s0_lo = smem_u32(smem) >> 4, ring_lo = smem_u32(smem + SM::OFF_RING) >> 4;
+    constexpr uint64_t LBO = (uint64_t)(128u >> 4) << 16;
+    const uint64_t dz = (uint64_t)((smem_u32(smem + SM::OFF_ZERO) >> 4) & 0x3fffu) | LBO;     // zero block, SBO 0
+    unsigned g_next = 0;                                       // chunk loads consumed so far (ring position)
+    int slot = 0;
+    float d[NF / 2];                                           // the chain being accumulated
+    float acc[4][NF / 2];                                      // the finished chains of the current (phase, block)
+
+    // This CTA's part of operand `kind`, unit block `blk` (GLOBAL block id) of the image at `off` is written.  Cluster
     // form: the block is written LOCALLY like in the one-CTA form, then three elected threads (one per peer) push it into
     // the same place of the peers' images with bulk copies (shared::cta -> shared::cluster, NF/8 pieces of 2 KB: the 16
     // K-chunks of the block are contiguous within a fold group) that complete_tx on the peer's readiness barrier.
-    // (Round-2 measurement: 2-byte st.shared::cluster stores into four CTAs + cluster-scope fences cost ~6,000 cycles per
-    //  phase; y2 is only needed by rank 0, which owns fc3.)
     auto publish_ready = [&](int kind, int blk, int off) {
       const uint32_t b = bar(BAR_READY + 2 + (kind - W_H1NEW) * 4 + blk);
       proxy_fence_smem();
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(b) : "memory");
+      mbar_arrive(b);
       if constexpr (CL > 1) {
-        named_bar_sync(2, 128);                                // every epilogue thread's stores (and proxy fences) are done
-        const int q = warp & 3;
-        if (lane == 0 && q != 0) {
-          const uint32_t peer = (uint32_t)((rank + q) & 3);
+        named_bar_sync(2, N_CONSUMERS);                        // every consumer thread's stores (and proxy fences) are done
+        if (lane == 0 && warp >= 1 && warp <= 3) {
+          const uint32_t peer = (uint32_t)((rank + warp) & 3);
           if (kind != W_Y2 || peer == 0u) {
             const uint32_t rb = map_to_rank(b, peer);
             asm volatile("mbarrier.arrive.expect_tx.relaxed.cluster.shared::cluster.b64 _, [%0], %1;" :: "r"(rb), "r"((uint32_t)(NF * 256)) : "memory");
@@ -435,34 +296,28 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
       }
     };
     // element (fold f, unit k) of a K = 512 operand image
-    auto img_ptr = [&](int off, int f, int k) -> uint16_t* {
-      return reinterpret_cast<uint16_t*>(smem + off + (f >> 3) * SBO_H + (k >> 3) * 128 + (f & 7) * 16 + (k & 7) * 2);
+    auto img_store = [&](int off, int f, int k, float v) {
+      *reinterpret_cast<uint16_t*>(smem + off + (f >> 3) * SBO_H + (k >> 3) * 128 + (f & 7) * 16 + (k & 7) * 2) = (uint16_t)(pack2<FMT>(v, 0.f) & 0xffffu);
     };
-    auto img_store = [&](int off, int f, int k, uint16_t bits) { *img_ptr(off, f, k) = bits; };
-    constexpr int NBLK = (CL == 1) ? 4 : 1;                      // unit blocks this CTA computes: all four, or block `rank`
-    auto to_bits = [&](float v) -> uint16_t { return (uint16_t)(pack2<FMT>(v, 0.f) & 0xffffu); };
 
-    volatile int* ep_stop = s_abort + 1;                      // the epilogue warps leave the loop together (named barrier inside)
-    if (tid == EPI_TID0) *ep_stop = 0;
-    named_bar_sync(1, 128);
+    volatile int* ep_stop = s_abort + 1;                      // the consumers leave the loop together (named barriers inside)
+    if (tid == 0) *ep_stop = 0;
+    named_bar_sync(1, N_CONSUMERS);
     for (int t = 0; t < S; ++t) {
       const int cur = t & 1;
       const int off_h1new = cur ? SM::OFF_X0 : SM::OFF_X1, off_y1 = cur ? SM::OFF_X1 : SM::OFF_X0;
-      const int off_h2new = (CL == 1) ? SM::OFF_H2 : (cur ? SM::OFF_H2 : SM::OFF_H2B);        // in place, or H[cur^1]
-      const int off_y2 = (CL == 1) ? off_y1 : (cur ? SM::OFF_H2B : SM::OFF_H2);                 // over y1 (deferred), or H[cur]
-      long long w0 = 0;
-      if (profiling) w0 = clock64();
-      // draws of this step for the fold this thread samples (threads of lane quarter 0, lane < B)
+      const int off_h2new = cur ? SM::OFF_H2 : SM::OFF_H2B, off_y2 = cur ? SM::OFF_H2B : SM::OFF_H2;
+      // draws of this step for the fold this thread samples (rank 0, threads 0 .. B-1)
       float ur[11];
 #pragma unroll
       for (int i = 0; i < 11; ++i) ur[i] = 0.5f;
-      const bool sampler = rank == 0 && (warp & 3) == 0 && lane < B;
-      if (p.uniforms && rank == 0 && (warp & 3) == 0) {        // streamed draws: read row t once rows t .. t+3 have landed (see wrnn_tc.cu)
+      const bool sampler = rank == 0 && tid < B;
+      if (p.uniforms && rank == 0 && warp == 0) {              // streamed draws: read row t once rows t .. t+3 have landed (see wrnn_tc.cu)
         const unsigned need = min((unsigned)S, (unsigned)t + 4u);
         if (rows_known < need) rows_known = rows_wait(p.uniforms_ready, need, p.abort_flag);
       }
       if (sampler) {
-        const int gf = f0 + lane;
+        const int gf = f0 + tid;
         if (p.uniforms) {
           const float* u = p.uniforms + (size_t)t * 11 * p.n_total;
 #pragma unroll
@@ -478,219 +333,186 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
         }
       }
 
-      // ---- P1 / P2: the two GRU cells ----------------------------------------------------------------------------
-#pragma unroll 1
-      for (int cell = 0; cell < 2; ++cell) {
-        float* st = cell ? st_h2 : st_h1;
-        const float* bh = cell ? p.b2h : p.b1h;
-        const int qbase = cell * 3 * H;                        // rows of qk / vq: gi1 = 0.., gi2 = 3H..
-        const int off_out = cell ? off_h2new : off_h1new;
-#pragma unroll 1
-        for (int bi = 0; bi < NBLK; ++bi) {                    // ba: accumulator set / barrier block in this CTA; b: unit block of the layer
-          const int ba = (CL == 1) ? bi : cell, b = (CL == 1) ? bi : rank;
-          const int u = b * MROWS + row;
-          const float qk_r = __ldg(p.qk + qbase + u), qk_z = __ldg(p.qk + qbase + H + u), qk_n = __ldg(p.qk + qbase + 2 * H + u);
-          const float vq_r = __ldg(p.vq + qbase + u), vq_z = __ldg(p.vq + qbase + H + u), vq_n = __ldg(p.vq + qbase + 2 * H + u);
-          const float bh_r = __ldg(bh + u), bh_z = __ldg(bh + H + u), bh_n = __ldg(bh + 2 * H + u);
-          float* hrow = st + (size_t)u * NF;
-          float hp[NF];
-          if (t > 0) {
+      // ---- epilogue of one (phase, block) group: accumulators -> gates / relu / logits -----------------------------------
+      auto epilogue = [&](int phase, int blk) {
+        if (phase <= 1) {                                      // P1 / P2: the two GRU cells
+          const int cell = phase;
+          float* stt = cell ? st_h2 : st_h1;
+          const float* bh = cell ? p.b2h : p.b1h;
+          const int qbase = cell * 3 * H;                      // rows of qk / vq: gi1 = 0.., gi2 = 3H..
+          const int off_out = cell ? off_h2new : off_h1new;
 #pragma unroll
-            for (int i = 0; i < NF / 4; ++i) {
-              const float4 v = __ldcg(reinterpret_cast<const float4*>(hrow) + i);
-              hp[4 * i] = v.x; hp[4 * i + 1] = v.y; hp[4 * i + 2] = v.z; hp[4 * i + 3] = v.w;
-            }
-          } else {
+          for (int hr = 0; hr < 2; ++hr) {
+            const int u = blk * MROWS + rw + 8 * hr;
+            const float qk_r = __ldg(p.qk + qbase + u), qk_z = __ldg(p.qk + qbase + H + u), qk_n = __ldg(p.qk + qbase + 2 * H + u);
+            const float vq_r = __ldg(p.vq + qbase + u), vq_z = __ldg(p.vq + qbase + H + u), vq_n = __ldg(p.vq + qbase + 2 * H + u);
+            const float bh_r = __ldg(bh + u), bh_z = __ldg(bh + H + u), bh_n = __ldg(bh + 2 * H + u);
+            float* hrow = stt + (size_t)u * NF;
 #pragma unroll
-            for (int i = 0; i < NF; ++i) hp[i] = 0.f;
-          }
-          wait_full(ba);
+            for (int j = 0; j < NF / 8; ++j) {
+              const int f = 8 * j + fc;
+              float2 hp = make_float2(0.f, 0.f);
+              if (t > 0) hp = __ldcg(reinterpret_cast<const float2*>(hrow + f));
+              float hv[2] = {hp.x, hp.y};
 #pragma unroll
-          for (int half = 0; half < NF / 16; ++half) {
-            float ar[16], az[16], ai[16], ah[16];
-            tmem_ld16(tlane + (4 * ba + 0) * NF + half * 16, ar);
-            tmem_ld16(tlane + (4 * ba + 1) * NF + half * 16, az);
-            tmem_ld16(tlane + (4 * ba + 2) * NF + half * 16, ai);
-            tmem_ld16(tlane + (4 * ba + 3) * NF + half * 16, ah);
-            tmem_ld_wait();
-            if (half == NF / 16 - 1) release_acc(ba);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const int f = half * 16 + i;
-              const float x = x_s[f];
-              const float h = gru_unit_fast(ar[i] + qk_r + x * vq_r, az[i] + qk_z + x * vq_z, ai[i] + qk_n + x * vq_n,
-                                            bh_r, bh_z, ah[i] + bh_n, hp[f]);
-              // (the recurrent r / z contributions are already inside ar / az: one accumulator per gate)
-              hp[f] = h;
-              img_store(off_out, f, u, to_bits(h));
+              for (int e = 0; e < 2; ++e) {
+                const int i = 4 * j + 2 * hr + e;
+                const float x = x_s[f + e];
+                // (the recurrent r / z contributions are already inside acc[0] / acc[1]: one accumulator per gate)
+                hv[e] = gru_unit_fast(acc[0][i] + qk_r + x * vq_r, acc[1][i] + qk_z + x * vq_z, acc[2][i] + qk_n + x * vq_n,
+                                      bh_r, bh_z, acc[3][i] + bh_n, hv[e]);
+                img_store(off_out, f + e, u, hv[e]);
+              }
+              __stcg(reinterpret_cast<float2*>(hrow + f), make_float2(hv[0], hv[1]));
             }
           }
+          publish_ready(cell ? W_H2NEW : W_H1NEW, blk, off_out);
+        } else if (phase <= 3) {                               // P3 fc1 -> y1 into X[cur], P4 fc2 -> y2 into H[cur]
+          const int qbase = (phase == 2 ? 6 : 7) * H;
 #pragma unroll
-          for (int i = 0; i < NF / 4; ++i)
-            __stcg(reinterpret_cast<float4*>(hrow) + i, make_float4(hp[4 * i], hp[4 * i + 1], hp[4 * i + 2], hp[4 * i + 3]));
-          publish_ready(cell ? W_H2NEW : W_H1NEW, b, off_out);           // block by block: the consumers' K chunks wait per block
-        }
-      }
-
-      // ---- P3: fc1 -> y1 into X[cur] (its readers, this step's W1h h1 MMAs, completed before P1's block-full) ------
-      {
-        const int qbase = 6 * H;
-#pragma unroll 1
-        for (int bi = 0; bi < NBLK; ++bi) {
-          const int ba = (CL == 1) ? bi : 2, b = (CL == 1) ? bi : rank;
-          const int u = b * MROWS + row;
-          const float qk_u = __ldg(p.qk + qbase + u), vq_u = __ldg(p.vq + qbase + u);
-          wait_full(ba);
+          for (int hr = 0; hr < 2; ++hr) {
+            const int u = blk * MROWS + rw + 8 * hr;
+            const float qk_u = __ldg(p.qk + qbase + u), vq_u = phase == 2 ? __ldg(p.vq + qbase + u) : 0.f;
 #pragma unroll
-          for (int half = 0; half < NF / 16; ++half) {
-            float a[16], a1[16], a2[16], a3[16];                // the four K-quarter partials (one per issuing warp)
-            tmem_ld16(tlane + (4 * ba + 0) * NF + half * 16, a);
-            tmem_ld16(tlane + (4 * ba + 1) * NF + half * 16, a1);
-            tmem_ld16(tlane + (4 * ba + 2) * NF + half * 16, a2);
-            tmem_ld16(tlane + (4 * ba + 3) * NF + half * 16, a3);
-            tmem_ld_wait();
-            if (half == NF / 16 - 1) release_acc(ba);
+            for (int j = 0; j < NF / 8; ++j) {
 #pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const int f = half * 16 + i;
-              img_store(off_y1, f, u, to_bits(fmaxf(((a[i] + a1[i]) + (a2[i] + a3[i])) + qk_u + x_s[f] * vq_u, 0.f)));
+              for (int e = 0; e < 2; ++e) {
+                const int i = 4 * j + 2 * hr + e, f = 8 * j + fc + e;
+                const float a = (acc[0][i] + acc[1][i]) + (acc[2][i] + acc[3][i]);
+                const float y = phase == 2 ? fmaxf(a + qk_u + x_s[f] * vq_u, 0.f) : fmaxf(a + qk_u, 0.f);
+                img_store(phase == 2 ? off_y1 : off_y2, f, u, y);
+              }
             }
           }
-          publish_ready(W_Y1, b, off_y1);
-        }
-      }
-      // ---- P4: fc2 -> y2.  y2 REPLACES y1 in X[cur], which the fc2 MMAs of the later blocks still read: the values are
-      // held in registers (packed pairs) until block 3's block-full, i.e. until every fc2 MMA of every issuing warp has
-      // completed (each warp's block-3 commit follows its chunks of blocks 0-2), and written then.  One image saved =
-      // two more ring slots for the weight stream.
-      if constexpr (CL == 1)
-      {
-        const int qbase = 7 * H;
-        uint32_t ypk[4][NF / 2];
+          publish_ready(phase == 2 ? W_Y1 : W_Y2, blk, phase == 2 ? off_y1 : off_y2);
+        } else {                                               // P5 (rank 0): logits -> transpose -> one thread per fold samples
+          if (wg == 0 && rw < 32) {
 #pragma unroll
-        for (int b = 0; b < 4; ++b) {
-          const float qk_u = __ldg(p.qk + qbase + b * MROWS + row);
-          wait_full(b);
+            for (int hr = 0; hr < 2; ++hr) {
+              const int row = rw + 8 * hr;
+              const float b3 = __ldg(p.b3 + row);
 #pragma unroll
-          for (int half = 0; half < NF / 16; ++half) {
-            float a[16], a1[16], a2[16], a3[16];
-            tmem_ld16(tlane + (4 * b + 0) * NF + half * 16, a);
-            tmem_ld16(tlane + (4 * b + 1) * NF + half * 16, a1);
-            tmem_ld16(tlane + (4 * b + 2) * NF + half * 16, a2);
-            tmem_ld16(tlane + (4 * b + 3) * NF + half * 16, a3);
-            tmem_ld_wait();
-            if (half == NF / 16 - 1) release_acc(b);
+              for (int j = 0; j < NF / 8; ++j) {
 #pragma unroll
-            for (int i = 0; i < 16; i += 2) {
-              const float y0 = fmaxf(((a[i] + a1[i]) + (a2[i] + a3[i])) + qk_u, 0.f);
-              const float y1v = fmaxf(((a[i + 1] + a1[i + 1]) + (a2[i + 1] + a3[i + 1])) + qk_u, 0.f);
-              ypk[b][half * 8 + i / 2] = pack2<FMT>(y0, y1v);
+                for (int e = 0; e < 2; ++e) {
+                  const int i = 4 * j + 2 * hr + e;
+                  log_s[(8 * j + fc + e) * SM::LOGP + row] = ((acc[0][i] + acc[1][i]) + (acc[2][i] + acc[3][i])) + b3;   // [fold][class]
+                }
+              }
             }
           }
-        }
+          named_bar_sync(3, N_CONSUMERS);                      // the logits of every fold are in log_s
+          if (warp == 0) {
+            float xnew = 0.f;
+            if (sampler) {
+              float lgo[32];
 #pragma unroll
-        for (int b = 0; b < 4; ++b) {
+              for (int i = 0; i < 32; ++i) lgo[i] = log_s[lane * SM::LOGP + i];
+              xnew = mol_sample_fast(lgo, ur);
+              const int gf = f0 + lane;
+              p.out[(size_t)gf * p.out_pitch + t] = xnew;
+              if (p.logits_out) {
 #pragma unroll
-          for (int i = 0; i < NF / 2; ++i) {
-            *img_ptr(off_y1, 2 * i, b * MROWS + row) = (uint16_t)(ypk[b][i] & 0xffffu);
-            *img_ptr(off_y1, 2 * i + 1, b * MROWS + row) = (uint16_t)(ypk[b][i] >> 16);
-          }
-        }
-#pragma unroll
-        for (int b = 0; b < 4; ++b) publish_ready(W_Y2, b, off_y1);
-      }
-      else {                                                     // cluster form: y2 has its own place (the stale h2 image), nothing to defer
-        const int u = rank * MROWS + row;
-        const float qk_u = __ldg(p.qk + 7 * H + u);
-        wait_full(3);                                            // accumulator set 3 (= phase)
-#pragma unroll
-        for (int half = 0; half < NF / 16; ++half) {
-          float a[16], a1[16], a2[16], a3[16];
-          tmem_ld16(tlane + 12 * NF + half * 16, a);
-          tmem_ld16(tlane + 13 * NF + half * 16, a1);
-          tmem_ld16(tlane + 14 * NF + half * 16, a2);
-          tmem_ld16(tlane + 15 * NF + half * 16, a3);
-          tmem_ld_wait();
-          if (half == NF / 16 - 1) release_acc(3);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) img_store(off_y2, half * 16 + i, u, to_bits(fmaxf(((a[i] + a1[i]) + (a2[i] + a3[i])) + qk_u, 0.f)));
-        }
-        publish_ready(W_Y2, rank, off_y2);                               // each CTA delivers ITS block of y2; rank 0's fc3 chunks wait per block
-      }
-
-      // ---- P5: logits -> transpose through shared memory -> one thread per fold samples ----------------------------
-      // (cluster form: fc3 lives in rank 0 only; it samples and hands x to the other three CTAs)
-      if (rank == 0) {
-        wait_full(0);
-        if ((warp & 3) == 0) {
-#pragma unroll
-          for (int half = 0; half < NF / 16; ++half) {
-            float a[16], a1[16], a2[16], a3[16];
-            tmem_ld16(tlane + 0 * NF + half * 16, a);
-            tmem_ld16(tlane + 1 * NF + half * 16, a1);
-            tmem_ld16(tlane + 2 * NF + half * 16, a2);
-            tmem_ld16(tlane + 3 * NF + half * 16, a3);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) a[i] = (a[i] + a1[i]) + (a2[i] + a3[i]);
-            const float b3 = __ldg(p.b3 + row);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) log_s[(half * 16 + i) * SM::LOGP + lane] = a[i] + b3;   // [fold][class], class == lane
-          }
-        }
-        release_acc(0);
-        if ((warp & 3) == 0) {
-          __syncwarp();
-          float xnew = 0.f;
-          if (sampler) {
-            float lgo[32];
-#pragma unroll
-            for (int i = 0; i < 32; ++i) lgo[i] = log_s[lane * SM::LOGP + i];
-            xnew = mol_sample_fast(lgo, ur);
-            const int gf = f0 + lane;
-            p.out[(size_t)gf * p.out_pitch + t] = xnew;
-            if (p.logits_out) {
-#pragma unroll
-              for (int i = 0; i < 30; ++i) p.logits_out[((size_t)t * p.n_total + gf) * 30 + i] = lgo[i];
-            }
-            if (p.x_force) xnew = __ldg(p.x_force + (size_t)t * p.n_total + gf);             // teacher forcing: step t+1 consumes x_force[t]
-          }
-          __syncwarp();
-          if constexpr (CL == 1) {
-            if (lane < NF) x_s[lane] = xnew;
-          } else {
-            if (lane < NF) {
-              const uint32_t a = smem_u32(x_s + lane);
-#pragma unroll
-              for (int r = 0; r < CL; ++r)
-                asm volatile("st.shared::cluster.f32 [%0], %1;" :: "r"(map_to_rank(a, (uint32_t)r)), "f"(xnew) : "memory");
+                for (int i = 0; i < 30; ++i) p.logits_out[((size_t)t * p.n_total + gf) * 30 + i] = lgo[i];
+              }
+              if (p.x_force) xnew = __ldg(p.x_force + (size_t)t * p.n_total + gf);             // teacher forcing: step t+1 consumes x_force[t]
             }
             __syncwarp();
-            if (lane == 0) {
+            if constexpr (CL == 1) {
+              if (lane < NF) x_s[lane] = xnew;
+            } else {
+              if (lane < NF) {
+                const uint32_t a = smem_u32(x_s + lane);
 #pragma unroll
-              for (int r = 0; r < CL; ++r)
-                asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" :: "r"(map_to_rank(bar(BAR_X), (uint32_t)r)) : "memory");
+                for (int r = 0; r < CL; ++r)
+                  asm volatile("st.shared::cluster.f32 [%0], %1;" :: "r"(map_to_rank(a, (uint32_t)r)), "f"(xnew) : "memory");
+              }
+              __syncwarp();
+              if (lane == 0) {
+#pragma unroll
+                for (int r = 0; r < CL; ++r)
+                  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" :: "r"(map_to_rank(bar(BAR_X), (uint32_t)r)) : "memory");
+              }
             }
           }
         }
+      };
+
+      // ---- the step program ---------------------------------------------------------------------------------------------
+      uint4 nx = __ldg(prog);
+#pragma unroll 1
+      for (int c = 0; c < n_prog; ++c) {
+        const uint4 r = nx;
+        if (c + 1 < n_prog) nx = __ldg(prog + c + 1);
+        const uint32_t accsel = r.z & 0xffu, flags = (r.z >> 8) & 0xffu, wait_b = (r.z >> 16) & 0xffu;
+        const uint32_t phase = (r.z >> 24) & 0xfu, blk = r.z >> 28;
+        long long c0 = 0, c1 = 0, c2 = 0;
+        if (profiling) c0 = clock64();
+        const uint32_t wkind = wait_b & 15u;
+        if (wkind == W_COND) wait(bar(BAR_READY + cur), (uint32_t)(t >> 1) & 1);
+        else if (wkind != W_NONE) {
+          // the block this K range reads: written here through the generic proxy (fenced by its writers), or a peer's
+          // block that arrived by bulk copy (async proxy, complete_tx on this barrier) -- like a TMA load, no fence
+          wait(bar(BAR_READY + 2 + (wkind - W_H1NEW) * 4 + (wait_b >> 4)), (uint32_t)t & 1);
+        }
+        if (profiling) c1 = clock64();
+        if (!(flags & DF_SAME_SLOT)) {
+          slot = g_next % SM::STAGES;
+          wait(bar(BAR_FULL + slot), (g_next / SM::STAGES) & 1);
+          ++g_next;
+        }
+        if (profiling) c2 = clock64();
+        {
+          const bool one = (flags & DF_NK1) != 0;
+          // (address field: 14 bits of byte address >> 4 -- masked, because in a cluster launch the shared::cta window of
+          //  ranks > 0 need not start at 0)
+          const uint32_t a_lo = (ring_lo + (uint32_t)slot * (SM::SLOT_BYTES >> 4) + (uint32_t)wg * (one ? (2048u >> 4) : (8192u >> 4))) & 0x3fffu;
+          const uint64_t da = (uint64_t)a_lo | LBO | ((uint64_t)((one ? 256u : 1024u) >> 4) << 32);
+          const uint64_t sbo_b = (uint64_t)(((flags & DF_B_COND) ? (uint32_t)SBO_Q : (uint32_t)SBO_H) >> 4) << 32;
+          const uint32_t blo = cur ? (r.y >> 16) : (r.y & 0xffffu);
+          const uint64_t db = (uint64_t)((s0_lo + blo) & 0x3fffu) | LBO | sbo_b;
+          const uint32_t scale0 = (flags & DF_FIRST) ? 0u : 1u;
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k)           // K = 16 chunk: steps 1-3 multiply the zero block (SBO 0: every row group)
+            wgmma_ss<NF, FMT>(d, da + (uint64_t)(16 * k), (one && k > 0) ? dz : db + (uint64_t)(16 * k), k == 0 ? scale0 : 1u);
+          wgmma_commit();
+          wgmma_wait<0>();
+        }
+        __syncwarp();
+        if (lane == 0) {
+          if (!(flags & DF_KEEP_SLOT)) mbar_arrive(bar(BAR_EMPTY + slot));   // this warp's reads of the slot are complete
+          if (flags & DF_COND_RELEASE) mbar_arrive(bar(BAR_COND_FREE + cur));
+        }
+        if (flags & DF_ACC_END) {
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+#pragma unroll
+            for (int i = 0; i < NF / 2; ++i) acc[j][i] = (accsel == (uint32_t)j) ? d[i] : acc[j][i];
+          }
+        }
+        if (profiling) { const long long c3 = clock64(); t_b += c1 - c0; t_ring += c2 - c1; t_issue += c3 - c2; }
+        if (flags & DF_END) {
+          long long e0 = 0;
+          if (profiling) e0 = clock64();
+          epilogue((int)phase, (int)blk);
+          if (profiling) t_epi += clock64() - e0;
+        }
       }
-      // cluster form: x of this step has landed here (rank 0's remote stores, released at cluster scope).  One thread
+      // x of this step has landed here (cluster form: rank 0's remote stores, released at cluster scope).  One thread
       // acquires -- every poll of an acquire.cluster wait invalidates L1 --, the named barrier below hands it on.
-      if (tid == EPI_TID0) {
+      if (tid == 0) {
         if constexpr (CL > 1) wait_peer(bar(BAR_X), (uint32_t)t & 1);
         *ep_stop = *s_abort;
       }
-      named_bar_sync(1, 128);                                  // x of this step (and the stop decision) visible to all epilogue threads
-      if (profiling) t_work += clock64() - w0;
+      named_bar_sync(1, N_CONSUMERS);                          // x of this step (and the stop decision) visible to all consumers
       if (*ep_stop) break;
     }
-    if (profiling) { p.prof[4] = t_wait; p.prof[5] = t_work; }
+    if (profiling) { p.prof[0] = t_b; p.prof[1] = t_ring; p.prof[2] = t_issue; p.prof[3] = t_epi; }
   }
 
-  tc_fence_before();
   __syncthreads();
   if constexpr (CL > 1) cluster_sync_all();                  // nobody leaves while a peer may still write into its shared memory
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem), "n"(TMEM_COLS));
 }
 
 // --------------------------------------------------------------------------------------------------------------------
@@ -700,9 +522,10 @@ class StreamEngine : public Engine {
  public:
   ~StreamEngine() override {
     cudaSetDevice(device);
-    for (auto& v : var_) { cudaFree(v.d_blob); cudaFree(v.d_prog); cudaFree(v.d_sizes); }
+    for (auto& v : var_) { cudaFree(v.d_blob); cudaFree(v.d_prog); }
     cudaFree(d_vec_); cudaFree(d_state_); cudaFree(d_sync_);
   }
+  // (engine names are part of the C ABI's introspection surface and predate the Hopper port)
   const char* name() const override {
     if (last_cluster_) return cfg.precision == WRNN_PREC_BF16 ? "tcgen05-stream-x4-bf16" : "tcgen05-stream-x4-fp16";
     return cfg.precision == WRNN_PREC_BF16 ? "tcgen05-stream-bf16" : "tcgen05-stream-fp16";
@@ -714,44 +537,33 @@ class StreamEngine : public Engine {
     return frames ? (const void*)wrnn_stream_kernel<NF, 0, true, PROF, CL> : (const void*)wrnn_stream_kernel<NF, 0, false, PROF, CL>;
   }
   template <int NF, int CL> const void* kernel_nf(bool frames, bool prof) const { return prof ? kernel_p<NF, CL, true>(frames) : kernel_p<NF, CL, false>(frames); }
-  template <int NF, int CL> static SmemLayout layout() {
-    using S = Smem<NF, CL>;
-    return SmemLayout{S::OFF_X0, S::OFF_X1, {S::OFF_H2, S::OFF_H2B}, S::OFF_COND, S::COND, S::CPS, CL > 1};
+  template <int NF> static SmemLayout layout() {
+    using S = Smem<NF>;
+    return SmemLayout{S::OFF_X0, S::OFF_X1, {S::OFF_H2, S::OFF_H2B}, S::OFF_COND, S::COND};
   }
 
-  // one (cluster size, folds per CTA) combination: its weight streams (one per cluster rank), device programs and kernel
+  // one (cluster size, folds per CTA) combination: its weight streams (one per cluster rank) and device programs
   struct Variant {
     int nf = 0, cl = 1, smem = 0;
-    void *d_blob = nullptr, *d_prog = nullptr, *d_sizes = nullptr;
-    size_t blob_off[4] = {0, 0, 0, 0}, prog_off[4][N_ISSUERS] = {}, sizes_off[4] = {0, 0, 0, 0};
-    int n_mine[4][N_ISSUERS] = {}, n_slots[4] = {0, 0, 0, 0};
+    void *d_blob = nullptr, *d_prog = nullptr;
+    size_t blob_off[4] = {0, 0, 0, 0}, prog_off[4] = {0, 0, 0, 0};
+    int n_prog[4] = {0, 0, 0, 0};
   };
 
   int upload(Variant& v, const std::vector<Plan>& plans, const SmemLayout& L) {
-    std::vector<uint8_t> blob; std::vector<DevChunk> prog; std::vector<uint16_t> sizes;
+    std::vector<uint8_t> blob; std::vector<DevChunk> prog;
     for (size_t r = 0; r < plans.size(); ++r) {
       const Plan& pl = plans[r];
-      if (L.cps == 2) {
-        if (pl.prog.size() % 2) { set_error("stream plan: odd chunk count"); return WRNN_E_INVALID; }
-        for (size_t i = 0; i < pl.prog.size(); i += 2)
-          if (pl.prog[i].owner != pl.prog[i + 1].owner) { set_error("stream plan: a chunk pair with two owners"); return WRNN_E_INVALID; }
-      }
-      for (int o = 0; o < N_ISSUERS; ++o)
-        if (pl.mine[o].size() % 2) { set_error("stream plan: an issuing warp with an odd number of chunks"); return WRNN_E_INVALID; }
-      DevProgram dp;
-      compile_device(pl, L, dp);
+      std::vector<DevChunk> dp;
+      compile_device(pl, L, plans.size() > 1 ? (int)r : -1, dp);
       v.blob_off[r] = blob.size(); blob.insert(blob.end(), pl.blob.begin(), pl.blob.end());
       while (blob.size() % 16) blob.push_back(0);
-      for (int o = 0; o < N_ISSUERS; ++o) { v.prog_off[r][o] = prog.size(); v.n_mine[r][o] = (int)dp.mine[o].size(); prog.insert(prog.end(), dp.mine[o].begin(), dp.mine[o].end()); }
-      const std::vector<uint16_t>& sz = L.cps == 2 ? dp.pair_size16 : dp.chunk_size16;
-      v.sizes_off[r] = sizes.size(); v.n_slots[r] = (int)sz.size(); sizes.insert(sizes.end(), sz.begin(), sz.end());
+      v.prog_off[r] = prog.size(); v.n_prog[r] = (int)dp.size(); prog.insert(prog.end(), dp.begin(), dp.end());
     }
     WRNN_CUDA_OK(cudaMalloc(&v.d_blob, blob.size()));
     WRNN_CUDA_OK(cudaMemcpy(v.d_blob, blob.data(), blob.size(), cudaMemcpyHostToDevice));
     WRNN_CUDA_OK(cudaMalloc(&v.d_prog, prog.size() * sizeof(DevChunk)));
     WRNN_CUDA_OK(cudaMemcpy(v.d_prog, prog.data(), prog.size() * sizeof(DevChunk), cudaMemcpyHostToDevice));
-    WRNN_CUDA_OK(cudaMalloc(&v.d_sizes, sizes.size() * sizeof(uint16_t)));
-    WRNN_CUDA_OK(cudaMemcpy(v.d_sizes, sizes.data(), sizes.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
     return WRNN_OK;
   }
 
@@ -762,10 +574,10 @@ class StreamEngine : public Engine {
     for (int r = 0; r < 4; ++r) build_plan(w, bf, split[r], r);
     n_chunks_ = (int)whole[0].prog.size(); n_mma_ = whole[0].n_mma;
     int rc;
-    var_[0].nf = 16; var_[0].cl = 1; var_[0].smem = Smem<16, 1>::BYTES; if ((rc = upload(var_[0], whole, layout<16, 1>())) != WRNN_OK) return rc;
-    var_[1].nf = 32; var_[1].cl = 1; var_[1].smem = Smem<32, 1>::BYTES; if ((rc = upload(var_[1], whole, layout<32, 1>())) != WRNN_OK) return rc;
-    var_[2].nf = 16; var_[2].cl = 4; var_[2].smem = Smem<16, 4>::BYTES; if ((rc = upload(var_[2], split, layout<16, 4>())) != WRNN_OK) return rc;
-    var_[3].nf = 32; var_[3].cl = 4; var_[3].smem = Smem<32, 4>::BYTES; if ((rc = upload(var_[3], split, layout<32, 4>())) != WRNN_OK) return rc;
+    var_[0].nf = 16; var_[0].cl = 1; var_[0].smem = Smem<16>::BYTES; if ((rc = upload(var_[0], whole, layout<16>())) != WRNN_OK) return rc;
+    var_[1].nf = 32; var_[1].cl = 1; var_[1].smem = Smem<32>::BYTES; if ((rc = upload(var_[1], whole, layout<32>())) != WRNN_OK) return rc;
+    var_[2].nf = 16; var_[2].cl = 4; var_[2].smem = Smem<16>::BYTES; if ((rc = upload(var_[2], split, layout<16>())) != WRNN_OK) return rc;
+    var_[3].nf = 32; var_[3].cl = 4; var_[3].smem = Smem<32>::BYTES; if ((rc = upload(var_[3], split, layout<32>())) != WRNN_OK) return rc;
     const Plan& plan = whole[0];
     std::vector<float> vec;
     off_qk_ = 0; vec.insert(vec.end(), plan.qk.begin(), plan.qk.end());
@@ -779,12 +591,23 @@ class StreamEngine : public Engine {
     WRNN_CUDA_OK(cudaMemset(d_sync_, 0, 256));
     for (int k = 0; k < 4; ++k) {
       const bool fr = (k & 1) != 0, pr = (k & 2) != 0;
-      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<16, 1>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<16, 1>::BYTES));
-      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<32, 1>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<32, 1>::BYTES));
-      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<16, 4>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<16, 4>::BYTES));
-      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<32, 4>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<32, 4>::BYTES));
+      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<16, 1>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<16>::BYTES));
+      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<32, 1>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<32>::BYTES));
+      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<16, 4>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<16>::BYTES));
+      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<32, 4>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<32>::BYTES));
     }
     WRNN_CUDA_OK(cudaDeviceGetAttribute(&n_sm_, cudaDevAttrMultiProcessorCount, device));
+    // clusters of four that fit the device at once (GPC granularity); both tile sizes use the same shared memory class
+    {
+      cudaLaunchConfig_t lc{};
+      lc.gridDim = dim3(4 * n_sm_); lc.blockDim = dim3(NT); lc.dynamicSmemBytes = Smem<32>::BYTES;
+      cudaLaunchAttribute at[1];
+      at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 4; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+      lc.attrs = at; lc.numAttrs = 1;
+      int n_cl = 0;
+      WRNN_CUDA_OK(cudaOccupancyMaxActiveClusters(&n_cl, kernel_nf<32, 4>(false, false), &lc));
+      max_clusters_ = n_cl;
+    }
     return WRNN_OK;
   }
 
@@ -793,12 +616,12 @@ class StreamEngine : public Engine {
   }
   bool supports(const wrnn_job& job) const override { return job.expo == nullptr && !(job.mel_frames && job.cond_mode == WRNN_COND_EXPAND && job.fold_row0); }
 
-  // Which form serves n folds (per-step times measured on B200, profiles/r02_stream.md):
-  //   one CTA per tile : ~66 us (16 folds per CTA, <= 148 tiles), ~95 us (32 folds per CTA) per wave of 148 tiles
+  // Which form serves n folds:
+  //   one CTA per tile : 16 folds per CTA while the tiles fit one wave (one tile per SM), 32 folds per CTA beyond
   //   cluster of 4     : the rows of every layer split over four CTAs -> a quarter of the stream per SM; used while the
-  //                      clusters of the job are co-resident (33 clusters of 4 with this shared-memory footprint)
+  //                      clusters of the job are co-resident (cudaOccupancyMaxActiveClusters at init)
   void choose(int n_seg, int& nf, int& cl) const {
-    const int max_cl = (n_sm_ / 4) - 4;            // 33 on a 148-SM part (GPC granularity), measured with cudaOccupancyMaxActiveClusters
+    const int max_cl = max_clusters_;
     if ((n_seg + 15) / 16 <= max_cl) { nf = 16; cl = 4; }
     else if ((n_seg + 31) / 32 <= max_cl) { nf = 32; cl = 4; }
     else if ((n_seg + 15) / 16 <= n_sm_) { nf = 16; cl = 1; }
@@ -823,9 +646,8 @@ class StreamEngine : public Engine {
     const float* v = static_cast<const float*>(d_vec_);
     for (int r = 0; r < cl; ++r) {
       p.blob[r] = static_cast<const unsigned char*>(V.d_blob) + V.blob_off[r];
-      p.slot_size16[r] = static_cast<const unsigned short*>(V.d_sizes) + V.sizes_off[r];
-      p.n_slots[r] = V.n_slots[r];
-      for (int o = 0; o < N_ISSUERS; ++o) { p.mine[r * N_ISSUERS + o] = static_cast<const uint4*>(V.d_prog) + V.prog_off[r][o]; p.n_mine[r * N_ISSUERS + o] = V.n_mine[r][o]; }
+      p.prog[r] = static_cast<const uint4*>(V.d_prog) + V.prog_off[r];
+      p.n_prog[r] = V.n_prog[r];
     }
     p.qk = v + off_qk_; p.vq = v + off_vq_; p.b1h = v + off_b1h_; p.b2h = v + off_b2h_; p.b3 = v + off_b3_;
     p.mels_up = job.mels_up; p.aux = job.aux; p.L = job.L; p.seg_stride = job.seg_stride; p.row_base = 0;
@@ -861,9 +683,9 @@ class StreamEngine : public Engine {
     if (getenv("WRNN_STREAM_PROF") && last_steps_ > 0) {
       long long prof[16]; std::memcpy(prof, buf + 64, sizeof(prof));
       const long long n = last_steps_;
-      fprintf(stderr, "[wrnn_stream prof] NF=%d cluster=%d CTAs=%d steps=%d mma/step=%d chunks/step=%d | issuer 0: acc-wait=%lld operand-wait=%lld ring-wait=%lld "
-              "issue=%lld | epilogue thread: mma-wait=%lld step=%lld (cycles per step)\n",
-              last_nf_, last_cluster_ ? 4 : 1, last_grid_, last_steps_, n_mma_, n_chunks_, prof[0] / n, prof[1] / n, prof[2] / n, prof[3] / n, prof[4] / n, prof[5] / n);
+      fprintf(stderr, "[wrnn_stream prof] NF=%d cluster=%d CTAs=%d steps=%d mma/step=%d chunks/step=%d | consumer thread 0: operand-wait=%lld "
+              "ring-wait=%lld mma=%lld epilogue=%lld (cycles per step)\n",
+              last_nf_, last_cluster_ ? 4 : 1, last_grid_, last_steps_, n_mma_, n_chunks_, prof[0] / n, prof[1] / n, prof[2] / n, prof[3] / n);
     }
     if (flag != 0) { set_error("stream kernel aborted: an mbarrier wait (TMA / MMA / operand hand-off) timed out"); return WRNN_E_WATCHDOG; }
     return WRNN_OK;
@@ -873,7 +695,7 @@ class StreamEngine : public Engine {
   Variant var_[4];
   void *d_vec_ = nullptr, *d_state_ = nullptr, *d_sync_ = nullptr;
   size_t state_bytes_ = 0, off_qk_ = 0, off_vq_ = 0, off_b1h_ = 0, off_b2h_ = 0, off_b3_ = 0;
-  int n_chunks_ = 0, n_mma_ = 0, n_sm_ = 0, last_grid_ = 0, last_steps_ = 0, last_nf_ = 0;
+  int n_chunks_ = 0, n_mma_ = 0, n_sm_ = 0, max_clusters_ = 0, last_grid_ = 0, last_steps_ = 0, last_nf_ = 0;
   bool last_cluster_ = false;
 };
 

@@ -6,10 +6,10 @@
 // Decomposition ("activation-stationary"; the opposite of wrnn_tc.cu).  A CTA owns NF folds for the whole sequence
 // and runs EVERY layer for them; nothing is exchanged between SMs.  The weights (7.4 MB as fp16) do not fit one SM,
 // so they are streamed from L2 every step, in the order the step consumes them, through a shared-memory ring (TMA
-// bulk copies; every CTA of the grid reads the same stream, which the 126 MB L2 serves at ~100 B/cycle/SM --
-// profiles/r02_probes.md).  Contractions are "swap-AB": the weight rows are the MMA M dimension (tiles of 128 rows =
-// 128 TMEM lanes), the CTA's folds are N (NF = 16 or 32), D[rows, folds] += W[rows, k0:k0+16] * act[folds, k0:k0+16]^T.
-// A GRU unit's r / z / n pre-activations sit in the SAME TMEM lane of different accumulators, so the gate math is
+// bulk copies; every CTA of the grid reads the same stream, which the 50 MB L2 serves to every SM).  Contractions are
+// "swap-AB": the weight rows are the MMA M dimension (tiles of 128 rows, two wgmma M tiles of 64), the CTA's folds are
+// N (NF = 16 or 32), D[rows, folds] += W[rows, k0:k0+16] * act[folds, k0:k0+16]^T.
+// A GRU unit's r / z / n pre-activations sit in the SAME fragment position of different accumulators, so the gate math is
 // thread-local (one thread per unit row, NF folds each).
 //
 // Per step (folded algebra of wrnn_fold.h; reference models/fatchord_version.py:208-223), unit blocks b = 0..3 of 128:
@@ -21,6 +21,7 @@
 // The program lists the weight chunks in exactly this order; within P2 every chunk that does not depend on h1' is
 // issued first, so those MMAs (and the epilogue-free h2 reads) overlap the P1 gate math.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <cstring>
 #include <vector>
@@ -30,7 +31,7 @@
 namespace wrnn {
 namespace stream {
 
-constexpr int MROWS = 128;          // weight rows per MMA tile (UMMA M)
+constexpr int MROWS = 128;          // weight rows per streamed chunk (two wgmma M tiles)
 constexpr int KCH = 64;             // K elements per streamed chunk (4 MMAs of K = 16)
 constexpr int CHUNK_BYTES = MROWS * KCH * 2;   // 16 KB: one chunk
 constexpr int PAIR_BYTES = 2 * CHUNK_BYTES;    // 32 KB ring slot: chunks are loaded two at a time (halves the producer's work per byte)
@@ -40,14 +41,14 @@ enum : uint8_t { B_COND = 0, B_H1PREV = 1, B_H1NEW = 2, B_H2 = 3, B_Y1 = 4, B_Y2
 // readiness barriers an issuer may have to wait for before a chunk
 enum : uint8_t { W_NONE = 0, W_COND = 1, W_H1NEW = 2, W_H2NEW = 3, W_Y1 = 4, W_Y2 = 5 };
 enum : uint8_t { F_FIRST = 1, F_COND_RELEASE = 2 };
-constexpr int N_ISSUERS = 4;        // issuing warps; every accumulator chain belongs to exactly one of them
+constexpr int N_ISSUERS = 4;        // owners: every accumulator chain of a (phase, block) belongs to exactly one of them
 constexpr int N_PHASES = 5;
 
 struct Chunk {            // 16 bytes, read as one uint4
   uint16_t size16;        // size of this chunk in the weight stream in 16-byte units (chunks are consecutive): 128 rows x (16*nk) x 2 B
   uint16_t a_off16;       // where the chunk lands inside its ring slot (16-byte units): chunks travel in PAIRS (one TMA, one
                           // barrier per pair), the second chunk of a pair sits right behind the first
-  uint8_t acc;            // accumulator index: TMEM column = acc * NF
+  uint8_t acc;            // accumulator index: 4 * block + owner
   uint8_t nk;             // K = 16 steps in this chunk
   uint8_t b_buf;          // B operand image (B_*)
   uint8_t b_buf2;         // second B operand for the same weight chunk (fc1: h2'), B_NONE otherwise
@@ -58,7 +59,7 @@ struct Chunk {            // 16 bytes, read as one uint4
                           // the block its K range reads
   uint8_t wait_acc;       // 0, or block + 1: first chunk of this issuer in (phase, block): the previous phase's epilogue must have drained the block
   uint8_t commit;         // 0, or block + 1: last chunk of this issuer in (phase, block): signal "my accumulators of the block are full"
-  uint8_t owner;          // issuing warp 0..3
+  uint8_t owner;          // owner 0..3 (the accumulator within its (phase, block) group)
   uint8_t phase;          // 0..4 (P1..P5)
 };
 static_assert(sizeof(Chunk) == 16, "Chunk must stay one uint4");
@@ -79,8 +80,8 @@ inline size_t tile_index(int r, int k, int kc) { return (size_t)(r / 8) * (kc / 
 
 // Builds the plan.  `bf` selects bf16 instead of fp16 operand bits.  n_classes <= 128 (MoL: 30).
 //
-// Ownership (one issuing warp per accumulator chain, four chains per unit block in every phase, so that the four warps
-// issue concurrently and "block full" always takes exactly four commits):
+// Ownership (one owner per accumulator chain, four chains per unit block in every phase; the stream order below
+// interleaves the four owners' chunks -- the kernel regroups them per owner, see compile_device):
 //   GRU phases : warp 0 = r, 1 = z, 2 = in (input-side n), 3 = hn (hidden-side n)            accumulators 4b + q
 //   fc phases  : the K dimension is split in four: warp q owns conditioning K-chunk q and K = [128q, 128q + 128) of the
 //                recurrent operand, into its own partial accumulator 4b + q (the epilogue adds the four partials)
@@ -162,7 +163,7 @@ inline void build_plan(const HostWeights& w, bool bf, Plan& p, int only_block = 
   const int NB = H / MROWS;             // 4 unit blocks
   const int B0 = only_block >= 0 ? only_block : 0, B1 = only_block >= 0 ? only_block + 1 : NB;     // blocks of this program
   // block id used for accumulators and their barriers: the unit block, or -- one-block programs -- the PHASE (P1..P4 ->
-  // sets 0..3, fc3 -> set 0 again): nothing else lives in the other three quarters of TMEM, and with a set per phase the
+  // sets 0..3, fc3 -> set 0 again): nothing else is computed in the other three, and with a set per phase the
   // MMAs of a phase never wait for the previous phase's epilogue to drain.
   auto ab = [&](int b, int phase) -> int { return only_block >= 0 ? (phase & 3) : b; };
   std::vector<double> F3((size_t)MROWS * H, 0.0);
@@ -231,62 +232,78 @@ inline void build_plan(const HostWeights& w, bool bf, Plan& p, int only_block = 
 }
 
 // ---- what the kernel reads -----------------------------------------------------------------------------------------
-// One 16-byte record per chunk with everything pre-digested for a given shared-memory layout (NF), so that the issuing
-// warps spend their instructions on MMAs, not on decoding: operand addresses are descriptor start-address fields
-// (byte offset >> 4 from the start of dynamic shared memory) for both parities of the h1 ping-pong.
-enum : uint8_t { DF_FIRST = 1, DF_COND_RELEASE = 2, DF_B_COND = 4, DF_NK1 = 8, DF_HAS_B2 = 16 };
+// The kernel's consumer warpgroups accumulate ONE chain at a time in registers and keep the finished chains of the current
+// (phase, block) until that block's epilogue, which they run as soon as its last chunk is done.  So they consume the
+// program grouped by (phase, block) and, inside a group, by accumulator: a stable reordering of the stream that keeps the
+// order of every accumulator's chunks (hence its floating-point sums) and only moves chunks of other accumulators (of P2:
+// the h1'-independent chunks of block b next to the W2x h1' chunks of block b).  The producer loads the chunks in that
+// order from their places in the weight stream.  Since block b's GRU2 epilogue now runs before block b+1's W2h h2
+// chunks, h2 ping-pongs (H0 / H1) in both forms, and y2 goes to the stale h2 image.
+// Every record is exactly four K = 16 MMAs (no branch around the MMAs: a branch makes the compiler serialize them):
+// the K = 16 tail of the conditioning row multiplies a zero operand in its last three, and an fc1 chunk, which feeds
+// h1' and h2', becomes two records on the same ring slot.
+enum : uint8_t { DF_FIRST = 1, DF_COND_RELEASE = 2, DF_B_COND = 4, DF_NK1 = 8, DF_SAME_SLOT = 16, DF_END = 32, DF_ACC_END = 64,
+                 DF_KEEP_SLOT = 128 };
 struct DevChunk {
-  uint16_t a_lo;          // chunk offset inside its 32 KB ring slot, >> 4
-  uint16_t b_lo[2];       // B operand start (>> 4) when the step parity cur is 0 / 1
-  uint16_t b2_lo[2];      // second B operand (fc1: h2'), same
-  uint8_t acc_phase;      // accumulator index | phase << 4
-  uint8_t flags;          // DF_*
-  uint16_t sync;          // wait_b | wait_acc << 3 | commit << 6 | wait_blk << 9     (W_* / block + 1 / block + 1 / block of the operand)
-  uint16_t pair;          // ring position of the chunk's slot load within the step (pair index, or chunk index if a slot holds one chunk)
+  uint32_t src16;         // offset of the chunk in the weight stream, >> 4 (its size: 4 KB if DF_NK1, else 16 KB)
+  uint16_t b_lo[2];       // B operand start (byte offset from the start of dynamic shared memory, >> 4), step parity 0 / 1
+  uint8_t acc;            // accumulator of the (phase, block) group: 0..3 (the plan's owner)
+  uint8_t flags;          // DF_*: SAME_SLOT = operand of the previous record's slot (no load), KEEP_SLOT = the next record
+                          // reuses this slot, ACC_END / END = last record of its accumulator / of its (phase, block) group,
+                          // COND_RELEASE = last conditioning read of the step
+  uint8_t wait_b;         // W_* | block << 4: readiness barrier to wait for before issuing
+  uint8_t phase_blk;      // phase | (global unit block) << 4
+  uint32_t reserved;      // keeps the record one uint4
 };
 static_assert(sizeof(DevChunk) == 16, "DevChunk must stay one uint4");
 
-// byte offsets of the operand images.  One-CTA form: h2 updated in place (off_h2[0] == off_h2[1]), y2 over y1 in X[cur].
-// Cluster form: h2 ping-pongs like h1 (peers write into each other's images and cannot know when a peer's W2h MMAs are
-// done), y1 goes to the stale h1 image X[cur], y2 to the stale h2 image H[cur].  `cps`: chunks per ring slot.
-struct SmemLayout { int off_x0, off_x1, off_h2[2], off_cond, cond_bytes, cps; bool y2_in_h2; };
+// byte offsets of the operand images: h1 and h2 ping-pong (X[cur] / H[cur] hold the previous step's values), y1 goes
+// to the stale h1 image X[cur], y2 to the stale h2 image H[cur]
+struct SmemLayout { int off_x0, off_x1, off_h2[2], off_cond, cond_bytes; };
 
-struct DevProgram {
-  std::vector<DevChunk> mine[N_ISSUERS];     // per issuing warp, in its own order (pairs are adjacent records)
-  std::vector<uint16_t> pair_size16;         // per pair in stream order: bytes >> 4 of the TMA that loads it
-  std::vector<uint16_t> chunk_size16;        // per chunk in stream order (layouts whose ring slot holds one chunk)
-};
-
-inline void compile_device(const Plan& p, const SmemLayout& L, DevProgram& d) {
-  for (auto& v : d.mine) v.clear();
-  d.pair_size16.assign((p.prog.size() + 1) / 2, 0);
-  d.chunk_size16.clear();
-  for (const Chunk& c : p.prog) d.chunk_size16.push_back(c.size16);
+// `block`: the unit block of a one-block program (cluster rank), or -1 for the whole program
+inline void compile_device(const Plan& p, const SmemLayout& L, int block, std::vector<DevChunk>& d) {
+  d.clear();
   auto base_of = [&](uint8_t buf, int cur, int phase) -> int {
     switch (buf) {
       case B_COND: return L.off_cond + cur * L.cond_bytes;
       case B_H1NEW: return cur ? L.off_x0 : L.off_x1;
       case B_H2: return L.off_h2[phase <= 1 ? cur : cur ^ 1];       // GRU2 reads the previous h2 (H[cur]), fc1 the new one (H[cur^1])
-      case B_Y2: return L.y2_in_h2 ? L.off_h2[cur] : (cur ? L.off_x1 : L.off_x0);
+      case B_Y2: return L.off_h2[cur];
       default: return cur ? L.off_x1 : L.off_x0;          // B_H1PREV, B_Y1
     }
   };
-  for (size_t i = 0; i < p.prog.size(); ++i) {
-    const Chunk& c = p.prog[i];
-    d.pair_size16[i / 2] = (uint16_t)(d.pair_size16[i / 2] + c.size16);
-    DevChunk r{};
-    r.a_lo = c.a_off16;
-    for (int cur = 0; cur < 2; ++cur) {
-      r.b_lo[cur] = (uint16_t)((base_of(c.b_buf, cur, c.phase) + c.k0 * 16) >> 4);
-      r.b2_lo[cur] = c.b_buf2 == B_NONE ? 0 : (uint16_t)((base_of(c.b_buf2, cur, c.phase) + c.k0 * 16) >> 4);
+  std::vector<size_t> src(p.prog.size() + 1, 0);
+  for (size_t i = 0; i < p.prog.size(); ++i) src[i + 1] = src[i] + (size_t)p.prog[i].size16;
+  auto group = [&](const Chunk& c) { return c.phase * 4 + c.acc / 4; };
+  std::vector<size_t> order(p.prog.size());
+  for (size_t i = 0; i < order.size(); ++i) order[i] = i;
+  std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) {
+    const Chunk &x = p.prog[a], &y = p.prog[b];
+    return group(x) != group(y) ? group(x) < group(y) : x.acc % 4 < y.acc % 4;
+  });
+  int last_cond = -1;
+  for (size_t j = 0; j < order.size(); ++j) {
+    const Chunk& c = p.prog[order[j]];
+    const bool last_of_group = j + 1 == order.size() || group(p.prog[order[j + 1]]) != group(c);
+    const bool last_of_acc = last_of_group || p.prog[order[j + 1]].acc != c.acc;
+    for (int part = 0; part < (c.b_buf2 == B_NONE ? 1 : 2); ++part) {
+      const uint8_t buf = part ? c.b_buf2 : c.b_buf;
+      const bool last = c.b_buf2 == B_NONE || part == 1;
+      DevChunk r{};
+      r.src16 = (uint32_t)src[order[j]];
+      for (int cur = 0; cur < 2; ++cur) r.b_lo[cur] = (uint16_t)((base_of(buf, cur, c.phase) + c.k0 * 16) >> 4);
+      r.acc = (uint8_t)(c.acc % 4);
+      r.flags = (uint8_t)(((c.flags & F_FIRST) && part == 0 ? DF_FIRST : 0) | (buf == B_COND ? DF_B_COND : 0) | (c.nk == 1 ? DF_NK1 : 0) |
+                          (part == 1 ? DF_SAME_SLOT : 0) | (!last ? DF_KEEP_SLOT : 0) | (last && last_of_acc ? DF_ACC_END : 0) |
+                          (last && last_of_group ? DF_END : 0));
+      r.wait_b = c.wait_b;
+      r.phase_blk = (uint8_t)(c.phase | ((block >= 0 ? block : c.acc / 4) << 4));
+      if (buf == B_COND) last_cond = (int)d.size();
+      d.push_back(r);
     }
-    r.acc_phase = (uint8_t)(c.acc | (c.phase << 4));
-    r.flags = (uint8_t)(((c.flags & F_FIRST) ? DF_FIRST : 0) | ((c.flags & F_COND_RELEASE) ? DF_COND_RELEASE : 0) |
-                        (c.b_buf == B_COND ? DF_B_COND : 0) | (c.nk == 1 ? DF_NK1 : 0) | (c.b_buf2 != B_NONE ? DF_HAS_B2 : 0));
-    r.sync = (uint16_t)((c.wait_b & 7) | (c.wait_acc << 3) | (c.commit << 6) | ((c.wait_b >> 4) << 9));
-    r.pair = (uint16_t)(L.cps == 2 ? i / 2 : i);          // ring position within the step: pair index, or chunk index when a slot holds one chunk
-    d.mine[c.owner].push_back(r);
   }
+  if (last_cond >= 0) d[last_cond].flags |= DF_COND_RELEASE;
 }
 
 }  // namespace stream

@@ -1,4 +1,5 @@
-// wrnn_tc_common.cuh -- PTX wrappers and epilogue math shared by the tcgen05 engines (wrnn_tc.cu, wrnn_tcc.cu).
+// wrnn_tc_common.cuh -- PTX wrappers (wgmma, TMA, mbarrier) and epilogue math shared by the tensor-core engines
+// (wrnn_tc.cu, wrnn_stream.cu).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -13,28 +14,53 @@ namespace tc {
 // PTX wrappers
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  // SM100 shared-memory matrix descriptor: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48)
-  // layout_type [61,64) = 0 (SWIZZLE_NONE / interleaved 8x16B core matrices), K-major
-  return (uint64_t)((saddr >> 4) & 0x3fff) | ((uint64_t)((lbo >> 4) & 0x3fff) << 16) |
-         ((uint64_t)((sbo >> 4) & 0x3fff) << 32) | ((uint64_t)1 << 46);
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+  // SM90 shared-memory matrix descriptor: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | layout [62,64) = 0
+  // (no swizzle: 8-row x 16-byte core matrices, contiguous 128 B each), K-major.  LBO = byte distance of the two core
+  // matrices of one K = 16 step, SBO = byte distance of consecutive 8-row groups.
+  return (uint64_t)((saddr >> 4) & 0x3fff) | ((uint64_t)((lbo >> 4) & 0x3fff) << 16) | ((uint64_t)((sbo >> 4) & 0x3fff) << 32);
 }
-__device__ __forceinline__ uint32_t umma_idesc(int M, int N, int fmt) {
-  // c_format F32 [4,6)=1 | a_format [7,10) | b_format [10,13) | K-major A,B | N>>3 [17,23) | M>>4 [24,29)
-  return (1u << 4) | ((uint32_t)fmt << 7) | ((uint32_t)fmt << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
+
+// D[64, N] (+)= A[64, 16] * B[N, 16]^T, both operands K-major in shared memory, fp32 accumulators in registers
+// (m64nNk16 fragment: thread t of the warpgroup holds rows 16*(t/32) + (t%32)/4 (+8) and columns 8j + 2*(t%4) (+1)).
+// Executed by all 128 threads of a warpgroup; scale_d == 0 overwrites D.  FMT 0 = fp16, 1 = bf16 operands.
+template <int N, int FMT> __device__ __forceinline__ void wgmma_ss(float* d, uint64_t da, uint64_t db, uint32_t scale_d);
+template <> __device__ __forceinline__ void wgmma_ss<8, 0>(float* d, uint64_t da, uint64_t db, uint32_t s) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, 0, 0;\n\t}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "l"(da), "l"(db), "r"(s) : "memory");
 }
-// Executed by a WHOLE converged warp with warp-uniform operands; elect.sync predicates the instruction
-// onto one lane.  (Issuing from a `tid == k` branch makes ptxas wrap every UTCHMMA in an ELECT/BRA.U.ANY
-// loop: ~70 cycles per instruction instead of ~38, measured with tests/probes/umma_probe.cu.)
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p, e;\n\tsetp.ne.b32 p, %4, 0;\n\telect.sync _|e, 0xffffffff;\n\t"
-               "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-               :: "r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+template <> __device__ __forceinline__ void wgmma_ss<8, 1>(float* d, uint64_t da, uint64_t db, uint32_t s) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, 0, 0;\n\t}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "l"(da), "l"(db), "r"(s) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t mbar) {
-  asm volatile("{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t"
-               "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}\n" :: "r"(mbar) : "memory");
-}
+#define WRNN_WGMMA_N16(FMT, TY)                                                                                              \
+  template <> __device__ __forceinline__ void wgmma_ss<16, FMT>(float* d, uint64_t da, uint64_t db, uint32_t s) {          \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"                                                      \
+                 "wgmma.mma_async.sync.aligned.m64n16k16" TY " {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}\n" \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])           \
+                 : "l"(da), "l"(db), "r"(s) : "memory");                                                                     \
+  }
+#define WRNN_WGMMA_N32(FMT, TY)                                                                                              \
+  template <> __device__ __forceinline__ void wgmma_ss<32, FMT>(float* d, uint64_t da, uint64_t db, uint32_t s) {          \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"                                                      \
+                 "wgmma.mma_async.sync.aligned.m64n32k16" TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, "  \
+                 "%14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"                                                                 \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),          \
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])    \
+                 : "l"(da), "l"(db), "r"(s) : "memory");                                                                     \
+  }
+WRNN_WGMMA_N16(0, ".f32.f16.f16")
+WRNN_WGMMA_N16(1, ".f32.bf16.bf16")
+WRNN_WGMMA_N32(0, ".f32.f16.f16")
+WRNN_WGMMA_N32(1, ".f32.bf16.bf16")
+#undef WRNN_WGMMA_N16
+#undef WRNN_WGMMA_N32
+
 // TMA 1-D bulk copy global -> shared, completion counted in bytes on an mbarrier (whole warp, one lane elected)
 __device__ __forceinline__ void tma_bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t mbar) {
   asm volatile("{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t"
@@ -42,61 +68,9 @@ __device__ __forceinline__ void tma_bulk_g2s(uint32_t dst, const void* src, uint
                "@e cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n\t}\n"
                :: "r"(dst), "l"(src), "r"(bytes), "r"(mbar) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void proxy_fence_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void proxy_fence_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, float* v) {
-  uint32_t a, b, c, d;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "r"(taddr));
-  v[0] = __uint_as_float(a); v[1] = __uint_as_float(b); v[2] = __uint_as_float(c); v[3] = __uint_as_float(d);
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr));
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]) : "r"(taddr));
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t r[32];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31]) : "r"(taddr));
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void tmem_ldN(uint32_t taddr, float* v) {
-  if constexpr (N == 4) tmem_ld4(taddr, v);
-  else if constexpr (N == 8) tmem_ld8(taddr, v);
-  else if constexpr (N == 16) tmem_ld16(taddr, v);
-  else tmem_ld32(taddr, v);
-}
-// out[0 .. NC) = sum over the NW partial accumulators (column stride `wstride`) of NC columns at taddr.
-// One wide tcgen05.ld per partial (NL = NC rounded up to 4/8/16/32 columns; the surplus columns are ignored):
-// every tcgen05.ld instruction costs tens of cycles of issue on the critical path, so fewer and wider wins.
-template <int NC, int NW>
-__device__ __forceinline__ void tmem_ld_sum(uint32_t taddr, int wstride, float* out) {
-  constexpr int NL = NC <= 4 ? 4 : NC <= 8 ? 8 : NC <= 16 ? 16 : 32;
-  float part[NW][NL];
-#pragma unroll
-  for (int w = 0; w < NW; ++w) tmem_ldN<NL>(taddr + w * wstride, part[w]);
-  tmem_ld_wait();
-#pragma unroll
-  for (int i = 0; i < NC; ++i) {
-    float acc = part[0][i];
-#pragma unroll
-    for (int w = 1; w < NW; ++w) acc += part[w][i];
-    out[i] = acc;
-  }
-}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(bar) : "memory"); }
 __device__ __forceinline__ bool mbar_try(uint32_t bar, uint32_t parity) {
   uint32_t ok;
   asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"

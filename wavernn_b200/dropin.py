@@ -1,4 +1,4 @@
-"""Run an UNMODIFIED reference CLI (gen_wavernn.py, gen_tacotron.py, quick_start.py, train_wavernn.py) with the B200
+"""Run an UNMODIFIED reference CLI (gen_wavernn.py, gen_tacotron.py, quick_start.py, train_wavernn.py) with the H100
 vocoder underneath:
 
     cd /path/to/WaveRNN && python -m wavernn_b200.dropin gen_wavernn.py --file mel.npy --batched

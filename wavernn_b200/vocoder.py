@@ -1,7 +1,7 @@
 """Host side of the drop-in: a `WaveRNN` with the reference's constructor, state_dict
 layout and `generate(mels, save_path, batched, target, overlap, mu_law)` signature
 (reference models/fatchord_version.py:92-264), whose sample loop is the persistent
-sm_100a kernel behind include/wavernn_b200.h instead of ~43 PyTorch launches per
+sm_90a kernel behind include/wavernn_b200.h instead of ~43 PyTorch launches per
 sample.
 
 What stays in PyTorch (run once per call, as the reference does): the
@@ -145,7 +145,7 @@ class WaveRNN(nn.Module):
         self.num_params()
         self._flatten_parameters()
 
-        # ---- knobs of the B200 engine (not part of the reference surface) ----
+        # ---- knobs of the CUDA engine (not part of the reference surface) ----
         self.gen_rng = 'torch'          # 'torch' (reference-compatible CPU draws) | 'philox' (in-kernel)
         self.gen_precision = 'fp16'     # 'fp16' | 'bf16' tensor-core operands | 'fp32' strict SIMT mode
         self.gen_engine = 'auto'        # 'auto' | 'simt' | 'tcgen05' (weights stationary, lowest latency) | 'stream' (many folds)
@@ -213,7 +213,7 @@ class WaveRNN(nn.Module):
         device = next(self.parameters()).device
         if device.type != 'cuda':
             raise RuntimeError(
-                "wavernn_b200: WaveRNN.generate() runs only on a CUDA (sm_100a) device -- move the model with "
+                "wavernn_b200: WaveRNN.generate() runs only on a CUDA (sm_90a) device -- move the model with "
                 ".to('cuda'). There is deliberately no CPU fallback.")
         return device
 
