@@ -212,57 +212,12 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
       long long tp0 = 0;
       if (profiling) tp0 = clock64();
 
-      // draws for this step, fetched early so their latency hides under the step
-      float ur[11];
-#pragma unroll
-      for (int i = 0; i < 11; ++i) ur[i] = 0.5f;
-      float ex[4] = {1.f, 1.f, 1.f, 1.f};                 // RAW: Exp(1) draws of this CTA's 4 classes
-      if constexpr (RAW) {
-        if (owns_fold) {
-          if (p.expo) {
-            const float4 v = __ldg(reinterpret_cast<const float4*>(p.expo + ((size_t)t * p.n_total + p.f0 + fold) * NCLS + u0));
-            ex[0] = v.x; ex[1] = v.y; ex[2] = v.z; ex[3] = v.w;
-          } else {                                        // same keying as the SIMT engine: block 16 + class/4
-            const Philox4 r = philox4x32_10((unsigned)t, (unsigned)(p.seg_first + p.f0 + fold), 16u + (unsigned)cta,
-                                            (unsigned)p.offset, (unsigned)p.seed, (unsigned)(p.seed >> 32));
-            ex[0] = -logf(u01(r.x)); ex[1] = -logf(u01(r.y)); ex[2] = -logf(u01(r.z)); ex[3] = -logf(u01(r.w));
-          }
-        }
-      } else if (p.uniforms) {
-        if (p.uniforms_ready) {
-          // Streamed draws: rows land (DMA) while the kernel runs.  All 128 CTAs read the same row, so the loads must stay
-          // L1-cached (as L2 loads they cost 1 us per step: 27 k requests on a few hot lines, measured) -- which is safe
-          // only if no line is ever cached before all of it has landed: a row is >= 44 B, a 128 B line spans at most four
-          // rows, so row t is read once rows t .. t+3 are in (the host uploads in chunks of ~1000 rows: free).
-          const unsigned need = min((unsigned)S, (unsigned)t + 4u);
-          if (rows_known < need) rows_known = rows_wait(p.uniforms_ready, need, p.abort_flag);
-          if (owns_fold) {
-            const float* u = p.uniforms + (size_t)t * 11 * p.n_total;
-#pragma unroll
-            for (int i = 0; i < 10; ++i) ur[i] = __ldca(u + (p.f0 + fold) * 10 + i);
-            ur[10] = __ldca(u + 10 * p.n_total + p.f0 + fold);
-          }
-        } else if (owns_fold) {                            // resident draws: read-only path (11 values = 2 lines per fold)
-          const float* u = p.uniforms + (size_t)t * 11 * p.n_total;
-#pragma unroll
-          for (int i = 0; i < 10; ++i) ur[i] = __ldg(u + (p.f0 + fold) * 10 + i);
-          ur[10] = __ldg(u + 10 * p.n_total + p.f0 + fold);
-        }
-      } else if (owns_fold) {
-        {
-          const unsigned g = (unsigned)(p.seg_first + p.f0 + fold), k0 = (unsigned)p.seed, k1 = (unsigned)(p.seed >> 32), o0 = (unsigned)p.offset;
-          const Philox4 r0 = philox4x32_10((unsigned)t, g, 0u, o0, k0, k1), r1 = philox4x32_10((unsigned)t, g, 1u, o0, k0, k1),
-                        r2 = philox4x32_10((unsigned)t, g, 2u, o0, k0, k1);
-          ur[0] = u_ref_range(r0.x); ur[1] = u_ref_range(r0.y); ur[2] = u_ref_range(r0.z); ur[3] = u_ref_range(r0.w);
-          ur[4] = u_ref_range(r1.x); ur[5] = u_ref_range(r1.y); ur[6] = u_ref_range(r1.z); ur[7] = u_ref_range(r1.w);
-          ur[8] = u_ref_range(r2.x); ur[9] = u_ref_range(r2.y); ur[10] = u_ref_range(r2.z);
-        }
-      }
       float xf = 0.f;
       if (owns_fold && p.x_force && t > 0) xf = __ldg(p.x_force + (size_t)(t - 1) * p.n_total + p.f0 + fold);
 
       // ---- A: GRU1.  gi1 = pre_t (conditioning chain, D_Q) + x * v1 ; gh1 = W1h h1 + b1h (D_S1 of step t-1)
       float pre[32];                                      // this fold's 32 conditioning rows (+ qk + x*vq)
+      float gn[10], lu, lex[4];                           // sampler terms of this step's draws (MoL / RAW)
       {
         mbar_wait(bar_q, (uint32_t)(t & 1), p.abort_flag);           // pre_t is in the table
         if (p.x_force && t > 0) x = xf;
@@ -281,6 +236,62 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
         }
         publish(img_h1, hv);
         signal(0);
+        // This step's draws and everything computed from them alone, while the h1' exchange is in flight: at the top of
+        // the step or in the sampler they sit between x_{t-1} and the h1' publish, on the critical path of every step.
+        float ur[11];
+#pragma unroll
+        for (int i = 0; i < 11; ++i) ur[i] = 0.5f;
+        float ex[4] = {1.f, 1.f, 1.f, 1.f};                 // RAW: Exp(1) draws of this CTA's 4 classes
+        if constexpr (RAW) {
+          if (owns_fold) {
+            if (p.expo) {
+              const float4 v = __ldg(reinterpret_cast<const float4*>(p.expo + ((size_t)t * p.n_total + p.f0 + fold) * NCLS + u0));
+              ex[0] = v.x; ex[1] = v.y; ex[2] = v.z; ex[3] = v.w;
+            } else {                                        // same keying as the SIMT engine: block 16 + class/4
+              const Philox4 r = philox4x32_10((unsigned)t, (unsigned)(p.seg_first + p.f0 + fold), 16u + (unsigned)cta,
+                                              (unsigned)p.offset, (unsigned)p.seed, (unsigned)(p.seed >> 32));
+              ex[0] = -logf(u01(r.x)); ex[1] = -logf(u01(r.y)); ex[2] = -logf(u01(r.z)); ex[3] = -logf(u01(r.w));
+            }
+          }
+        } else if (p.uniforms) {
+          if (p.uniforms_ready) {
+            // Streamed draws: rows land (DMA) while the kernel runs.  All 128 CTAs read the same row, so the loads must stay
+            // L1-cached (as L2 loads they cost 1 us per step: 27 k requests on a few hot lines, measured) -- which is safe
+            // only if no line is ever cached before all of it has landed: a row is >= 44 B, a 128 B line spans at most four
+            // rows, so row t is read once rows t .. t+3 are in (the host uploads in chunks of ~1000 rows: free).
+            const unsigned need = min((unsigned)S, (unsigned)t + 4u);
+            if (rows_known < need) rows_known = rows_wait(p.uniforms_ready, need, p.abort_flag);
+            if (owns_fold) {
+              const float* u = p.uniforms + (size_t)t * 11 * p.n_total;
+#pragma unroll
+              for (int i = 0; i < 10; ++i) ur[i] = __ldca(u + (p.f0 + fold) * 10 + i);
+              ur[10] = __ldca(u + 10 * p.n_total + p.f0 + fold);
+            }
+          } else if (owns_fold) {                            // resident draws: read-only path (11 values = 2 lines per fold)
+            const float* u = p.uniforms + (size_t)t * 11 * p.n_total;
+#pragma unroll
+            for (int i = 0; i < 10; ++i) ur[i] = __ldg(u + (p.f0 + fold) * 10 + i);
+            ur[10] = __ldg(u + 10 * p.n_total + p.f0 + fold);
+          }
+        } else if (owns_fold) {
+          {
+            const unsigned g = (unsigned)(p.seg_first + p.f0 + fold), k0 = (unsigned)p.seed, k1 = (unsigned)(p.seed >> 32), o0 = (unsigned)p.offset;
+            const Philox4 r0 = philox4x32_10((unsigned)t, g, 0u, o0, k0, k1), r1 = philox4x32_10((unsigned)t, g, 1u, o0, k0, k1),
+                          r2 = philox4x32_10((unsigned)t, g, 2u, o0, k0, k1);
+            ur[0] = u_ref_range(r0.x); ur[1] = u_ref_range(r0.y); ur[2] = u_ref_range(r0.z); ur[3] = u_ref_range(r0.w);
+            ur[4] = u_ref_range(r1.x); ur[5] = u_ref_range(r1.y); ur[6] = u_ref_range(r1.z); ur[7] = u_ref_range(r1.w);
+            ur[8] = u_ref_range(r2.x); ur[9] = u_ref_range(r2.y); ur[10] = u_ref_range(r2.z);
+          }
+        }
+        if constexpr (RAW) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) { lex[i] = __logf(ex[i]); settle(lex[i]); }
+        } else {
+          mol_noise_fast(ur, gn, lu);
+#pragma unroll
+          for (int i = 0; i < 10; ++i) settle(gn[i]);
+          settle(lu);
+        }
       }
       if (profiling) { const long long c = clock64(); tprof[0] += c - tp0; tp0 = c; }
 
@@ -337,7 +348,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
         acc_rd(AC_F3, 30, lg);
 #pragma unroll
         for (int i = 0; i < 30; ++i) lg[i] += b3[i];
-        x = mol_sample_fast(lg, ur);
+        x = mol_sample_noise(lg, gn, lu);
         if (owns_fold && cta == 0) {
           p.out[(size_t)(p.f0 + fold) * p.out_pitch + t] = x;
           if (p.logits_out) {
@@ -353,7 +364,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           lg[i] += b3[i];
-          const float sc = lg[i] - __logf(ex[i]);
+          const float sc = lg[i] - lex[i];
           if (sc > best) { best = sc; bestk = u0 + i; }
         }
         unsigned char* cand_out = p.xch5 + (size_t)par * cand_bytes;

@@ -138,23 +138,37 @@ __device__ __forceinline__ float gru_unit_fast(float gi_r, float gi_z, float gi_
   const float n = fast_tanh(gi_n + r * gh_n);
   return (1.0f - z) * n + z * h;
 }
-// utils/distribution.py:99-121 on SFU logs/exp
-__device__ __forceinline__ float mol_sample_fast(const float* lg, const float* u) {
+// utils/distribution.py:99-121 on SFU logs/exp, split at the draws: mol_noise_fast needs only the uniforms u
+// (the Gumbel terms log(-log u_k) of :107 and the logistic term log(u) - log(1 - u) of :119), so a caller can compute it
+// off its critical path; mol_sample_noise then finishes the sample from the logits.
+__device__ __forceinline__ void mol_noise_fast(const float* u, float* gn, float& lu) {
+#pragma unroll
+  for (int k = 0; k < 10; ++k) gn[k] = __logf(-__logf(u[k]));
+  lu = __logf(u[10]) - __logf(1.0f - u[10]);
+}
+__device__ __forceinline__ float mol_sample_noise(const float* lg, const float* gn, float lu) {
   int best = 0;
   float bestv = -INFINITY;
 #pragma unroll
   for (int k = 0; k < 10; ++k) {
-    const float g = lg[k] - __logf(-__logf(u[k]));
+    const float g = lg[k] - gn[k];
     if (g > bestv) { bestv = g; best = k; }
   }
   float mean = lg[10], ls = lg[20];
 #pragma unroll
   for (int k = 1; k < 10; ++k) { if (best == k) { mean = lg[10 + k]; ls = lg[20 + k]; } }
   ls = fmaxf(ls, -32.23619130191664f);
-  const float x = mean + __expf(ls) * (__logf(u[10]) - __logf(1.0f - u[10]));
+  const float x = mean + __expf(ls) * lu;
   return fminf(fmaxf(x, -1.0f), 1.0f);
 }
-
+__device__ __forceinline__ float mol_sample_fast(const float* lg, const float* u) {
+  float gn[10], lu;
+  mol_noise_fast(u, gn, lu);
+  return mol_sample_noise(lg, gn, lu);
+}
+// Pins the computation of v before the next volatile asm (an mbarrier wait, say): the compiler may otherwise sink
+// arithmetic that depends on nothing but its inputs down to where its result is used.
+__device__ __forceinline__ void settle(float v) { asm volatile("" :: "f"(v)); }
 
 // K-major no-swizzle operand image (host side): element (r, k) at (r/8)*(K/8)*64 + (k/8)*64 + (r%8)*8 + k%8
 inline size_t img_index(int r, int k, int K) { return (size_t)(r / 8) * (K / 8) * 64 + (size_t)(k / 8) * 64 + (r % 8) * 8 + (k % 8); }
