@@ -95,9 +95,14 @@ __device__ __forceinline__ Philox4 philox4x32_10(unsigned c0, unsigned c1, unsig
   }
   return Philox4{c0, c1, c2, c3};
 }
-// 24 random bits -> open interval (0,1)
+// 24 random bits -> [2^-25, 1].  Closed at 1: above 2^23 the float sum (m + 0.5f) rounds to nearest even, so
+// x >> 8 == 0xffffff gives exactly 1.0f (once per 2^24 words).
 __device__ __forceinline__ float u01(unsigned x) { return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f); }
-// the reference's uniform_(1e-5, 1 - 1e-5): rand*(to-from)+from
+// u01 clamped into the open interval (0, 1): the RAW head's Exp(1) draws -logf(u) must be > 0 (at u = 1 they were -0.0,
+// which forced the class in the persistent engine and excluded it in the SIMT engine).  Every other word maps as u01.
+__device__ __forceinline__ float u01_open(unsigned x) { return fminf(u01(x), 0x1.fffffep-1f); }
+// the reference's uniform_(1e-5, 1 - 1e-5): rand*(to-from)+from, contracted to one FFMA.  u01 = 1 maps to
+// 1 - 1e-5 (rounded), inside the reference's range, so the MoL draws keep the closed u01.
 __device__ __forceinline__ float u_ref_range(unsigned x) { return u01(x) * (1.0f - 2e-5f) + 1e-5f; }
 
 // -------------------------------------------------------------------------------------

@@ -334,7 +334,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_simt_kernel(const SimtParams p) {
               const Philox4 r = philox4x32_10((unsigned)t, (unsigned)(p.seg_first + b), 16u + (unsigned)(i >> 2),
                                               (unsigned)p.offset, (unsigned)p.seed, (unsigned)(p.seed >> 32));
               const unsigned rv[4] = {r.x, r.y, r.z, r.w};
-              e = -logf(u01(rv[i & 3]));
+              e = -logf(u01_open(rv[i & 3]));
             }
             const float q = pr / e;
             if (q > bestq) { bestq = q; besti = i; }

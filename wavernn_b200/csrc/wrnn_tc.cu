@@ -250,7 +250,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
             } else {                                        // same keying as the SIMT engine: block 16 + class/4
               const Philox4 r = philox4x32_10((unsigned)t, (unsigned)(p.seg_first + p.f0 + fold), 16u + (unsigned)cta,
                                               (unsigned)p.offset, (unsigned)p.seed, (unsigned)(p.seed >> 32));
-              ex[0] = -logf(u01(r.x)); ex[1] = -logf(u01(r.y)); ex[2] = -logf(u01(r.z)); ex[3] = -logf(u01(r.w));
+              ex[0] = -logf(u01_open(r.x)); ex[1] = -logf(u01_open(r.y)); ex[2] = -logf(u01_open(r.z)); ex[3] = -logf(u01_open(r.w));
             }
           }
         } else if (p.uniforms) {
