@@ -53,7 +53,8 @@ enum { WRNN_PREC_F16 = 0, WRNN_PREC_FP32 = 1, WRNN_PREC_BF16 = 2 };
  *   TCGEN05: weights stationary in the shared memory of 128 SMs, activations exchanged through L2 -- lowest latency
  *            per step, tiles of <= 64 folds one after the other (BASELINE configs[1], [2]);
  *   STREAM : activations stationary (one CTA per 16/32 folds, any number of CTAs), weights streamed from L2 every
- *            step -- highest throughput for jobs with hundreds of folds (configs[3], [4]); MoL head;
+ *            step -- highest throughput for jobs with hundreds of folds (configs[3], [4]); MoL head (30 classes) and
+ *            9-bit RAW head (512 classes); AUTO routes only MoL jobs here;
  *   SIMT   : CUDA-core engine, the only one with strict fp32 arithmetic.                                       */
 enum { WRNN_ENGINE_AUTO = 0, WRNN_ENGINE_SIMT = 1, WRNN_ENGINE_TCGEN05 = 2, WRNN_ENGINE_STREAM = 3 };
 

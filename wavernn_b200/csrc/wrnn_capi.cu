@@ -239,13 +239,20 @@ int wrnn_expand_conditioning(const float* mel_frames, const float* aux_frames, c
 }
 
 // Test hook (CPU-only, no device needed): the stream engine's packed weight stream and step program for host-resident
-// weights, so the packing and the schedule can be interpreted and checked without a GPU (tests/test_stream_plan.py).
-// Call with blob == NULL to obtain the sizes.  Not part of the reference-facing surface.
+// weights, so the packing and the schedule can be interpreted and checked without a GPU (tests/test_stream_plan.py,
+// tests/test_stream_plan_raw.py).  cfg->mode selects the head: the MoL plan (n_classes <= 128) or the RAW plan
+// (n_classes == 512).  Call with blob == NULL to obtain the sizes.  Not part of the reference-facing surface.
 int wrnn_debug_stream_plan(const wrnn_cfg* cfg, const wrnn_weights* w, uint8_t* blob, uint64_t* blob_bytes, uint8_t* prog,
-                           uint64_t* n_chunks, float* vectors /* qk[4096] vq[4096] b1h[1536] b2h[1536] b3[128] */,
+                           uint64_t* n_chunks,
+                           float* vectors /* qk[4096] vq[4096] b1h[1536] b2h[1536] b3[n_classes padded to a multiple of 128:
+                                             128 for MoL, 512 for RAW] */,
                            uint16_t* mine /* [4][n_chunks]: per issuing warp, its chunk indices; unused tail = 0xffff */,
                            int32_t only_block /* -1: the whole program; 0..3: the share of that rank of a 4-CTA cluster */) {
   if (!cfg || !w || !blob_bytes || !n_chunks) { set_error("null argument"); return WRNN_E_INVALID; }
+  if (cfg->mode == WRNN_MODE_RAW ? cfg->n_classes != 512 : (cfg->n_classes <= 0 || cfg->n_classes > stream::MROWS)) {
+    set_error("stream plan: the MoL head needs n_classes <= 128, the RAW head n_classes == 512");
+    return WRNN_E_INVALID;
+  }
   HostWeights hw;
   hw.n_classes = cfg->n_classes;
   const size_t W2W = H + AUXD;
@@ -269,7 +276,7 @@ int wrnn_debug_stream_plan(const wrnn_cfg* cfg, const wrnn_weights* w, uint8_t* 
     std::memcpy(v, plan.vq.data(), 8 * H * 4); v += 8 * H;
     std::memcpy(v, plan.b1h.data(), G3 * 4); v += G3;
     std::memcpy(v, plan.b2h.data(), G3 * 4); v += G3;
-    std::memcpy(v, plan.b3.data(), stream::MROWS * 4);
+    std::memcpy(v, plan.b3.data(), plan.b3.size() * 4);
     if (mine) {
       std::memset(mine, 0xff, sizeof(uint16_t) * stream::N_ISSUERS * plan.prog.size());
       for (int o = 0; o < stream::N_ISSUERS; ++o) std::memcpy(mine + (size_t)o * plan.prog.size(), plan.mine[o].data(), plan.mine[o].size() * sizeof(uint16_t));

@@ -22,8 +22,9 @@
 //   warp 9     staging   : conditioning row of step t+1 for the NF folds (stream or frame-rate form) -> fp16 image
 //
 // Cluster form (template CL = 4; jobs whose clusters are co-resident): a tile belongs to a thread-block cluster of four
-// CTAs.  CTA r runs the program of unit block r of every layer (a quarter of the weight stream and of the MMAs; fc3 +
-// sampling in rank 0, which hands the sample to its peers), keeps all four K = 512 operand images, and pushes the block
+// CTAs.  CTA r runs the program of unit block r of every layer (a quarter of the weight stream and of the MMAs; MoL:
+// fc3 + sampling in rank 0, which hands the sample to its peers; RAW: fc3 block r in rank r, whose best (score, class)
+// goes into every rank's candidate table, and every rank reduces the four), keeps all four K = 512 operand images, and pushes the block
 // it has just computed into the peers' images with cp.async.bulk.shared::cluster.shared::cta (complete_tx on the PEER's
 // readiness barrier, arrive.expect_tx by the sender), so that a peer's block arrives exactly like a TMA load.  Same MMAs
 // in the same order: results are bit-identical to the one-CTA form.
@@ -54,7 +55,10 @@ constexpr int SBO_H = (H / 8) * 128;         // 8192: same for the K = 512 image
 constexpr int NBAR = 48;
 constexpr int MAX_STAGES = 9;               // ring slots (one chunk each)
 
-template <int NF> struct Smem {
+// RAW: the 9-bit head's classes (fc3 in four unit blocks of 128)
+constexpr int NCLS_RAW = 512;
+
+template <int NF, bool RAW = false> struct Smem {
   static constexpr int GROUPS = NF / 8;
   static constexpr int ACT = GROUPS * SBO_H;                 // one K = 512 activation image
   static constexpr int COND = GROUPS * SBO_Q;                // one conditioning image
@@ -65,22 +69,29 @@ template <int NF> struct Smem {
   static constexpr int OFF_RING = (OFF_COND + 2 * COND + 1023) / 1024 * 1024;
   static constexpr int SLOT_BYTES = CHUNK_BYTES;
   static constexpr int LOGP = 33;                                            // padded row of the logits transpose (conflict-free both ways)
-  static constexpr int MISC = LOGP * NF * 4 + NF * 4 + NBAR * 8 + 64 + 256;  // logits transpose, x, barriers, flags, zero block
+  // RAW, cluster form: [4 ranks][NF] (score, class) candidates of the step, written by every rank into every rank
+  static constexpr int CAND = RAW ? 4 * NF * 8 : 0;
+  static constexpr int MISC = LOGP * NF * 4 + NF * 4 + NBAR * 8 + 64 + 256 + CAND;  // logits transpose, x, barriers, flags, zero block
   static constexpr int STAGES = (227 * 1024 - OFF_RING - MISC) / SLOT_BYTES > MAX_STAGES ? MAX_STAGES : (227 * 1024 - OFF_RING - MISC) / SLOT_BYTES;
-  static constexpr int OFF_LOG = OFF_RING + STAGES * SLOT_BYTES;             // [NF][LOGP] fp32
+  static constexpr int OFF_LOG = OFF_RING + STAGES * SLOT_BYTES;             // [NF][LOGP] fp32 (RAW: [2][8 warps][NF] candidates)
   static constexpr int OFF_XS = OFF_LOG + LOGP * NF * 4;                       // [NF] fp32: previous sample per fold
   static constexpr int OFF_BAR = OFF_XS + NF * 4;
   static constexpr int OFF_ZERO = OFF_BAR + NBAR * 8 + 64;                  // 256 B of zeros: B operand of padding MMAs
-  static constexpr int BYTES = OFF_ZERO + 256;
+  static constexpr int OFF_CAND = OFF_ZERO + 256;
+  static constexpr int BYTES = OFF_CAND + CAND;
   static_assert(STAGES >= 3, "ring too shallow");
   static_assert(BYTES <= 227 * 1024, "shared memory budget");
+  static_assert(2 * 8 * NF * 8 <= LOGP * NF * 4, "RAW: the per-warp candidates of two blocks fit the logits transpose");
 };
+// the RAW head's candidate tables take shared memory the ring could not use anyway: as many ring slots as MoL
+static_assert(Smem<16, true>::STAGES == Smem<16>::STAGES && Smem<32, true>::STAGES == Smem<32>::STAGES, "RAW ring depth");
 // barrier indices
 constexpr int BAR_FULL = 0, BAR_EMPTY = MAX_STAGES,
               BAR_READY = 2 * MAX_STAGES /* + {0, 1: cond[parity]; 2..5: h1' block b; 6..9: h2' block b; 10..13: y1 block b; 14..17: y2 block b} */,
               BAR_COND_FREE = BAR_READY + 18;
 constexpr int BAR_X = BAR_COND_FREE + 2;    // cluster form: "the sample of this step has been written into this CTA's x_s"
-static_assert(BAR_X + 1 <= NBAR, "barrier table");
+constexpr int BAR_CAND = BAR_X + 1;         // RAW cluster form: "every rank's candidates of this step are in this CTA's table"
+static_assert(BAR_CAND + 1 <= NBAR, "barrier table");
 
 struct StreamParams {
   // per cluster rank (one-CTA form: rank 0 only): the weight stream and the chunk list of one step
@@ -95,6 +106,7 @@ struct StreamParams {
   float* state;                 // [tiles][2][H][NF] fp32 hidden state
   int* abort_flag;
   long long* prof;              // optional cycle counters of CTA 0
+  const float* expo;            // RAW: optional explicit Exp(1) draws [steps][n_total][512] (else Philox)
 };
 
 __device__ __forceinline__ uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
@@ -105,9 +117,9 @@ __device__ __forceinline__ uint32_t map_to_rank(uint32_t addr, uint32_t rank) {
   uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank)); return r;
 }
 
-template <int NF, int FMT, bool FRAMES, bool PROF, int CL>
+template <int NF, int FMT, bool FRAMES, bool PROF, int CL, bool RAW>
 __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p) {
-  using SM = Smem<NF>;
+  using SM = Smem<NF, RAW>;
   extern __shared__ __align__(1024) unsigned char smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM::OFF_BAR);
   volatile int* s_abort = reinterpret_cast<volatile int*>(smem + SM::OFF_BAR + NBAR * 8 + 16);   // CTA-local copy of the abort flag
@@ -146,6 +158,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 8;" :: "r"(bar(BAR_COND_FREE + 0)));
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 8;" :: "r"(bar(BAR_COND_FREE + 1)));
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar(BAR_X)));
+    if constexpr (RAW) asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(bar(BAR_CAND)), "r"((uint32_t)CL));   // one arrival per rank
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   proxy_fence_smem();
@@ -282,7 +295,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
         named_bar_sync(2, N_CONSUMERS);                        // every consumer thread's stores (and proxy fences) are done
         if (lane == 0 && warp >= 1 && warp <= 3) {
           const uint32_t peer = (uint32_t)((rank + warp) & 3);
-          if (kind != W_Y2 || peer == 0u) {
+          if (RAW || kind != W_Y2 || peer == 0u) {              // y2: MoL's fc3 runs in rank 0 only, RAW's in every rank
             const uint32_t rb = map_to_rank(b, peer);
             asm volatile("mbarrier.arrive.expect_tx.relaxed.cluster.shared::cluster.b64 _, [%0], %1;" :: "r"(rb), "r"((uint32_t)(NF * 256)) : "memory");
 #pragma unroll
@@ -312,11 +325,11 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
 #pragma unroll
       for (int i = 0; i < 11; ++i) ur[i] = 0.5f;
       const bool sampler = rank == 0 && tid < B;
-      if (p.uniforms && rank == 0 && warp == 0) {              // streamed draws: read row t once rows t .. t+3 have landed (see wrnn_tc.cu)
+      if (!RAW && p.uniforms && rank == 0 && warp == 0) {      // streamed draws: read row t once rows t .. t+3 have landed (see wrnn_tc.cu)
         const unsigned need = min((unsigned)S, (unsigned)t + 4u);
         if (rows_known < need) rows_known = rows_wait(p.uniforms_ready, need, p.abort_flag);
       }
-      if (sampler) {
+      if (!RAW && sampler) {                                   // (RAW: the fc3 epilogue draws per class)
         const int gf = f0 + tid;
         if (p.uniforms) {
           const float* u = p.uniforms + (size_t)t * 11 * p.n_total;
@@ -332,6 +345,11 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
           ur[8] = u_ref_range(r2.x); ur[9] = u_ref_range(r2.y); ur[10] = u_ref_range(r2.z);
         }
       }
+
+      // RAW, one-CTA form: the best (score, class) of fold `lane` over the fc3 blocks done so far (warp 0, lanes < NF)
+      float run_best = -INFINITY;
+      int run_k = 0x7fffffff;
+      auto better = [](float s, int k, float bs, int bk) { return s > bs || (s == bs && k < bk); };   // ties: lowest class
 
       // ---- epilogue of one (phase, block) group: accumulators -> gates / relu / logits -----------------------------------
       auto epilogue = [&](int phase, int blk) {
@@ -385,6 +403,104 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
             }
           }
           publish_ready(phase == 2 ? W_Y1 : W_Y2, blk, phase == 2 ? off_y1 : off_y2);
+        } else if constexpr (RAW) {
+          // P5, RAW head, classes [128 blk, 128 blk + 128): logit = F3 y2 + b3, score = logit - log e with e the class's
+          // Exp(1) draw (Philox keyed as wrnn_tc.cu / wrnn_simt.cu: block 16 + class / 4, word class % 4; or `expo`);
+          // the pick is the best score, ties to the lowest class.  This thread holds rows rw, rw + 8 of folds 8j + fc (+1):
+          // two words of two different Philox blocks per fold, each block computed for the one word it gives.
+          uint2* cw = reinterpret_cast<uint2*>(smem + SM::OFF_LOG) + (blk & 1) * 8 * NF;      // [warp][fold] best of the warp's 16 rows
+          const unsigned k0 = (unsigned)p.seed, k1 = (unsigned)(p.seed >> 32), o0 = (unsigned)p.offset;
+#pragma unroll
+          for (int j = 0; j < NF / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int f = 8 * j + fc + e;
+              const size_t row_out = ((size_t)t * p.n_total + f0 + f) * NCLS_RAW;
+              float best = 0.f;
+              int bk = 0;
+#pragma unroll
+              for (int hr = 0; hr < 2; ++hr) {
+                const int i = 4 * j + 2 * hr + e, k = blk * MROWS + rw + 8 * hr;
+                const float lg = ((acc[0][i] + acc[1][i]) + (acc[2][i] + acc[3][i])) + __ldg(p.b3 + k);
+                float ex = 1.f;
+                if (f < B) {
+                  if (p.expo) {
+                    ex = __ldg(p.expo + row_out + k);
+                  } else {
+                    const Philox4 r = philox4x32_10((unsigned)t, (unsigned)(p.seg_first + f0 + f), 16u + (unsigned)(k >> 2), o0, k0, k1);
+                    const unsigned w = (k & 3) == 0 ? r.x : (k & 3) == 1 ? r.y : (k & 3) == 2 ? r.z : r.w;
+                    ex = -logf(u01_open(w));
+                  }
+                  if (p.logits_out) p.logits_out[row_out + k] = lg;
+                }
+                const float sc = lg - __logf(ex);
+                if (hr == 0 || better(sc, k, best, bk)) { best = sc; bk = k; }
+              }
+              // the warp's 8 row groups (lanes 4, 8, 16 apart)
+#pragma unroll
+              for (int m = 4; m < 32; m <<= 1) {
+                const float ob = __shfl_xor_sync(0xffffffffu, best, m);
+                const int ok = __shfl_xor_sync(0xffffffffu, bk, m);
+                if (better(ob, ok, best, bk)) { best = ob; bk = ok; }
+              }
+              if (lane < 4) cw[warp * NF + f] = make_uint2(__float_as_uint(best), (unsigned)bk);
+            }
+          }
+          named_bar_sync(3, N_CONSUMERS);                      // every warp's candidates of this block are in cw
+          if (warp == 0) {
+            float bs = -INFINITY;
+            int bk = 0x7fffffff;
+            if (lane < NF) {
+#pragma unroll
+              for (int w = 0; w < 8; ++w) {                    // warps in ascending class order
+                const uint2 v = cw[w * NF + lane];
+                if (better(__uint_as_float(v.x), (int)v.y, bs, bk)) { bs = __uint_as_float(v.x); bk = (int)v.y; }
+              }
+            }
+            bool done = false;
+            if constexpr (CL == 1) {
+              if (better(bs, bk, run_best, run_k)) { run_best = bs; run_k = bk; }
+              bs = run_best; bk = run_k;
+              done = blk == NCLS_RAW / MROWS - 1;
+            } else {
+              // this rank's candidate into slot `rank` of every rank's table, then a release at cluster scope on every
+              // rank's candidate barrier; every rank then reduces the same four candidates the same way
+              uint2* ct = reinterpret_cast<uint2*>(smem + SM::OFF_CAND);                        // [rank][fold]
+              if (lane < NF) {
+                const uint32_t a = smem_u32(ct + rank * NF + lane);
+#pragma unroll
+                for (int r = 0; r < CL; ++r)
+                  asm volatile("st.shared::cluster.v2.u32 [%0], {%1, %2};" :: "r"(map_to_rank(a, (uint32_t)r)), "r"(__float_as_uint(bs)), "r"((uint32_t)bk) : "memory");
+              }
+              __syncwarp();
+              if (lane == 0) {
+#pragma unroll
+                for (int r = 0; r < CL; ++r)
+                  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" :: "r"(map_to_rank(bar(BAR_CAND), (uint32_t)r)) : "memory");
+                wait_peer(bar(BAR_CAND), (uint32_t)t & 1);
+              }
+              __syncwarp();
+              bs = -INFINITY; bk = 0x7fffffff;
+              if (lane < NF) {
+#pragma unroll
+                for (int r = 0; r < CL; ++r) {
+                  const uint2 v = ct[r * NF + lane];
+                  if (better(__uint_as_float(v.x), (int)v.y, bs, bk)) { bs = __uint_as_float(v.x); bk = (int)v.y; }
+                }
+              }
+              done = true;
+            }
+            if (done && lane < NF) {
+              float xnew = 0.f;
+              if (lane < B) {
+                const int gf = f0 + lane;
+                xnew = 2.0f * (float)bk / ((float)NCLS_RAW - 1.0f) - 1.0f;          // reference :235
+                if (rank == 0) p.out[(size_t)gf * p.out_pitch + t] = xnew;
+                if (p.x_force) xnew = __ldg(p.x_force + (size_t)t * p.n_total + gf);
+              }
+              x_s[lane] = xnew;                                // read after the end-of-step barrier
+            }
+          }
         } else {                                               // P5 (rank 0): logits -> transpose -> one thread per fold samples
           if (wg == 0 && rw < 32) {
 #pragma unroll
@@ -502,7 +618,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
       // x of this step has landed here (cluster form: rank 0's remote stores, released at cluster scope).  One thread
       // acquires -- every poll of an acquire.cluster wait invalidates L1 --, the named barrier below hands it on.
       if (tid == 0) {
-        if constexpr (CL > 1) wait_peer(bar(BAR_X), (uint32_t)t & 1);
+        if constexpr (CL > 1 && !RAW) wait_peer(bar(BAR_X), (uint32_t)t & 1);   // (RAW: every rank computed x itself)
         *ep_stop = *s_abort;
       }
       named_bar_sync(1, N_CONSUMERS);                          // x of this step (and the stop decision) visible to all consumers
@@ -532,15 +648,20 @@ class StreamEngine : public Engine {
   }
   int grid_ctas() const override { return last_grid_; }
 
+  template <int NF, int CL, bool PROF, bool RAW> const void* kernel_r(bool frames) const {
+    if (cfg.precision == WRNN_PREC_BF16) return frames ? (const void*)wrnn_stream_kernel<NF, 1, true, PROF, CL, RAW> : (const void*)wrnn_stream_kernel<NF, 1, false, PROF, CL, RAW>;
+    return frames ? (const void*)wrnn_stream_kernel<NF, 0, true, PROF, CL, RAW> : (const void*)wrnn_stream_kernel<NF, 0, false, PROF, CL, RAW>;
+  }
   template <int NF, int CL, bool PROF> const void* kernel_p(bool frames) const {
-    if (cfg.precision == WRNN_PREC_BF16) return frames ? (const void*)wrnn_stream_kernel<NF, 1, true, PROF, CL> : (const void*)wrnn_stream_kernel<NF, 1, false, PROF, CL>;
-    return frames ? (const void*)wrnn_stream_kernel<NF, 0, true, PROF, CL> : (const void*)wrnn_stream_kernel<NF, 0, false, PROF, CL>;
+    return raw() ? kernel_r<NF, CL, PROF, true>(frames) : kernel_r<NF, CL, PROF, false>(frames);
   }
   template <int NF, int CL> const void* kernel_nf(bool frames, bool prof) const { return prof ? kernel_p<NF, CL, true>(frames) : kernel_p<NF, CL, false>(frames); }
   template <int NF> static SmemLayout layout() {
     using S = Smem<NF>;
     return SmemLayout{S::OFF_X0, S::OFF_X1, {S::OFF_H2, S::OFF_H2B}, S::OFF_COND, S::COND};
   }
+  bool raw() const { return cfg.mode == WRNN_MODE_RAW; }
+  template <int NF> int smem_bytes() const { return raw() ? Smem<NF, true>::BYTES : Smem<NF>::BYTES; }
 
   // one (cluster size, folds per CTA) combination: its weight streams (one per cluster rank) and device programs
   struct Variant {
@@ -574,10 +695,10 @@ class StreamEngine : public Engine {
     for (int r = 0; r < 4; ++r) build_plan(w, bf, split[r], r);
     n_chunks_ = (int)whole[0].prog.size(); n_mma_ = whole[0].n_mma;
     int rc;
-    var_[0].nf = 16; var_[0].cl = 1; var_[0].smem = Smem<16>::BYTES; if ((rc = upload(var_[0], whole, layout<16>())) != WRNN_OK) return rc;
-    var_[1].nf = 32; var_[1].cl = 1; var_[1].smem = Smem<32>::BYTES; if ((rc = upload(var_[1], whole, layout<32>())) != WRNN_OK) return rc;
-    var_[2].nf = 16; var_[2].cl = 4; var_[2].smem = Smem<16>::BYTES; if ((rc = upload(var_[2], split, layout<16>())) != WRNN_OK) return rc;
-    var_[3].nf = 32; var_[3].cl = 4; var_[3].smem = Smem<32>::BYTES; if ((rc = upload(var_[3], split, layout<32>())) != WRNN_OK) return rc;
+    var_[0].nf = 16; var_[0].cl = 1; var_[0].smem = smem_bytes<16>(); if ((rc = upload(var_[0], whole, layout<16>())) != WRNN_OK) return rc;
+    var_[1].nf = 32; var_[1].cl = 1; var_[1].smem = smem_bytes<32>(); if ((rc = upload(var_[1], whole, layout<32>())) != WRNN_OK) return rc;
+    var_[2].nf = 16; var_[2].cl = 4; var_[2].smem = smem_bytes<16>(); if ((rc = upload(var_[2], split, layout<16>())) != WRNN_OK) return rc;
+    var_[3].nf = 32; var_[3].cl = 4; var_[3].smem = smem_bytes<32>(); if ((rc = upload(var_[3], split, layout<32>())) != WRNN_OK) return rc;
     const Plan& plan = whole[0];
     std::vector<float> vec;
     off_qk_ = 0; vec.insert(vec.end(), plan.qk.begin(), plan.qk.end());
@@ -591,16 +712,16 @@ class StreamEngine : public Engine {
     WRNN_CUDA_OK(cudaMemset(d_sync_, 0, 256));
     for (int k = 0; k < 4; ++k) {
       const bool fr = (k & 1) != 0, pr = (k & 2) != 0;
-      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<16, 1>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<16>::BYTES));
-      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<32, 1>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<32>::BYTES));
-      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<16, 4>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<16>::BYTES));
-      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<32, 4>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, Smem<32>::BYTES));
+      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<16, 1>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<16>()));
+      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<32, 1>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<32>()));
+      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<16, 4>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<16>()));
+      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<32, 4>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<32>()));
     }
     WRNN_CUDA_OK(cudaDeviceGetAttribute(&n_sm_, cudaDevAttrMultiProcessorCount, device));
     // clusters of four that fit the device at once (GPC granularity); both tile sizes use the same shared memory class
     {
       cudaLaunchConfig_t lc{};
-      lc.gridDim = dim3(4 * n_sm_); lc.blockDim = dim3(NT); lc.dynamicSmemBytes = Smem<32>::BYTES;
+      lc.gridDim = dim3(4 * n_sm_); lc.blockDim = dim3(NT); lc.dynamicSmemBytes = smem_bytes<32>();
       cudaLaunchAttribute at[1];
       at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 4; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
       lc.attrs = at; lc.numAttrs = 1;
@@ -612,9 +733,12 @@ class StreamEngine : public Engine {
   }
 
   static bool supports_cfg(const wrnn_cfg& c) {
-    return c.precision != WRNN_PREC_FP32 && c.mode == WRNN_MODE_MOL && c.n_classes == 30;
+    return c.precision != WRNN_PREC_FP32 && ((c.mode == WRNN_MODE_MOL && c.n_classes == 30) || (c.mode == WRNN_MODE_RAW && c.n_classes == NCLS_RAW));
   }
-  bool supports(const wrnn_job& job) const override { return job.expo == nullptr && !(job.mel_frames && job.cond_mode == WRNN_COND_EXPAND && job.fold_row0); }
+  // explicit Exp(1) draws (`expo`) belong to the RAW head; streamed uniforms (`uniforms_ready`) are MoL draws and unused by it
+  bool supports(const wrnn_job& job) const override {
+    return (raw() || job.expo == nullptr) && !(job.mel_frames && job.cond_mode == WRNN_COND_EXPAND && job.fold_row0);
+  }
 
   // Which form serves n folds:
   //   one CTA per tile : 16 folds per CTA while the tiles fit one wave (one tile per SM), 32 folds per CTA beyond
@@ -653,7 +777,7 @@ class StreamEngine : public Engine {
     p.mels_up = job.mels_up; p.aux = job.aux; p.L = job.L; p.seg_stride = job.seg_stride; p.row_base = 0;
     p.n_total = job.n_seg; p.steps = job.steps > 0 ? job.steps : job.seg_len; p.out_pitch = p.steps; p.seg_first = job.seg_first;
     p.uniforms = job.uniforms; p.uniforms_ready = job.uniforms_ready; p.seed = job.philox_seed; p.offset = job.philox_offset;
-    p.out = job.out; p.x_force = job.x_force; p.logits_out = job.logits_out;
+    p.out = job.out; p.x_force = job.x_force; p.logits_out = job.logits_out; p.expo = raw() ? job.expo : nullptr;
     p.fold_row0 = reinterpret_cast<const long long*>(job.fold_row0); p.fold_row_end = reinterpret_cast<const long long*>(job.fold_row_end);
     p.mel_frames = job.mel_frames; p.aux_frames = job.aux_frames; p.up_taps = job.up_taps; p.hop = job.hop;
     p.state = static_cast<float*>(d_state_);
@@ -703,7 +827,7 @@ class StreamEngine : public Engine {
 
 int make_stream_engine(const wrnn_cfg& cfg, const HostWeights& w, int device, Engine** out) {
   if (!StreamEngine::supports_cfg(cfg)) {
-    set_error("stream engine serves the MoL head (30 classes) with fp16/bf16 operands");
+    set_error("stream engine serves the MoL head (30 classes) and the 9-bit RAW head (512 classes) with fp16/bf16 operands");
     return WRNN_E_INVALID;
   }
   StreamEngine* e = new StreamEngine();

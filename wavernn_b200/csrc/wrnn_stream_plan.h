@@ -17,7 +17,7 @@
 //   P2 GRU2 :  acc r,z = Q2[g,b] cond + W2h[g,b] h2 + W2x[g,b] h1' | acc in = Q2[n,b] cond + W2x[n,b] h1' | acc hn = W2h[n,b] h2
 //   P3 fc1  :  acc = Q3[b] cond + F1x[b] h1' + F1x[b] h2'      (one streamed F1x chunk feeds two MMAs)
 //   P4 fc2  :  acc = Q4[b] cond + F2x[b] y1
-//   P5 fc3  :  acc = F3 y2        (MoL: 30 rows in one 128-row tile)
+//   P5 fc3  :  acc = F3 y2        (MoL: 30 rows in one 128-row tile; RAW: 512 rows, four unit blocks like fc1 / fc2)
 // The program lists the weight chunks in exactly this order; within P2 every chunk that does not depend on h1' is
 // issued first, so those MMAs (and the epilogue-free h2 reads) overlap the P1 gate math.
 #pragma once
@@ -70,7 +70,7 @@ struct Plan {
   std::vector<uint16_t> mine[N_ISSUERS];   // per issuing warp: indices into prog, ascending
   std::vector<float> qk, vq;      // [4096] conditioning-row constants, row order gi1 | gi2 | fc1 | fc2 (gate-major inside the GRUs)
   std::vector<float> b1h, b2h;    // [1536] gate-major
-  std::vector<float> b3;          // [n_classes padded to 128]
+  std::vector<float> b3;          // [n_classes padded to a multiple of 128]
   int n_classes = 0;
   int n_mma = 0;                  // MMA instructions per step (for the roofline bookkeeping)
 };
@@ -78,7 +78,8 @@ struct Plan {
 // K-major no-swizzle operand image of a [128 x kc] tile: element (r, k) at (r/8)*(kc/8)*64 + (k/8)*64 + (r%8)*8 + k%8
 inline size_t tile_index(int r, int k, int kc) { return (size_t)(r / 8) * (kc / 8) * 64 + (size_t)(k / 8) * 64 + (r % 8) * 8 + (k % 8); }
 
-// Builds the plan.  `bf` selects bf16 instead of fp16 operand bits.  n_classes <= 128 (MoL: 30).
+// Builds the plan.  `bf` selects bf16 instead of fp16 operand bits.  n_classes <= 128 (MoL: 30: one fc3 block) or
+// 512 (RAW: four fc3 blocks of 128 classes, in class order, each like an fc1 / fc2 block).
 //
 // Ownership (one owner per accumulator chain, four chains per unit block in every phase; the stream order below
 // interleaves the four owners' chunks -- the kernel regroups them per owner, see compile_device):
@@ -88,7 +89,7 @@ inline size_t tile_index(int r, int k, int kc) { return (size_t)(r / 8) * (kc / 
 // Stream order: the chains of one (phase, block) are interleaved round-robin, so consecutive ring slots go to different
 // warps; within P2 everything that does not depend on h1' is issued (for all blocks) before the W2x h1' chunks.
 // `only_block` >= 0 builds the program of ONE 128-unit block of every layer (accumulator set = phase, see ab() below;
-// fc3 only for block 0): the share of CTA `only_block` of a 4-CTA cluster that splits the rows of every layer
+// MoL's fc3 only for block 0, RAW's fc3 block r for block r): the share of CTA `only_block` of a 4-CTA cluster that splits the rows of every layer
 // (wrnn_stream.cu, cluster form).  Operand readiness codes (wait_b) keep the GLOBAL block of the K range they read.
 inline void build_plan(const HostWeights& w, bool bf, Plan& p, int only_block = -1) {
   Folded f; fold(w, f);
@@ -98,8 +99,10 @@ inline void build_plan(const HostWeights& w, bool bf, Plan& p, int only_block = 
   for (auto& m : p.mine) m.clear();
   p.n_classes = w.n_classes;
   p.qk = s.qk; p.vq = s.vq; p.b1h = s.b1h; p.b2h = s.b2h;
-  p.b3.assign(MROWS, 0.f);
-  for (int r = 0; r < w.n_classes && r < MROWS; ++r) p.b3[r] = w.f3b[r];
+  const bool raw = w.n_classes > MROWS;                    // RAW: fc3 in four unit blocks
+  const int NC3 = raw ? (w.n_classes + MROWS - 1) / MROWS * MROWS : MROWS;   // fc3 rows, zero-padded
+  p.b3.assign(NC3, 0.f);
+  for (int r = 0; r < w.n_classes && r < NC3; ++r) p.b3[r] = w.f3b[r];
 
   struct Pending { Chunk c; std::vector<uint16_t> img; };
   std::vector<Pending> q[N_ISSUERS];
@@ -166,8 +169,8 @@ inline void build_plan(const HostWeights& w, bool bf, Plan& p, int only_block = 
   // sets 0..3, fc3 -> set 0 again): nothing else is computed in the other three, and with a set per phase the
   // MMAs of a phase never wait for the previous phase's epilogue to drain.
   auto ab = [&](int b, int phase) -> int { return only_block >= 0 ? (phase & 3) : b; };
-  std::vector<double> F3((size_t)MROWS * H, 0.0);
-  for (int r = 0; r < w.n_classes && r < MROWS; ++r) for (int k = 0; k < H; ++k) F3[(size_t)r * H + k] = w.f3w[(size_t)r * H + k];
+  std::vector<double> F3((size_t)NC3 * H, 0.0);
+  for (int r = 0; r < w.n_classes && r < NC3; ++r) for (int k = 0; k < H; ++k) F3[(size_t)r * H + k] = w.f3w[(size_t)r * H + k];
   const int QK[5] = {0, 64, 128, 192, CDIM};              // the four K-chunks of a conditioning row (64, 64, 64, 16)
 
   // ---- P1: GRU1 (phase 0).  Accumulators of block b: 4b + {0: r, 1: z, 2: in, 3: hn}
@@ -219,8 +222,20 @@ inline void build_plan(const HostWeights& w, bool bf, Plan& p, int only_block = 
     }
     flush();            // per layer: 3 chunks per issuer and block -> 12 per issuer, even (one-block programs: 3, their ring slots hold one chunk)
   }
-  // ---- P5: fc3 (phase 4): partial accumulators 0..3 of block 0
-  if (only_block <= 0) {
+  // ---- P5: fc3 (phase 4).  RAW: classes [128b, 128b + 128) are unit block b, K split over the four issuers like fc1 /
+  // fc2 (partial accumulators 4b + q, two chunks each); every chunk waits for the y2 block its K range reads.
+  if (raw) {
+    for (int b = B0; b < B1; ++b) {
+      new_block();
+      for (int o = 0; o < N_ISSUERS; ++o) {
+        bool first = true;
+        emit(o, 4, ab(b, 4), F3.data(), H, NC3, b * MROWS, 128 * o, 128 * o + 128, (uint8_t)(4 * ab(b, 4) + o), B_Y2, B_NONE, first, W_Y2);
+        mark_commit(o, ab(b, 4));
+      }
+      flush();
+    }
+  } else if (only_block <= 0) {
+    // MoL: partial accumulators 0..3 of block 0
     new_block();
     for (int o = 0; o < N_ISSUERS; ++o) {
       bool first = true;
