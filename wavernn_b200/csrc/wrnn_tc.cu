@@ -202,6 +202,23 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
     float x = 0.f;
     unsigned n_mma = 0;                                   // completed phases of bar_mma
     unsigned rows_known = p.uniforms_ready ? 0u : 0xffffffffu;   // rows of p.uniforms known to have landed
+    // Phase A's shared-memory operands of step n: pre_n (conditioning chain), W1h h1 (S1 chain of step n-1) and the
+    // vectors qk, vq, b1h.  They are read at the end of phase D of step n-1, while the fold thread waits for the fc3
+    // chain anyway.  Read at the top of phase A, their 120 loads sat between the sample x and the h1 publish, on the
+    // critical path of every step (CTA 0, phase A: 3,050 -> 2,030 cycles per step; cfg2 9.29 -> 8.81 us).
+    // pre_n is complete once bar_q's phase n is: the chain is issued after the S2 chain of step n-1, before the y1
+    // gather.  Its table block is next overwritten by chain n+1, after the h2' gather of step n.
+    float pre_a[32], gh_a[12], qk_a[32], vq_a[32], b1h_a[12];
+    auto read_phase_a = [&](int n) {
+      mbar_wait(bar_q, (uint32_t)(n & 1), p.abort_flag);
+      acc_rd(AC_Q, 32, pre_a);
+      acc_rd(AC_S1 + 12, 12, gh_a);
+#pragma unroll
+      for (int q = 0; q < 32; ++q) { qk_a[q] = qk[q]; vq_a[q] = vq[q]; }
+#pragma unroll
+      for (int q = 0; q < 12; ++q) b1h_a[q] = b1h[q];
+    };
+    read_phase_a(0);
 
     for (int t = 0; t < S; ++t) {
       const int par = t & 1;
@@ -219,18 +236,15 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
       float pre[32];                                      // this fold's 32 conditioning rows (+ qk + x*vq)
       float gn[10], lu, lex[4];                           // sampler terms of this step's draws (MoL / RAW)
       {
-        mbar_wait(bar_q, (uint32_t)(t & 1), p.abort_flag);           // pre_t is in the table
         if (p.x_force && t > 0) x = xf;
-        acc_rd(AC_Q, 32, pre);
-        float gh[12];
-        acc_rd(AC_S1 + 12, 12, gh);                                  // W1h h1 (step t-1, phase B)
+        const float* gh = gh_a;                                      // W1h h1 (step t-1, phase B)
 #pragma unroll
-        for (int q = 0; q < 32; ++q) pre[q] += qk[q] + x * vq[q];
+        for (int q = 0; q < 32; ++q) pre[q] = pre_a[q] + (qk_a[q] + x * vq_a[q]);
         float hv[U];
 #pragma unroll
         for (int j = 0; j < U; ++j) {
-          const float ghr = (t > 0 ? gh[j] : 0.f) + b1h[j], ghz = (t > 0 ? gh[U + j] : 0.f) + b1h[U + j],
-                      ghn = (t > 0 ? gh[2 * U + j] : 0.f) + b1h[2 * U + j];
+          const float ghr = (t > 0 ? gh[j] : 0.f) + b1h_a[j], ghz = (t > 0 ? gh[U + j] : 0.f) + b1h_a[U + j],
+                      ghn = (t > 0 ? gh[2 * U + j] : 0.f) + b1h_a[2 * U + j];
           h1[j] = gru_unit_fast(pre[j], pre[U + j], pre[2 * U + j], ghr, ghz, ghn, h1[j]);
           hv[j] = h1[j];
         }
@@ -338,6 +352,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
         for (int j = 0; j < U; ++j) yv[j] = fmaxf(a[j] + pre[7 * U + j], 0.f);
         publish(img_y2, yv);
         signal(3);
+        if (t + 1 < S) read_phase_a(t + 1);
       }
       if (profiling) { const long long c = clock64(); tprof[3] += c - tp0; tp0 = c; }
 
