@@ -76,39 +76,70 @@ def _gru(gi, gh, h):
     return ((F32(1) - z) * n + z * h).astype(F32)
 
 
+def expand_rows(mel_frames, aux_frames, taps, hop, row_lo, n_rows):
+    """Rows [row_lo, row_lo + n_rows) of the per-sample conditioning stream from frame-rate tensors, in float64:
+    m[n] = sum_d taps[n % hop, d] * mel_frames[n // hop + d] and aux[n] = aux_frames[n // hop] (UpsampleNetwork's
+    stretch+conv cascade as a 5-tap table per output phase; `WaveRNN.upsample_taps`).  mel_frames is the padded
+    (T + 4, 80) mel, so the last row of a (T * hop)-row stream reads frames up to T + 3."""
+    n = np.arange(row_lo, row_lo + n_rows)
+    fr, ph = n // hop, n % hop
+    taps = np.asarray(taps, dtype=np.float64)
+    mel = np.asarray(mel_frames, dtype=np.float64)
+    m = sum(taps[ph, d][:, None] * mel[fr + d] for d in range(5))
+    return m, np.asarray(aux_frames, dtype=np.float64)[fr]
+
+
 def generate_segments(w: dict, mels_up, aux, *, n_seg, seg_len, seg_stride, uniforms=None, mode="MOL",
-                      expo=None, x_force=None, want_logits=False, steps=None, precision="fp16"):
-    """Same signature/semantics as wavernn_oracle.generate_segments, engine arithmetic."""
+                      expo=None, x_force=None, want_logits=False, steps=None, precision="fp16",
+                      fold_row0=None, fold_row_end=None, accumulate="f32"):
+    """Same signature/semantics as wavernn_oracle.generate_segments, engine arithmetic.
+
+    fold_row0 / fold_row_end: per-fold conditioning windows (the engines' fold tables): fold f reads row
+    fold_row0[f] + t, and rows at or past fold_row_end[f] as zero.  Without them fold f starts at f * seg_stride and
+    rows at or past len(mels_up) are zero.
+    accumulate: "f32" sums every matmul in float32 like the tensor cores' accumulators; "f64" sums in float64 and
+    rounds once.  Their difference estimates the accumulation-order noise at a given operand precision."""
     f = fold_weights(w)
     rnd = rounder(precision)
     mats = {k: rnd(f[k].astype(F32)) for k in ("Q", "W2x", "W1h", "F1x", "W2h", "F2x", "F3")}
+    if accumulate == "f64":
+        mats_t = {k: np.ascontiguousarray(v.T, dtype=np.float64) for k, v in mats.items()}
+        mm = lambda a, k: (a.astype(np.float64) @ mats_t[k]).astype(F32)
+    else:
+        assert accumulate == "f32", accumulate
+        mm = lambda a, k: (a @ mats[k].T).astype(F32)
     B, S = n_seg, (steps if steps is not None else seg_len)
     L = mels_up.shape[0]
     G3 = 3 * H
     n_classes = f["F3"].shape[0]
     cond_z = np.concatenate([np.concatenate([mels_up, aux], axis=1).astype(F32), np.zeros((1, CDIM), F32)])
-    base = np.arange(B) * seg_stride
+    if fold_row0 is None:
+        base, end = np.arange(B) * seg_stride, np.full(B, L)
+    else:
+        base, end = np.asarray(fold_row0, dtype=np.int64), np.asarray(fold_row_end, dtype=np.int64)
+        assert base.shape == end.shape == (B,) and end.max() <= L
     h1 = np.zeros((B, H), F32); h2 = np.zeros((B, H), F32)
     gh1 = np.tile(f["b1h"], (B, 1)); gh2 = np.tile(f["b2h"], (B, 1))
     x = np.zeros((B, 1), F32)
     out = np.zeros((B, S), F32)
     logits_all = np.zeros((S, B, n_classes), F32) if want_logits else None
     for t in range(S):
-        cond = rnd(cond_z[np.minimum(base + t, L)])
+        row = base + t
+        cond = rnd(cond_z[np.where(row < end, row, L)])
         if x_force is not None and t > 0:
             x = x_force[t - 1].reshape(B, 1).astype(F32)
-        pre = (cond @ mats["Q"].T + f["qk"] + x * f["vq"]).astype(F32)
+        pre = (mm(cond, "Q") + f["qk"] + x * f["vq"]).astype(F32)
         h1 = _gru(pre[:, :G3], gh1, h1)
         h1o = rnd(h1)
-        gi2 = (h1o @ mats["W2x"].T).astype(F32) + pre[:, G3:2 * G3]
-        gh1 = (h1o @ mats["W1h"].T).astype(F32) + f["b1h"]
-        fc1p = (h1o @ mats["F1x"].T).astype(F32)
+        gi2 = mm(h1o, "W2x") + pre[:, G3:2 * G3]
+        gh1 = mm(h1o, "W1h") + f["b1h"]
+        fc1p = mm(h1o, "F1x")
         h2 = _gru(gi2, gh2, h2)
         h2o = rnd(h2)
-        y1 = np.maximum(fc1p + (h2o @ mats["F1x"].T).astype(F32) + pre[:, 2 * G3:2 * G3 + H], 0).astype(F32)
-        gh2 = (h2o @ mats["W2h"].T).astype(F32) + f["b2h"]
-        y2 = np.maximum((rnd(y1) @ mats["F2x"].T).astype(F32) + pre[:, 2 * G3 + H:], 0).astype(F32)
-        logits = ((rnd(y2) @ mats["F3"].T).astype(F32) + f["b3"]).astype(F32)
+        y1 = np.maximum(fc1p + mm(h2o, "F1x") + pre[:, 2 * G3:2 * G3 + H], 0).astype(F32)
+        gh2 = mm(h2o, "W2h") + f["b2h"]
+        y2 = np.maximum(mm(rnd(y1), "F2x") + pre[:, 2 * G3 + H:], 0).astype(F32)
+        logits = (mm(rnd(y2), "F3") + f["b3"]).astype(F32)
         if want_logits:
             logits_all[t] = logits
         if mode == "MOL":

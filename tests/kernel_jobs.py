@@ -1,0 +1,103 @@
+"""The job matrix that runs every compiled tensor-core kernel (tests/test_gpu_instantiations.py), the emulation of
+each job (oracle/contract.py) and the logit tolerances, which the CPU predicts (tests/test_contract.py).
+
+Every job is teacher-forced with explicit draws and has the edges where the kernels' per-instantiation code differs:
+  - seg_stride 271 against a hop of 275: fold windows start at many phases of the hop and cross frame boundaries;
+  - steps < seg_len, seg_first != 0;
+  - the stream ends half way into the last fold's window, which reads zero rows from there on;
+  - fold tables (frame-rate jobs): starts that are not multiples of the stride, windows that end mid-frame and before
+    `steps`, one window shorter than 8 rows.
+Rows come from frame-rate tensors through the 5-tap table, in float64 (`contract.expand_rows`); the materialised jobs
+read those rows rounded to float32."""
+from __future__ import annotations
+
+import numpy as np
+
+from oracle import contract as C
+from oracle import philox as P
+from test_gpu_sampling import forced_inputs
+
+HOP, STRIDE, STEPS, SEG_LEN, SEG_FIRST = 275, 271, 32, 300, 7
+SEED, OFFSET = (3 << 32) | 11, 0x55
+PERSISTENT_FOLDS = (24, 25, 73)          # last small tile, first BIG tile, a 64-fold BIG tile then a 9-fold small one
+STREAM_FOLDS = {16: 17, 32: 33}          # two tiles of NF folds per CTA, the second one ragged
+SMALL_TILE = 24
+
+# Teacher-forced logits of a kernel against contract.generate_segments at the kernel's operand precision.  Each bound is
+# at least 4 x the largest float32-vs-float64 accumulation spread of the emulation on these jobs (asserted on the CPU in
+# tests/test_contract.py, which prints the spreads: fp16 8.9e-5 MoL / 1.1e-4 RAW, bf16 6.9e-4 / 7.5e-4), with room for
+# another CPU's float32 summation order; fp16 stays under the suite's 1e-3.
+LOGIT_TOL = {("fp16", "MOL"): 6e-4, ("fp16", "RAW"): 6e-4, ("bf16", "MOL"): 4e-3, ("bf16", "RAW"): 4e-3}
+
+
+def geometry(n):
+    """(L, T): the stream ends half way into the last fold's window; T frames cover it."""
+    L = (SEG_FIRST + n - 1) * STRIDE + STEPS // 2
+    return L, L // HOP + 1
+
+
+def frames(n, seed):
+    """Padded mel frames (T + 4, 80) and aux frames (T + 4, 128), float32."""
+    _, T = geometry(n)
+    rs = np.random.RandomState(seed)
+    return rs.rand(T + 4, 80).astype(np.float32), rs.randn(T + 4, 128).astype(np.float32)
+
+
+def fold_tables(n, seed):
+    """fold_row0 / fold_row_end (int64, absolute rows of the stream) for n folds."""
+    L, _ = geometry(n)
+    rs = np.random.RandomState(seed)
+    row0 = rs.randint(0, L - 2 * STEPS, n).astype(np.int64)
+    row0[row0 % STRIDE == 0] += 1
+    length = rs.randint(STEPS // 2, 2 * STEPS, n)          # about a third end before `steps`
+    length[1] = 5                                          # shorter than one 8-row group
+    end = np.minimum(row0 + length, L)
+    end[end % HOP == 0] -= 1                               # every window ends mid-frame
+    return row0, end.astype(np.int64)
+
+
+def make_job(n, mode, taps, tables=False):
+    """Everything a kernel and the emulation need for one job of n folds.  Strided: `m_up` / `aux` are the job's rows
+    from its first fold on (row SEG_FIRST * STRIDE of the stream), as the materialised path indexes them.  Tables:
+    the whole stream, indexed by the absolute fold_row0."""
+    L, T = geometry(n)
+    seed = 1000 * n + (2 if tables else 0) + (mode == "RAW")
+    mel_fr, aux_fr = frames(n, seed)
+    row_lo = 0 if tables else SEG_FIRST * STRIDE
+    m, a = C.expand_rows(mel_fr, aux_fr, taps, HOP, row_lo, L - row_lo)
+    job = dict(n=n, mode=mode, tables=tables, L=L, T=T, mel_frames=mel_fr, aux_frames=aux_fr, taps=np.asarray(taps, np.float32),
+               row_lo=row_lo, m_up=m.astype(np.float32), aux=a.astype(np.float32), x_force=forced_inputs(n, STEPS, seed + 7),
+               fold_row0=None, fold_row_end=None, uniforms=None, expo=None)
+    if tables:
+        job["fold_row0"], job["fold_row_end"] = fold_tables(n, seed + 3)
+    if mode == "MOL":
+        job["uniforms"] = P.mol_uniforms(SEED, OFFSET, SEG_FIRST, n, STEPS)
+    else:
+        job["expo"] = P.raw_expo(SEED, OFFSET, SEG_FIRST, n, STEPS)[0]
+    return job
+
+
+def emulate(w, job, precision, accumulate="f32"):
+    """contract.generate_segments on the job: (samples (n, STEPS), logits (STEPS, n, classes))."""
+    return C.generate_segments(w, job["m_up"], job["aux"], n_seg=job["n"], seg_len=SEG_LEN, seg_stride=STRIDE, steps=STEPS,
+                               mode=job["mode"], uniforms=job["uniforms"], expo=job["expo"], x_force=job["x_force"],
+                               fold_row0=job["fold_row0"], fold_row_end=job["fold_row_end"], want_logits=True,
+                               precision=precision, accumulate=accumulate)
+
+
+def all_jobs():
+    """(n, tables) of every job the GPU matrix emulates."""
+    return [(n, t) for n in PERSISTENT_FOLDS + tuple(STREAM_FOLDS.values()) for t in (False, True)]
+
+
+def slice_folds(job, a, b):
+    """The draws, teacher inputs and fold tables of folds [a, b) of a job, as a job of b - a folds starting at fold a
+    (seg_first + a) would take them."""
+    n = job["n"]
+    out = {"x_force": np.ascontiguousarray(job["x_force"][:, a:b])}
+    u = job["uniforms"]
+    out["uniforms"] = None if u is None else np.ascontiguousarray(np.concatenate([u[:, 10 * a:10 * b], u[:, 10 * n + a:10 * n + b]], 1))
+    out["expo"] = None if job["expo"] is None else np.ascontiguousarray(job["expo"][:, a:b])
+    out["fold_row0"] = None if job["fold_row0"] is None else job["fold_row0"][a:b].copy()
+    out["fold_row_end"] = None if job["fold_row_end"] is None else job["fold_row_end"][a:b].copy()
+    return out

@@ -2,8 +2,10 @@
 reference-order oracle.  States the FP tolerance of the product path on the CPU."""
 import numpy as np
 import pytest
+import torch
 
 import helpers
+import kernel_jobs as K
 from oracle import contract as C
 from oracle import wavernn_oracle as O
 
@@ -42,3 +44,64 @@ def test_operand_rounding_teacher_forced_tolerance(setup, precision, tol):
     w, m_up, aux, kw, ref, lref = setup
     _, lg = C.generate_segments(w, m_up, aux, precision=precision, want_logits=True, x_force=ref.T.copy(), **kw)
     assert np.abs(lg - lref).max() < tol
+
+
+def test_fold_tables_of_the_strided_windows_reproduce_the_strided_run_and_short_windows_read_zero_rows(setup):
+    w, m_up, aux, kw, _, _ = setup
+    kw = dict(kw, steps=40)
+    B, stride, L = kw["n_seg"], kw["seg_stride"], m_up.shape[0]
+    base = np.arange(B, dtype=np.int64) * stride
+    out, lg = C.generate_segments(w, m_up, aux, want_logits=True, **kw)
+    out_t, lg_t = C.generate_segments(w, m_up, aux, want_logits=True, fold_row0=base, fold_row_end=np.full(B, L), **kw)
+    assert np.array_equal(out, out_t) and np.array_equal(lg, lg_t)
+    # windows of 25, 1 and 40 rows: the same as the strided run on rows zeroed past each window's end
+    end = base + np.array([25, 1, 40])
+    m_z, a_z = m_up.copy(), aux.copy()
+    for f in range(B):
+        m_z[end[f]:base[f] + 40] = 0
+        a_z[end[f]:base[f] + 40] = 0
+    out_z, lg_z = C.generate_segments(w, m_z, a_z, want_logits=True, **kw)
+    out_e, lg_e = C.generate_segments(w, m_up, aux, want_logits=True, fold_row0=base, fold_row_end=end, **kw)
+    assert np.array_equal(out_z, out_e) and np.array_equal(lg_z, lg_e)
+    assert not np.array_equal(lg_e, lg)
+
+
+def test_expand_rows_restates_the_upsample_network():
+    """contract.expand_rows (float64 5-tap sum over the padded mel) against model.upsample, the whole stream and a
+    slice starting at a non-zero phase."""
+    model = helpers.make_model(0, "MOL").eval()
+    T, hop = 23, 275
+    mp = torch.nn.functional.pad(helpers.make_mel(T, 4), (2, 2))
+    with torch.no_grad():
+        full_m, full_a = model.upsample(mp)
+        aux_fr = model.upsample.resnet(mp)[0].T.numpy()
+    taps = model.upsample_taps(torch.device("cpu")).numpy()
+    mel_fr = mp[0].T.numpy()
+    m, a = C.expand_rows(mel_fr, aux_fr, taps, hop, 0, T * hop)
+    np.testing.assert_allclose(m, full_m[0].numpy(), rtol=0, atol=2e-6)
+    assert np.array_equal(a, full_a[0].numpy())
+    m2, a2 = C.expand_rows(mel_fr, aux_fr, taps, hop, 3 * hop + 101, 700)
+    assert np.array_equal(m2, m[3 * hop + 101:3 * hop + 801]) and np.array_equal(a2, a[3 * hop + 101:3 * hop + 801])
+
+
+@pytest.mark.parametrize("precision", ["fp16", "bf16"])
+@pytest.mark.parametrize("mode", ["MOL", "RAW"])
+def test_accumulation_spread_predicts_the_kernel_matrix_tolerances(mode, precision):
+    """Teacher-forced logits of every job of tests/test_gpu_instantiations.py, summed in float32 and in float64 at the
+    same operand precision: their largest difference estimates the accumulation-order noise a kernel may show, and the
+    GPU tolerance must be at least 4 x that (fp16: at most the suite's 1e-3)."""
+    model = helpers.make_model(0, mode)
+    w = O.hot_weights(helpers.state_numpy(model))
+    taps = model.upsample_taps(torch.device("cpu")).numpy()
+    spread = 0.0
+    for n, tables in K.all_jobs():
+        job = K.make_job(n, mode, taps, tables)
+        _, l32 = K.emulate(w, job, precision)
+        _, l64 = K.emulate(w, job, precision, accumulate="f64")
+        assert np.isfinite(l32).all() and np.abs(l64).max() > 0.1
+        spread = max(spread, float(np.abs(l32 - l64).max()))
+    tol = K.LOGIT_TOL[(precision, mode)]
+    print(f"{precision} {mode}: predicted accumulation spread of the teacher-forced logits {spread:.3e}; GPU tolerance {tol:.1e}")
+    assert spread <= tol / 4
+    if precision == "fp16":
+        assert tol <= 1e-3
