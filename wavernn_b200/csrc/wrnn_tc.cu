@@ -12,8 +12,8 @@
 //     Q  = folded conditioning rows (N=32, K=208) consumes cond_t, runs one step ahead
 // The folds are the M dimension ("swap-AB"): tile of M=64 folds (one wgmma M tile).  The issuing warpgroup writes
 // each finished accumulator to a shared-memory table [column][fold], so every epilogue (GRU gates, relu, MoL
-// sampling) is thread-local: one thread owns one fold, reads its columns and keeps that fold's hidden state in
-// registers for the whole sequence.
+// sampling) is thread-local: one thread owns one (fold, hidden unit) pair (two units above 24 folds), reads that
+// unit's columns and keeps its hidden state in registers for the whole sequence.
 //
 // Per step only the four 512-wide activation vectors cross SMs.  They are exchanged through
 // L2-resident buffers that are byte images of the wgmma A-operand layout, so a consumer pulls a
@@ -78,6 +78,13 @@ constexpr int WEIGHT_BYTES = OFF_VEC + NVEC * 4 - OFF_S1; // per-CTA blob == sme
 // t, long after the fold warps have read pre_t.
 constexpr int AC_S1 = 0, AC_S2 = AC_S1 + N_S1, AC_S3 = AC_S2 + N_S2, AC_F3 = AC_S3 + N_S3, AC_Q = AC_F3 + N_F3,
               AC_COLS = AC_Q + N_Q, ACP = MT + 4;
+// Image row (= accumulator column) of local row blk * U + j of the S1 / S2 / S3 / Q maps (wrnn_fold.h; RAW F3: blk 0).
+// A fold thread reads one unit's column per load while the three other threads of its quad read the other units'
+// (same block): unit j of block blk at 8 (blk / 2) + 2 j + blk % 2 puts the four at 4 * column = 8 j (mod 32) apart,
+// so the 8 folds x 4 units of a warp's load hit 32 distinct banks (at adjacent columns they collide 2-way).  Permuting
+// the N rows of a wgmma permutes its accumulator columns and changes no column's sums.
+static_assert(U == 4, "column map");
+__host__ __device__ constexpr int tcol(int blk, int j) { return 8 * (blk >> 1) + 2 * j + (blk & 1); }
 constexpr int OFF_ACC = OFF_VEC + NVEC * 4;
 constexpr int OFF_BAR = OFF_ACC + AC_COLS * ACP * 4;      // 3 mbarriers
 constexpr int SMEM_BYTES = OFF_BAR + 64;
@@ -177,47 +184,73 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
 
   if (warp < 4) {
     // =========================================================================================
-    // fold warps: thread (warp, lane < 16) owns fold 16 * warp + lane; lanes 16-31 shadow lanes 0-15
+    // fold warps: thread tid owns fold tid / TPF and this CTA's units [UT * (tid % TPF), + UT), i.e. the TPF threads of a
+    // fold are adjacent lanes.  Per step each thread reads only its units' accumulator columns: 11 loads per unit for
+    // phase A, 3 + 1 + 1 on the critical paths of phases B, C, D, and 12 for the MoL sampler.  All four fold warps issue
+    // their loads at once into one shared-memory pipe, so every load taken off these paths shortens the step.
     // =========================================================================================
-    const int fold = warp * 16 + lane;
-    const bool owns_fold = lane < 16 && fold < B;
-    const float* acc_f = acc + warp * 16 + (lane & 15);     // this fold's entry of accumulator column 0
-    auto acc_rd = [&](int col0, int n, float* v) {
+    constexpr int UT = BIG ? 2 : 1;                       // units per thread: <= 24 folds x 4 units fit 128 threads once
+    constexpr int TPF = U / UT;                           // threads per fold
+    const int fold = tid / TPF, slot = tid % TPF, j0 = slot * UT;
+    const bool owns_fold = fold < B;
+    // warp-uniform: the warp holds at least one fold.  A warp without one skips every load and all the arithmetic, but
+    // still takes part in every wait and named barrier.
+    const bool active = warp * (32 / TPF) < B;
+    const float* acc_f = acc + fold;                      // this fold's entry of accumulator column 0
+    auto acc_rd = [&](int col0, int blk, float* v) {      // this thread's units of block blk of a chain's columns
 #pragma unroll
-      for (int i = 0; i < n; ++i) v[i] = acc_f[(col0 + i) * ACP];
+      for (int i = 0; i < UT; ++i) v[i] = acc_f[(col0 + tcol(blk, j0 + i)) * ACP];
     };
-    const size_t pub_off = (size_t)(fold >> 3) * SBO_H + (u0 >> 3) * 128 + (fold & 7) * 16 + (u0 & 7) * 2;
+    const size_t pub_off = (size_t)(fold >> 3) * SBO_H + (u0 >> 3) * 128 + (fold & 7) * 16 + ((u0 & 7) + j0) * 2;
     const bool profiling = (p.prof != nullptr) && cta == 0 && tid == 0;
     long long tprof[5] = {0, 0, 0, 0, 0};
-    auto publish = [&](unsigned char* img, const float* v) {   // this fold's 4 values of this CTA's units
-      uint2 w;
-      w.x = pack2<FMT>(v[0], v[1]); w.y = pack2<FMT>(v[2], v[3]);
-      if (owns_fold) *reinterpret_cast<uint2*>(img + pub_off) = w;
+    auto publish = [&](unsigned char* img, const float* v) {   // this thread's values of this fold; a fold's 4 units: 8 B
+      if (!owns_fold) return;
+      if constexpr (UT == 1) *reinterpret_cast<uint16_t*>(img + pub_off) = pack1<FMT>(v[0]);
+      else *reinterpret_cast<uint32_t*>(img + pub_off) = pack2<FMT>(v[0], v[1]);
     };
     auto signal = [&](int v) {                           // all fold warps have stored: one release increment per CTA
       named_bar_sync(1, 128);
       if (tid == 0) red_release_add_u32(p.counters + v, 1u);
     };
-    float h1[U] = {0.f, 0.f, 0.f, 0.f}, h2[U] = {0.f, 0.f, 0.f, 0.f};
+    // the vectors of this thread's units, loop-invariant: registers (index blk * UT + i, as the column blocks)
+    float qk_r[8 * UT], vq_r[8 * UT], b1h_r[3 * UT], b2h_r[3 * UT];
+#pragma unroll
+    for (int blk = 0; blk < 8; ++blk)
+#pragma unroll
+      for (int i = 0; i < UT; ++i) { qk_r[blk * UT + i] = qk[blk * U + j0 + i]; vq_r[blk * UT + i] = vq[blk * U + j0 + i]; }
+#pragma unroll
+    for (int g = 0; g < 3; ++g)
+#pragma unroll
+      for (int i = 0; i < UT; ++i) { b1h_r[g * UT + i] = b1h[g * U + j0 + i]; b2h_r[g * UT + i] = b2h[g * U + j0 + i]; }
+    float b3_r[RAW ? UT : 10];                           // MoL: the 10 mixture-weight biases; RAW: this thread's classes
+#pragma unroll
+    for (int i = 0; i < (RAW ? UT : 10); ++i) b3_r[i] = b3[RAW ? j0 + i : i];
+    float h1[UT], h2[UT];
+#pragma unroll
+    for (int i = 0; i < UT; ++i) { h1[i] = 0.f; h2[i] = 0.f; }
     float x = 0.f;
     unsigned n_mma = 0;                                   // completed phases of bar_mma
     unsigned rows_known = p.uniforms_ready ? 0u : 0xffffffffu;   // rows of p.uniforms known to have landed
-    // Phase A's shared-memory operands of step n: pre_n (conditioning chain), W1h h1 (S1 chain of step n-1) and the
-    // vectors qk, vq, b1h.  They are read at the end of phase D of step n-1, while the fold thread waits for the fc3
-    // chain anyway.  Read at the top of phase A, their 120 loads sat between the sample x and the h1 publish, on the
-    // critical path of every step (CTA 0, phase A: 3,050 -> 2,030 cycles per step; cfg2 9.29 -> 8.81 us).
+    // Phase A's shared-memory operands of step n: pre_n (conditioning chain) and W1h h1 (S1 chain of step n-1).  They
+    // are read at the end of phase D of step n-1, while the fold thread waits for the fc3 chain anyway: read at the top
+    // of phase A they would sit between the sample x and the h1 publish, on the critical path of every step.
     // pre_n is complete once bar_q's phase n is: the chain is issued after the S2 chain of step n-1, before the y1
     // gather.  Its table block is next overwritten by chain n+1, after the h2' gather of step n.
-    float pre_a[32], gh_a[12], qk_a[32], vq_a[32], b1h_a[12];
+    float pre_a[8 * UT], gh_a[3 * UT];
     auto read_phase_a = [&](int n) {
       mbar_wait(bar_q, (uint32_t)(n & 1), p.abort_flag);
-      acc_rd(AC_Q, 32, pre_a);
-      acc_rd(AC_S1 + 12, 12, gh_a);
+      if (!active) return;
 #pragma unroll
-      for (int q = 0; q < 32; ++q) { qk_a[q] = qk[q]; vq_a[q] = vq[q]; }
+      for (int blk = 0; blk < 8; ++blk) acc_rd(AC_Q, blk, pre_a + blk * UT);
 #pragma unroll
-      for (int q = 0; q < 12; ++q) b1h_a[q] = b1h[q];
+      for (int g = 0; g < 3; ++g) acc_rd(AC_S1, 3 + g, gh_a + g * UT);
     };
+    // Read after the publish of the phase before their use, off its critical path: W2h h2 (phase C of step t-1, for
+    // phase B of step t; the S2 block is next overwritten after the h2' gather of step t) and F1x h1' (phase B, for C).
+    float w2h_a[3 * UT], f1h1_a[UT];
+#pragma unroll
+    for (int i = 0; i < 3 * UT; ++i) w2h_a[i] = 0.f;
     read_phase_a(0);
 
     for (int t = 0; t < S; ++t) {
@@ -233,38 +266,44 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
       if (owns_fold && p.x_force && t > 0) xf = __ldg(p.x_force + (size_t)(t - 1) * p.n_total + p.f0 + fold);
 
       // ---- A: GRU1.  gi1 = pre_t (conditioning chain, D_Q) + x * v1 ; gh1 = W1h h1 + b1h (D_S1 of step t-1)
-      float pre[32];                                      // this fold's 32 conditioning rows (+ qk + x*vq)
-      float gn[10], lu, lex[4];                           // sampler terms of this step's draws (MoL / RAW)
+      float pre[8 * UT];                                  // this thread's 8 conditioning rows per unit (+ qk + x*vq)
+      float gn[10], lu, lex[UT];                          // sampler terms of this step's draws (MoL / RAW)
       {
         if (p.x_force && t > 0) x = xf;
-        const float* gh = gh_a;                                      // W1h h1 (step t-1, phase B)
+        if (active) {
 #pragma unroll
-        for (int q = 0; q < 32; ++q) pre[q] = pre_a[q] + (qk_a[q] + x * vq_a[q]);
-        float hv[U];
+          for (int q = 0; q < 8 * UT; ++q) pre[q] = pre_a[q] + (qk_r[q] + x * vq_r[q]);
 #pragma unroll
-        for (int j = 0; j < U; ++j) {
-          const float ghr = (t > 0 ? gh[j] : 0.f) + b1h_a[j], ghz = (t > 0 ? gh[U + j] : 0.f) + b1h_a[U + j],
-                      ghn = (t > 0 ? gh[2 * U + j] : 0.f) + b1h_a[2 * U + j];
-          h1[j] = gru_unit_fast(pre[j], pre[U + j], pre[2 * U + j], ghr, ghz, ghn, h1[j]);
-          hv[j] = h1[j];
+          for (int i = 0; i < UT; ++i) {                  // gh_a: W1h h1 (step t-1, phase B)
+            const float ghr = (t > 0 ? gh_a[i] : 0.f) + b1h_r[i], ghz = (t > 0 ? gh_a[UT + i] : 0.f) + b1h_r[UT + i],
+                        ghn = (t > 0 ? gh_a[2 * UT + i] : 0.f) + b1h_r[2 * UT + i];
+            h1[i] = gru_unit_fast(pre[i], pre[UT + i], pre[2 * UT + i], ghr, ghz, ghn, h1[i]);
+          }
+          publish(img_h1, h1);
         }
-        publish(img_h1, hv);
         signal(0);
         // This step's draws and everything computed from them alone, while the h1' exchange is in flight: at the top of
         // the step or in the sampler they sit between x_{t-1} and the h1' publish, on the critical path of every step.
+        // Every thread of a fold draws the fold's MoL uniforms (the same values, so all compute the same sample).
         float ur[11];
 #pragma unroll
         for (int i = 0; i < 11; ++i) ur[i] = 0.5f;
-        float ex[4] = {1.f, 1.f, 1.f, 1.f};                 // RAW: Exp(1) draws of this CTA's 4 classes
+        float ex[UT];                                       // RAW: Exp(1) draws of this thread's classes
+#pragma unroll
+        for (int i = 0; i < UT; ++i) ex[i] = 1.f;
         if constexpr (RAW) {
           if (owns_fold) {
             if (p.expo) {
-              const float4 v = __ldg(reinterpret_cast<const float4*>(p.expo + ((size_t)t * p.n_total + p.f0 + fold) * NCLS + u0));
-              ex[0] = v.x; ex[1] = v.y; ex[2] = v.z; ex[3] = v.w;
+#pragma unroll
+              for (int i = 0; i < UT; ++i) ex[i] = __ldg(p.expo + ((size_t)t * p.n_total + p.f0 + fold) * NCLS + u0 + j0 + i);
             } else {                                        // same keying as the SIMT engine: block 16 + class/4
               const Philox4 r = philox4x32_10((unsigned)t, (unsigned)(p.seg_first + p.f0 + fold), 16u + (unsigned)cta,
                                               (unsigned)p.offset, (unsigned)p.seed, (unsigned)(p.seed >> 32));
-              ex[0] = -logf(u01_open(r.x)); ex[1] = -logf(u01_open(r.y)); ex[2] = -logf(u01_open(r.z)); ex[3] = -logf(u01_open(r.w));
+#pragma unroll
+              for (int i = 0; i < UT; ++i) {
+                const int j = j0 + i;
+                ex[i] = -logf(u01_open(j == 0 ? r.x : j == 1 ? r.y : j == 2 ? r.z : r.w));
+              }
             }
           }
         } else if (p.uniforms) {
@@ -299,7 +338,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
         }
         if constexpr (RAW) {
 #pragma unroll
-          for (int i = 0; i < 4; ++i) { lex[i] = __logf(ex[i]); settle(lex[i]); }
+          for (int i = 0; i < UT; ++i) { lex[i] = __logf(ex[i]); settle(lex[i]); }
         } else {
           mol_noise_fast(ur, gn, lu);
 #pragma unroll
@@ -312,45 +351,51 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
       // ---- B: [W2x ; W1h ; F1x] h1'  ->  GRU2, gh1 for step t+1, fc1 partial ---------------------
       {
         mbar_wait(bar_mma, n_mma & 1, p.abort_flag); ++n_mma;
-        float gi[12], gh[12];
-        acc_rd(AC_S1, 12, gi);                                       // W2x h1'
-        acc_rd(AC_S2 + 4, 12, gh);                                   // W2h h2 (step t-1, phase C)
-        float hv[U];
+        if (active) {
+          float gi[3 * UT];
 #pragma unroll
-        for (int j = 0; j < U; ++j) {
-          const float ghr = (t > 0 ? gh[j] : 0.f) + b2h[j], ghz = (t > 0 ? gh[U + j] : 0.f) + b2h[U + j],
-                      ghn = (t > 0 ? gh[2 * U + j] : 0.f) + b2h[2 * U + j];
-          h2[j] = gru_unit_fast(gi[j] + pre[3 * U + j], gi[U + j] + pre[4 * U + j], gi[2 * U + j] + pre[5 * U + j], ghr, ghz, ghn, h2[j]);
-          hv[j] = h2[j];
+          for (int g = 0; g < 3; ++g) acc_rd(AC_S1, g, gi + g * UT);          // W2x h1'
+#pragma unroll
+          for (int i = 0; i < UT; ++i) {                                     // w2h_a: W2h h2 (step t-1, phase C)
+            const float ghr = (t > 0 ? w2h_a[i] : 0.f) + b2h_r[i], ghz = (t > 0 ? w2h_a[UT + i] : 0.f) + b2h_r[UT + i],
+                        ghn = (t > 0 ? w2h_a[2 * UT + i] : 0.f) + b2h_r[2 * UT + i];
+            h2[i] = gru_unit_fast(gi[i] + pre[3 * UT + i], gi[UT + i] + pre[4 * UT + i], gi[2 * UT + i] + pre[5 * UT + i], ghr, ghz, ghn, h2[i]);
+          }
+          publish(img_h2, h2);
         }
-        publish(img_h2, hv);
         signal(1);
+        if (active) acc_rd(AC_S1, 6, f1h1_a);                                // F1x h1', for phase C
       }
       if (profiling) { const long long c = clock64(); tprof[1] += c - tp0; tp0 = c; }
 
       // ---- C: [F1x ; W2h] h2'  ->  y1 = relu(fc1), gh2 for step t+1 ------------------------------
       {
         mbar_wait(bar_mma, n_mma & 1, p.abort_flag); ++n_mma;
-        float a[4], b4[4];
-        acc_rd(AC_S2, 4, a);                                         // F1x h2'
-        acc_rd(AC_S1 + 24, 4, b4);                                   // F1x h1' (phase B)
-        float yv[U];
+        if (active) {
+          float a[UT], yv[UT];
+          acc_rd(AC_S2, 0, a);                                               // F1x h2'
 #pragma unroll
-        for (int j = 0; j < U; ++j) yv[j] = fmaxf(a[j] + b4[j] + pre[6 * U + j], 0.f);
-        publish(img_y1, yv);
+          for (int i = 0; i < UT; ++i) yv[i] = fmaxf(a[i] + f1h1_a[i] + pre[6 * UT + i], 0.f);
+          publish(img_y1, yv);
+        }
         signal(2);
+        if (active) {
+#pragma unroll
+          for (int g = 0; g < 3; ++g) acc_rd(AC_S2, 1 + g, w2h_a + g * UT);  // W2h h2', for phase B of step t+1
+        }
       }
       if (profiling) { const long long c = clock64(); tprof[2] += c - tp0; tp0 = c; }
 
       // ---- D: F2x y1 -> y2 = relu(fc2) --------------------------------------------------------------
       {
         mbar_wait(bar_mma, n_mma & 1, p.abort_flag); ++n_mma;
-        float a[4];
-        acc_rd(AC_S3, 4, a);
-        float yv[U];
+        if (active) {
+          float a[UT], yv[UT];
+          acc_rd(AC_S3, 0, a);
 #pragma unroll
-        for (int j = 0; j < U; ++j) yv[j] = fmaxf(a[j] + pre[7 * U + j], 0.f);
-        publish(img_y2, yv);
+          for (int i = 0; i < UT; ++i) yv[i] = fmaxf(a[i] + pre[7 * UT + i], 0.f);
+          publish(img_y2, yv);
+        }
         signal(3);
         if (t + 1 < S) read_phase_a(t + 1);
       }
@@ -359,56 +404,74 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
       // ---- E: logits = F3 y2 + b3, sample ---------------------------------------------------------------
       if constexpr (!RAW) {                                 // MoL: fc3 + sampler replicated in every CTA
         mbar_wait(bar_mma, n_mma & 1, p.abort_flag); ++n_mma;
-        float lg[32];
-        acc_rd(AC_F3, 30, lg);
+        if (active) {
+          // every thread of a fold: the 10 mixture logits, then only the chosen component's mean and log-scale
+          const float* lgc = acc_f + AC_F3 * ACP;
+          float lg[10];
 #pragma unroll
-        for (int i = 0; i < 30; ++i) lg[i] += b3[i];
-        x = mol_sample_noise(lg, gn, lu);
-        if (owns_fold && cta == 0) {
-          p.out[(size_t)(p.f0 + fold) * p.out_pitch + t] = x;
-          if (p.logits_out) {
+          for (int k = 0; k < 10; ++k) lg[k] = lgc[k * ACP] + b3_r[k];
+          const int k = mol_pick(lg, gn);
+          x = mol_finish(lgc[(10 + k) * ACP] + b3[10 + k], lgc[(20 + k) * ACP] + b3[20 + k], lu);
+          if (owns_fold && slot == 0 && cta == 0) {
+            p.out[(size_t)(p.f0 + fold) * p.out_pitch + t] = x;
+            if (p.logits_out) {
 #pragma unroll
-            for (int i = 0; i < 30; ++i) p.logits_out[((size_t)t * p.n_total + p.f0 + fold) * 30 + i] = lg[i];
+              for (int i = 0; i < 30; ++i) p.logits_out[((size_t)t * p.n_total + p.f0 + fold) * 30 + i] = lgc[i * ACP] + b3[i];
+            }
           }
         }
       } else {                                              // RAW: this CTA's 4 classes, then the candidate exchange
         mbar_wait(bar_mma, n_mma & 1, p.abort_flag); ++n_mma;
-        float lg[4];
-        acc_rd(AC_F3, 4, lg);
-        float best = -INFINITY; int bestk = 0;
+        // The best of the first maximum / lowest class among equals: (score, class) pairs combine with that rule in any
+        // grouping, so a thread takes its own classes in order and the TPF threads of a fold combine by shuffles.
+        auto combine = [](float& best, int& bestk, float ob, int ok) {
+          if (ob > best || (ob == best && ok < bestk)) { best = ob; bestk = ok; }
+        };
+        auto combine_fold = [&](float& best, int& bestk) {
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          lg[i] += b3[i];
-          const float sc = lg[i] - lex[i];
-          if (sc > best) { best = sc; bestk = u0 + i; }
-        }
+          for (int o = 1; o < TPF; o <<= 1)
+            combine(best, bestk, __shfl_xor_sync(0xffffffffu, best, o), __shfl_xor_sync(0xffffffffu, bestk, o));
+        };
         unsigned char* cand_out = p.xch5 + (size_t)par * cand_bytes;
-        if (owns_fold) {
-          *reinterpret_cast<uint2*>(cand_out + ((size_t)cta * n_groups * 8 + fold) * 8) = make_uint2(__float_as_uint(best), (unsigned)bestk);
-          if (p.logits_out)
-            *reinterpret_cast<float4*>(p.logits_out + ((size_t)t * p.n_total + p.f0 + fold) * NCLS + u0) = make_float4(lg[0], lg[1], lg[2], lg[3]);
-        }
-        signal(4);
-        // every CTA reduces the 128 candidates of each fold the same way; the two half-warps split the CTAs
-        mbar_wait(bar_g, (uint32_t)((GPS * t + 4) & 1), p.abort_flag);
-        const uint2* cand = reinterpret_cast<const uint2*>(smem + OFF_A);
-        const int fr = warp * 16 + (lane & 15), c0 = (lane >> 4) * (P / 2);
-        best = -INFINITY; bestk = 0x7fffffff;
-        if (fr < n_groups * 8) {
-#pragma unroll 8
-          for (int c = c0; c < c0 + P / 2; ++c) {
-            const uint2 v = cand[c * n_groups * 8 + fr];
-            const float sc = __uint_as_float(v.x);
-            if (sc > best) { best = sc; bestk = (int)v.y; }        // ascending class order: first maximum wins
+        if (active) {
+          float lg[UT];
+          acc_rd(AC_F3, 0, lg);
+          float best = -INFINITY; int bestk = 0;
+#pragma unroll
+          for (int i = 0; i < UT; ++i) {
+            lg[i] += b3_r[i];
+            const float sc = lg[i] - lex[i];
+            if (sc > best) { best = sc; bestk = u0 + j0 + i; }
+          }
+          combine_fold(best, bestk);
+          if (owns_fold) {
+            if (slot == 0)
+              *reinterpret_cast<uint2*>(cand_out + ((size_t)cta * n_groups * 8 + fold) * 8) = make_uint2(__float_as_uint(best), (unsigned)bestk);
+            if (p.logits_out) {
+#pragma unroll
+              for (int i = 0; i < UT; ++i) p.logits_out[((size_t)t * p.n_total + p.f0 + fold) * NCLS + u0 + j0 + i] = lg[i];
+            }
           }
         }
-        {
-          const float ob = __shfl_xor_sync(0xffffffffu, best, 16);
-          const int ok = __shfl_xor_sync(0xffffffffu, bestk, 16);
-          if (ob > best || (ob == best && ok < bestk)) { best = ob; bestk = ok; }
+        signal(4);
+        // every CTA reduces the 128 candidates of each fold the same way; the TPF threads of a fold split the CTAs
+        mbar_wait(bar_g, (uint32_t)((GPS * t + 4) & 1), p.abort_flag);
+        if (active) {
+          const uint2* cand = reinterpret_cast<const uint2*>(smem + OFF_A);
+          const int c0 = slot * (P / TPF);
+          float best = -INFINITY; int bestk = 0x7fffffff;
+          if (fold < n_groups * 8) {
+#pragma unroll 8
+            for (int c = c0; c < c0 + P / TPF; ++c) {
+              const uint2 v = cand[c * n_groups * 8 + fold];
+              const float sc = __uint_as_float(v.x);
+              if (sc > best) { best = sc; bestk = (int)v.y; }        // ascending class order: first maximum wins
+            }
+          }
+          combine_fold(best, bestk);
+          x = 2.0f * (float)bestk / ((float)NCLS - 1.0f) - 1.0f;     // :235
+          if (owns_fold && slot == 0 && cta == 0) p.out[(size_t)(p.f0 + fold) * p.out_pitch + t] = x;
         }
-        x = 2.0f * (float)bestk / ((float)NCLS - 1.0f) - 1.0f;     // :235
-        if (owns_fold && cta == 0) p.out[(size_t)(p.f0 + fold) * p.out_pitch + t] = x;
       }
       if (profiling) { tprof[4] += clock64() - tp0; }
       // no early exit on abort: every wait is bounded and fails fast once the abort flag is up, and the
@@ -693,14 +756,14 @@ class TcEngine : public Engine {
       uint16_t* q = reinterpret_cast<uint16_t*>(base + (OFF_Q - OFF_S1));
       float* fv = reinterpret_cast<float*>(base + (OFF_VEC - OFF_S1));
       for (int k = 0; k < H; ++k) {
-        for (int r = 0; r < 7 * U; ++r) s1[img_index(r, k, H)] = cvt(s.S1[(size_t)r * H + k]);
-        for (int r = 0; r < 4 * U; ++r) s2[img_index(r, k, H)] = cvt(s.S2[(size_t)r * H + k]);
-        for (int r = 0; r < U; ++r) s3[img_index(r, k, H)] = cvt(s.S3[(size_t)r * H + k]);
-        if (raw) { for (int r = 0; r < U; ++r) f3[img_index(r, k, H)] = cvt(w.f3w[(size_t)(c * U + r) * H + k]); }
+        for (int r = 0; r < 7 * U; ++r) s1[img_index(tcol(r / U, r % U), k, H)] = cvt(s.S1[(size_t)r * H + k]);
+        for (int r = 0; r < 4 * U; ++r) s2[img_index(tcol(r / U, r % U), k, H)] = cvt(s.S2[(size_t)r * H + k]);
+        for (int r = 0; r < U; ++r) s3[img_index(tcol(0, r), k, H)] = cvt(s.S3[(size_t)r * H + k]);
+        if (raw) { for (int r = 0; r < U; ++r) f3[img_index(tcol(0, r), k, H)] = cvt(w.f3w[(size_t)(c * U + r) * H + k]); }
         else for (int r = 0; r < cfg.n_classes; ++r) f3[img_index(r, k, H)] = cvt(w.f3w[(size_t)r * H + k]);
       }
       for (int k = 0; k < CDIM; ++k)
-        for (int r = 0; r < 8 * U; ++r) q[img_index(r, k, CDIM)] = cvt(s.Q[(size_t)r * CDIM + k]);
+        for (int r = 0; r < 8 * U; ++r) q[img_index(tcol(r / U, r % U), k, CDIM)] = cvt(s.Q[(size_t)r * CDIM + k]);
       for (int r = 0; r < 8 * U; ++r) { fv[r] = s.qk[r]; fv[32 + r] = s.vq[r]; }
       for (int r = 0; r < 3 * U; ++r) { fv[64 + r] = s.b1h[r]; fv[76 + r] = s.b2h[r]; }
       if (raw) { for (int r = 0; r < U; ++r) fv[88 + r] = w.f3b[c * U + r]; }

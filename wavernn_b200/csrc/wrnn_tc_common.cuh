@@ -127,6 +127,13 @@ template <> __device__ __forceinline__ uint32_t pack2<1>(float a, float b) {    
   const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<const uint32_t*>(&v);
 }
+template <int FMT> __device__ __forceinline__ uint16_t pack1(float a);             // one value, same rounding as pack2
+template <> __device__ __forceinline__ uint16_t pack1<0>(float a) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(r) : "f"(a));
+  return r;
+}
+template <> __device__ __forceinline__ uint16_t pack1<1>(float a) { return __bfloat16_as_ushort(__float2bfloat16_rn(a)); }
 
 // Epilogue transcendentals on the SFU (ex2/rcp/lg2 approx).  For the GRU gates their error is ~1e-6 relative, two
 // orders below the fp16 operand rounding of the contractions.  __logf, however, is documented to an ABSOLUTE 2^-21.41
@@ -149,7 +156,10 @@ __device__ __forceinline__ void mol_noise_fast(const float* u, float* gn, float&
   for (int k = 0; k < 10; ++k) gn[k] = __logf(-__logf(u[k]));
   lu = __logf(u[10]) - __logf(1.0f - u[10]);
 }
-__device__ __forceinline__ float mol_sample_noise(const float* lg, const float* gn, float lu) {
+// mol_pick: the mixture component (first maximum of logit - Gumbel term, :107-108); mol_finish: the logistic sample of
+// that component from its mean and log-scale (:110-121).  A caller holding only the 10 mixture logits reads the chosen
+// mean and log-scale by index.
+__device__ __forceinline__ int mol_pick(const float* lg, const float* gn) {
   int best = 0;
   float bestv = -INFINITY;
 #pragma unroll
@@ -157,12 +167,19 @@ __device__ __forceinline__ float mol_sample_noise(const float* lg, const float* 
     const float g = lg[k] - gn[k];
     if (g > bestv) { bestv = g; best = k; }
   }
-  float mean = lg[10], ls = lg[20];
-#pragma unroll
-  for (int k = 1; k < 10; ++k) { if (best == k) { mean = lg[10 + k]; ls = lg[20 + k]; } }
+  return best;
+}
+__device__ __forceinline__ float mol_finish(float mean, float ls, float lu) {
   ls = fmaxf(ls, -32.23619130191664f);
   const float x = mean + __expf(ls) * lu;
   return fminf(fmaxf(x, -1.0f), 1.0f);
+}
+__device__ __forceinline__ float mol_sample_noise(const float* lg, const float* gn, float lu) {
+  const int best = mol_pick(lg, gn);
+  float mean = lg[10], ls = lg[20];
+#pragma unroll
+  for (int k = 1; k < 10; ++k) { if (best == k) { mean = lg[10 + k]; ls = lg[20 + k]; } }
+  return mol_finish(mean, ls, lu);
 }
 __device__ __forceinline__ float mol_sample_fast(const float* lg, const float* u) {
   float gn[10], lu;
