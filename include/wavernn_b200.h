@@ -173,7 +173,8 @@ int wrnn_check(wrnn_t *h);
 
 /* Convenience for non-torch callers: same job but mels_up / aux / uniforms / expo /
  * out / x_force / logits_out are HOST pointers; copies in, runs, copies out and
- * synchronises.                                                                    */
+ * synchronises.  It takes per-sample conditioning rows; a caller holding a mel
+ * spectrogram and no conditioning network uses wrnn_vocode_host below.             */
 int wrnn_generate_host(wrnn_t *h, const wrnn_job *job);
 
 /* Introspection: name of the engine serving the handle ("simt", "tcgen05"), number
@@ -203,6 +204,72 @@ int wrnn_expand_conditioning(const float *mel_frames, const float *aux_frames, c
 int wrnn_epilogue(const float *samples, int32_t n_seg, int32_t seg_len, int64_t seg_stride, int32_t overlap,
                   const double *fade_in, const double *fade_out, const double *mu_table, int32_t n_classes,
                   const double *tail, int64_t tail_len, int64_t wave_len, double *wav, void *stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * From a mel spectrogram, without PyTorch: the conditioning network (MelResNet, fatchord_version.py:26-48) and the
+ * rest of generate() (:169-264) restated in the library.  A caller holding a state_dict exported as plain float32
+ * arrays attaches the `upsample.*` tensors once, then vocodes mels.  Draws are the in-kernel Philox ones
+ * (generate(gen_rng='philox')); there is no torch generator to replay.
+ * --------------------------------------------------------------------------------------------------------------- */
+
+/* One state_dict entry: its key and its fp32 values, row-major as torch stores them (host or device pointer). */
+typedef struct {
+  const char *name;
+  const float *data;
+  int64_t numel;
+} wrnn_tensor;
+
+/* The UpsampleNetwork arguments of the WaveRNN ctor (hparams voc_*).  feat_dims is the handle's (80). */
+typedef struct {
+  int32_t compute_dims;   /* 128 */
+  int32_t res_out_dims;   /* 128 (= 4 * aux_dims) */
+  int32_t res_blocks;     /* 10 */
+  int32_t pad;            /* 2 */
+  int32_t n_factors;      /* 3 */
+  int32_t factors[4];     /* (5, 5, 11) */
+  int32_t hop_length;     /* 275 == product of the factors */
+} wrnn_upsample_cfg;
+
+/* Reads the upsample.* tensors among t[0..n) by their state_dict keys (entries outside upsample.* and the BatchNorms'
+ * num_batches_tracked are ignored), folds each eval-mode BatchNorm (eps 1e-5) into the convolution before it -- in
+ * double, on the host -- builds the 5-tap interpolation table of the three stretch + conv stages and uploads both.
+ * Refused (WRNN_E_INVALID): a missing, repeated or unknown upsample.* key or one with the wrong number of elements
+ * (the message names it); compute_dims or res_out_dims other than 128; a geometry the 5-tap table does not encode
+ * (pad != 2, product of the factors != hop_length, or an impulse response wider than +-2 frames).  Replaces any
+ * upsampler attached before.                                                                                     */
+int wrnn_attach_upsampler(wrnn_t *h, const wrnn_upsample_cfg *cfg, const wrnn_tensor *t, int32_t n);
+
+/* The frame-rate conditioning of wrnn_job from a mel spectrogram, on the device (fp32 FFMA, no tensor cores):
+ *   mel        [feat, T]          the layout of the reference's mel .npy (gen_wavernn.py)
+ *   mel_frames [T + 2*pad, feat]  the zero-padded mel, transposed (F.pad(mel, (pad, pad))[0].T)
+ *   aux_frames [T, res_out]       MelResNet output, transposed
+ *   up_taps    [hop, 5]           the interpolation table; NULL when not wanted
+ * All DEVICE pointers; asynchronous on `stream`.                                                                 */
+int wrnn_conditioning_frames(wrnn_t *h, const float *mel, int64_t T, float *mel_frames, float *aux_frames,
+                             float *up_taps, void *stream);
+
+/* generate(mel, None, batched, target, overlap, mu_law) with gen_rng='philox', as one call: fold geometry
+ * (fold_with_overlap, :319-338; one fold of T*hop samples when unbatched), wrnn_conditioning_frames into handle
+ * scratch, the sample loop on the engine wrnn_generate would pick (Philox keyed by philox_seed, offset 0, folds
+ * numbered from 0), and wrnn_epilogue with float64 fade, fade-out and mu-law tables built on the host with the
+ * reference's expressions.  A handle whose engine is the SIMT one (fp32 strict arithmetic) takes the per-sample
+ * rows: they are expanded into scratch first, 832 B per sample of T*hop.                                        */
+typedef struct {
+  const float *mel;        /* [feat, T]                                                          */
+  int64_t T;               /* mel frames, >= 21 (the fade-out spans the last 20 hops)            */
+  int32_t batched;         /* fold with overlap (1) or one fold for the whole stream (0)         */
+  int32_t target;          /* samples per fold (batched)                                         */
+  int32_t overlap;         /* cross-faded samples between folds (batched; > 0)                   */
+  int32_t mu_law;          /* RAW head: labels are mu-law codes (ignored by the MoL head)        */
+  uint64_t philox_seed;    /* key of the in-kernel draws (WaveRNN.gen_philox_seed)               */
+  double *wav;             /* [(T - 1) * hop] float64                                            */
+} wrnn_vocode_job;
+
+/* DEVICE pointers; asynchronous on `stream`, no host synchronisation (device errors: wrnn_check after a sync).
+ * Refused: T < 21, a batched job with target <= 0 or overlap <= 0, a handle with no upsampler attached.        */
+int wrnn_vocode(wrnn_t *h, const wrnn_vocode_job *job, void *stream);
+/* The same with HOST mel and wav: copies in, runs, copies out, synchronises and returns wrnn_check's verdict. */
+int wrnn_vocode_host(wrnn_t *h, const wrnn_vocode_job *job);
 
 /* Host helper for parity mode: replays torch's default CPU generator (MT19937) natively, so the
  * draws the reference makes before / inside its loop cost a few ms instead of ~30.

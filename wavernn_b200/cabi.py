@@ -21,7 +21,8 @@ ABI_VERSION = 5
 
 EXPORTS = ("wrnn_abi_version", "wrnn_last_error", "wrnn_create", "wrnn_destroy", "wrnn_generate",
            "wrnn_check", "wrnn_generate_host", "wrnn_engine_name", "wrnn_grid_ctas", "wrnn_launch_count",
-           "wrnn_mt19937_uniform", "wrnn_mt19937_uniform_cols", "wrnn_epilogue", "wrnn_expand_conditioning")
+           "wrnn_mt19937_uniform", "wrnn_mt19937_uniform_cols", "wrnn_epilogue", "wrnn_expand_conditioning",
+           "wrnn_attach_upsampler", "wrnn_conditioning_frames", "wrnn_vocode", "wrnn_vocode_host")
 
 _fp = C.POINTER(C.c_float)
 
@@ -55,6 +56,20 @@ class WrnnJob(C.Structure):
                 ("fold_row0", C.c_void_p), ("fold_row_end", C.c_void_p),
                 ("mel_frames", C.c_void_p), ("aux_frames", C.c_void_p), ("up_taps", C.c_void_p),
                 ("hop", C.c_int32), ("cond_mode", C.c_int32), ("uniforms_ready", C.c_void_p)]
+
+
+class WrnnTensor(C.Structure):
+    _fields_ = [("name", C.c_char_p), ("data", C.c_void_p), ("numel", C.c_int64)]
+
+
+class WrnnUpsampleCfg(C.Structure):
+    _fields_ = [("compute_dims", C.c_int32), ("res_out_dims", C.c_int32), ("res_blocks", C.c_int32), ("pad", C.c_int32),
+                ("n_factors", C.c_int32), ("factors", C.c_int32 * 4), ("hop_length", C.c_int32)]
+
+
+class WrnnVocodeJob(C.Structure):
+    _fields_ = [("mel", C.c_void_p), ("T", C.c_int64), ("batched", C.c_int32), ("target", C.c_int32),
+                ("overlap", C.c_int32), ("mu_law", C.c_int32), ("philox_seed", C.c_uint64), ("wav", C.c_void_p)]
 
 
 _lib = None
@@ -104,6 +119,23 @@ def load() -> C.CDLL:
     lib.wrnn_mt19937_uniform_cols.restype = C.c_int32
     lib.wrnn_mt19937_uniform_cols.argtypes = [C.c_void_p, C.c_int32, C.c_uint64, C.c_void_p, C.c_uint64, C.c_uint64,
                                               C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64, C.c_float, C.c_float]
+    lib.wrnn_attach_upsampler.restype = C.c_int
+    lib.wrnn_attach_upsampler.argtypes = [C.c_void_p, C.POINTER(WrnnUpsampleCfg), C.POINTER(WrnnTensor), C.c_int32]
+    lib.wrnn_conditioning_frames.restype = C.c_int
+    lib.wrnn_conditioning_frames.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.wrnn_vocode.restype = C.c_int
+    lib.wrnn_vocode.argtypes = [C.c_void_p, C.POINTER(WrnnVocodeJob), C.c_void_p]
+    lib.wrnn_vocode_host.restype = C.c_int
+    lib.wrnn_vocode_host.argtypes = [C.c_void_p, C.POINTER(WrnnVocodeJob)]
+    # test hooks (not declared in the header)
+    lib.wrnn_debug_fold_geometry.restype = C.c_int
+    lib.wrnn_debug_fold_geometry.argtypes = [C.c_int64, C.c_int32, C.c_int64, C.c_int64, C.c_void_p]
+    lib.wrnn_debug_epilogue_tables.restype = C.c_int
+    lib.wrnn_debug_epilogue_tables.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                               C.c_void_p, C.c_void_p]
+    lib.wrnn_debug_upsampler.restype = C.c_int
+    lib.wrnn_debug_upsampler.argtypes = [C.POINTER(WrnnUpsampleCfg), C.POINTER(WrnnTensor), C.c_int32, C.c_void_p,
+                                         C.POINTER(C.c_uint64), C.c_void_p]
     if lib.wrnn_abi_version() != ABI_VERSION:
         raise RuntimeError(f"wavernn_b200: ABI mismatch (lib {lib.wrnn_abi_version()} != binding {ABI_VERSION})")
     _lib = lib
@@ -191,6 +223,45 @@ class Engine:
         _check(self.lib, self.lib.wrnn_generate_host(self._h, C.byref(job)))
         return (out, logits) if want_logits else out
 
+    # ---- from a mel, through the library alone (wrnn_attach_upsampler / wrnn_vocode) ----
+    def attach_upsampler(self, state_dict: dict, *, compute_dims=128, res_out_dims=128, res_blocks=10, pad=2,
+                         upsample_factors=(5, 5, 11), hop_length=275):
+        """wrnn_attach_upsampler with the `upsample.*` entries of `state_dict` (torch tensors on any device, or numpy
+        arrays); the WaveRNN ctor arguments of the same names describe the network."""
+        cfg = upsample_cfg(compute_dims=compute_dims, res_out_dims=res_out_dims, res_blocks=res_blocks, pad=pad,
+                           upsample_factors=upsample_factors, hop_length=hop_length)
+        arr, keep = tensor_list(state_dict)
+        _check(self.lib, self.lib.wrnn_attach_upsampler(self._h, C.byref(cfg), arr, len(arr)))
+        del keep
+        self.hop_length = int(hop_length)
+
+    def conditioning_frames(self, *, mel: int, T: int, mel_frames: int, aux_frames: int, up_taps: int = 0, stream: int = 0):
+        """wrnn_conditioning_frames with raw device addresses: mel [80, T] -> mel_frames [T+4, 80], aux_frames [T, 128]
+        (and up_taps [hop, 5] unless 0).  Asynchronous on `stream`."""
+        _check(self.lib, self.lib.wrnn_conditioning_frames(self._h, mel, int(T), mel_frames, aux_frames, up_taps or None,
+                                                           stream or None))
+
+    def vocode(self, *, mel: int, T: int, wav: int, batched: bool = True, target: int = 11000, overlap: int = 550,
+               mu_law: bool = False, philox_seed: int = 0, stream: int = 0):
+        """wrnn_vocode with raw device addresses: mel [80, T] fp32 -> wav [(T-1)*hop] float64.  Asynchronous."""
+        job = WrnnVocodeJob(mel, int(T), int(bool(batched)), int(target), int(overlap), int(bool(mu_law)), int(philox_seed), wav)
+        _check(self.lib, self.lib.wrnn_vocode(self._h, C.byref(job), C.c_void_p(stream or None)))
+
+    def vocode_host(self, mel, *, batched: bool = True, target: int = 11000, overlap: int = 550, mu_law: bool = False,
+                    philox_seed: int = 0):
+        """wrnn_vocode_host: mel (80, T) numpy -> float64 waveform of (T-1)*hop samples, what generate(mel[None], None,
+        batched, target, overlap, mu_law) returns with gen_rng='philox' -- without torch."""
+        import numpy as np
+        mel = np.ascontiguousarray(mel, dtype=np.float32)
+        if mel.ndim == 3 and mel.shape[0] == 1:
+            mel = mel[0]
+        T = mel.shape[-1]
+        wav = np.empty(max(T - 1, 0) * getattr(self, "hop_length", 275), dtype=np.float64)
+        job = WrnnVocodeJob(mel.ctypes.data, int(T), int(bool(batched)), int(target), int(overlap), int(bool(mu_law)),
+                            int(philox_seed), wav.ctypes.data)
+        _check(self.lib, self.lib.wrnn_vocode_host(self._h, C.byref(job)))
+        return wav
+
     def check(self):
         _check(self.lib, self.lib.wrnn_check(self._h))
 
@@ -209,6 +280,38 @@ class Engine:
 def _torch():
     import torch
     return torch
+
+
+def upsample_cfg(*, compute_dims=128, res_out_dims=128, res_blocks=10, pad=2, upsample_factors=(5, 5, 11),
+                 hop_length=275) -> WrnnUpsampleCfg:
+    f = tuple(int(x) for x in upsample_factors)
+    if not 1 <= len(f) <= 4:
+        raise ValueError("the C ABI takes 1 to 4 upsample factors")
+    return WrnnUpsampleCfg(compute_dims, res_out_dims, res_blocks, pad, len(f), (C.c_int32 * 4)(*(f + (0,) * (4 - len(f)))),
+                           hop_length)
+
+
+def tensor_list(state_dict: dict):
+    """The `upsample.*` entries of a state_dict as a wrnn_tensor array (fp32, contiguous; torch tensors keep their
+    device, numpy arrays are host memory).  Returns (array, objects to keep alive for the call)."""
+    import numpy as np
+    keep, items = [], []
+    for k, v in state_dict.items():
+        if not k.startswith("upsample."):
+            continue
+        if hasattr(v, "data_ptr"):
+            v = v.detach().float().contiguous()
+            ptr, n = v.data_ptr(), v.numel()
+        else:
+            v = np.ascontiguousarray(v, dtype=np.float32)
+            ptr, n = v.ctypes.data, v.size
+        name = k.encode()
+        keep += [v, name]
+        items.append((name, ptr, n))
+    arr = (WrnnTensor * max(len(items), 1))()
+    for i, (name, ptr, n) in enumerate(items):
+        arr[i] = WrnnTensor(name, ptr, n)
+    return (arr if items else (WrnnTensor * 0)()), keep
 
 
 def expand_conditioning(*, mel_frames: int, aux_frames: int, up_taps: int, hop: int, row_lo: int, n_rows: int,

@@ -7,6 +7,7 @@
 #include <string>
 #include <vector>
 
+#include "wrnn_cond.h"
 #include "wrnn_engine.h"
 #include "wrnn_stream_plan.h"
 
@@ -138,6 +139,7 @@ void wrnn_destroy(wrnn_t* h) {
   delete h->fallback;
   delete h->stream;
   delete h->host_weights;
+  destroy_upsampler(h->upsampler);
   delete h;
 }
 
@@ -236,6 +238,134 @@ int wrnn_expand_conditioning(const float* mel_frames, const float* aux_frames, c
     return WRNN_E_INVALID;
   }
   return expand_conditioning(mel_frames, aux_frames, up_taps, hop, row_lo, n_rows, mels_up, aux, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------------
+// wrnn_vocode: generate(gen_rng='philox') restated -- the frame-rate branch of WaveRNN._run_segments and the device branch
+// of WaveRNN._finish, with the conditioning network of wrnn_cond.cu in place of torch's.
+// ---------------------------------------------------------------------------------------------------------------------
+static int grow(void** buf, size_t* bytes, size_t want) {
+  if (want <= *bytes) return WRNN_OK;
+  if (*buf) cudaFree(*buf);
+  *buf = nullptr; *bytes = 0;
+  WRNN_CUDA_OK(cudaMalloc(buf, want));
+  *bytes = want;
+  return WRNN_OK;
+}
+
+static int validate_vocode(const wrnn_t* h, const wrnn_vocode_job* job) {
+  if (!h || !h->engine || !job) { set_error("null handle or job"); return WRNN_E_INVALID; }
+  if (!h->upsampler) { set_error("no upsampler attached (wrnn_attach_upsampler)"); return WRNN_E_INVALID; }
+  if (!job->mel || !job->wav) { set_error("mel and wav are required"); return WRNN_E_INVALID; }
+  if (job->T < 21) { set_error("T must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples"); return WRNN_E_INVALID; }
+  if (job->T * h->upsampler->hop >= (1ll << 31)) { set_error("stream longer than 2^31 samples"); return WRNN_E_INVALID; }
+  if (job->batched && (job->target <= 0 || job->overlap <= 0)) {
+    set_error("a batched job needs target > 0 and overlap > 0"); return WRNN_E_INVALID;
+  }
+  return WRNN_OK;
+}
+
+static size_t align_floats(size_t n) { return (n + 63) & ~size_t(63); }   // 256-byte aligned regions
+
+static int vocode(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st) {
+  Upsampler& u = *h->upsampler;
+  const int hop = u.hop;
+  const long long T = job->T, L = T * hop, wave_len = (T - 1) * hop;
+  const cond::Geometry g = cond::fold_geometry(L, job->batched != 0, job->target, job->overlap);
+  if (g.n_seg < 1 || g.n_seg >= (1ll << 31) || g.seg_len >= (1ll << 31)) {
+    set_error("target / overlap give no fold, or folds beyond 2^31"); return WRNN_E_INVALID;
+  }
+  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
+
+  wrnn_job j;
+  std::memset(&j, 0, sizeof(j));
+  j.L = L; j.seg_stride = g.seg_stride; j.n_seg = (int32_t)g.n_seg; j.seg_len = (int32_t)g.seg_len;
+  j.philox_seed = job->philox_seed;
+  j.hop = hop; j.cond_mode = WRNN_COND_AUTO;
+  j.mel_frames = j.aux_frames = j.up_taps = reinterpret_cast<const float*>(&u);   // placeholders: only tested against NULL
+  Engine* e = nullptr;
+  // the SIMT engine takes per-sample rows: pick_engine refuses the frame-rate job on a handle that has no other engine
+  const bool expanded = pick_engine(h, &j, &e) != WRNN_OK;
+  if (expanded) {
+    j.mel_frames = j.aux_frames = j.up_taps = nullptr;
+    j.mels_up = j.aux = reinterpret_cast<const float*>(&u);
+    const int rc = pick_engine(h, &j, &e);
+    if (rc != WRNN_OK) return rc;
+  }
+
+  const size_t n_mf = align_floats((size_t)(T + 4) * FEAT), n_af = align_floats((size_t)T * cond::CD);
+  const size_t n_smp = align_floats((size_t)g.n_seg * g.seg_len);
+  const size_t n_rows = expanded ? align_floats((size_t)L * FEAT) + align_floats((size_t)L * 4 * AUXD) : 0;
+  int rc = grow(&u.d_scratch, &u.scratch_bytes, (n_mf + n_af + n_smp + n_rows) * sizeof(float));
+  if (rc != WRNN_OK) return rc;
+  float* mel_frames = static_cast<float*>(u.d_scratch);
+  float* aux_frames = mel_frames + n_mf;
+  float* samples = aux_frames + n_af;
+
+  const bool mu_law = job->mu_law && h->engine->cfg.mode == WRNN_MODE_RAW;
+  const int ov = (int)g.overlap, nc = h->engine->cfg.n_classes;
+  if (u.tabs_key[0] != ov || u.tabs_key[1] != (mu_law ? 1 : 0) || u.tabs_key[2] != nc) {
+    u.tabs_key[0] = u.tabs_key[1] = u.tabs_key[2] = -1;
+    std::vector<double> fi, fo, mu, tail;
+    cond::epilogue_tables(ov, mu_law, nc, hop, fi, fo, mu, tail);
+    u.host_tabs.clear();
+    for (const auto* v : {&fi, &fo, &mu, &tail}) u.host_tabs.insert(u.host_tabs.end(), v->begin(), v->end());
+    if (u.host_tabs.size() > u.tabs_len) {
+      if (u.d_tabs) cudaFree(u.d_tabs);
+      u.d_tabs = nullptr; u.tabs_len = 0;
+      WRNN_CUDA_OK(cudaMalloc(&u.d_tabs, u.host_tabs.size() * sizeof(double)));
+      u.tabs_len = u.host_tabs.size();
+    }
+    WRNN_CUDA_OK(cudaMemcpyAsync(u.d_tabs, u.host_tabs.data(), u.host_tabs.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    u.tabs_key[0] = ov; u.tabs_key[1] = mu_law ? 1 : 0; u.tabs_key[2] = nc;
+  }
+  const double* fade_in = ov ? u.d_tabs : nullptr;
+  const double* fade_out = ov ? u.d_tabs + ov : nullptr;
+  const double* mu_table = mu_law ? u.d_tabs + 2 * ov : nullptr;
+  const double* tail = u.d_tabs + 2 * ov + (mu_law ? nc : 0);
+
+  if ((rc = conditioning_frames(u, job->mel, T, mel_frames, aux_frames, nullptr, st)) != WRNN_OK) return rc;
+  if (expanded) {
+    float* mels_up = samples + n_smp;
+    float* aux = mels_up + align_floats((size_t)L * FEAT);
+    if ((rc = expand_conditioning(mel_frames, aux_frames, u.d_taps, hop, 0, L, mels_up, aux, st)) != WRNN_OK) return rc;
+    j.mels_up = mels_up; j.aux = aux;
+  } else {
+    j.mel_frames = mel_frames; j.aux_frames = aux_frames; j.up_taps = u.d_taps;
+  }
+  j.out = samples;
+  h->last = e;
+  if ((rc = e->generate(j, st)) != WRNN_OK) return rc;
+  return wrnn_epilogue(samples, j.n_seg, j.seg_len, j.seg_stride, ov, fade_in, fade_out, mu_table, nc, tail, 20ll * hop,
+                       wave_len, job->wav, st);
+}
+
+extern "C" {
+
+int wrnn_vocode(wrnn_t* h, const wrnn_vocode_job* job, void* stream) {
+  const int rc = validate_vocode(h, job);
+  if (rc != WRNN_OK) return rc;
+  return vocode(h, job, static_cast<cudaStream_t>(stream));
+}
+
+int wrnn_vocode_host(wrnn_t* h, const wrnn_vocode_job* job) {
+  int rc = validate_vocode(h, job);
+  if (rc != WRNN_OK) return rc;
+  Upsampler& u = *h->upsampler;
+  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
+  const size_t n_mel = align_floats((size_t)job->T * FEAT), n_wav = (size_t)(job->T - 1) * u.hop;
+  if ((rc = grow(&u.d_stage, &u.stage_bytes, n_mel * sizeof(float) + n_wav * sizeof(double))) != WRNN_OK) return rc;
+  float* d_mel = static_cast<float*>(u.d_stage);
+  double* d_wav = reinterpret_cast<double*>(d_mel + n_mel);
+  WRNN_CUDA_OK(cudaMemcpyAsync(d_mel, job->mel, (size_t)job->T * FEAT * sizeof(float), cudaMemcpyHostToDevice, 0));
+  wrnn_vocode_job dj = *job;
+  dj.mel = d_mel; dj.wav = d_wav;
+  if ((rc = vocode(h, &dj, 0)) != WRNN_OK) return rc;
+  WRNN_CUDA_OK(cudaMemcpyAsync(job->wav, d_wav, n_wav * sizeof(double), cudaMemcpyDeviceToHost, 0));
+  WRNN_CUDA_OK(cudaStreamSynchronize(0));
+  return h->last->check();
 }
 
 // Test hook (CPU-only, no device needed): the stream engine's packed weight stream and step program for host-resident

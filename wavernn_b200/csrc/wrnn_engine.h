@@ -52,6 +52,9 @@ int make_stream_engine(const wrnn_cfg& cfg, const HostWeights& w, int device, En
 int expand_conditioning(const float* mel_frames, const float* aux_frames, const float* up_taps, int hop, long long row_lo,
                         long long n_rows, float* mels_up, float* aux, cudaStream_t stream);
 
+struct Upsampler;                                // conditioning network on the device (wrnn_cond.h)
+void destroy_upsampler(Upsampler* u);
+
 }  // namespace wrnn
 
 struct wrnn_handle {
@@ -65,4 +68,6 @@ struct wrnn_handle {
   // staging for wrnn_generate_host
   void* d_stage = nullptr;
   size_t stage_bytes = 0;
+  // wrnn_attach_upsampler: folded MelResNet, tap table and the scratch of wrnn_vocode
+  wrnn::Upsampler* upsampler = nullptr;
 };
