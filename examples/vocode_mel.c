@@ -1,7 +1,11 @@
-/* vocode_mel.c -- vocode one mel spectrogram through the C ABI alone: include/wavernn_b200.h, libwavernn_b200.so and
+/* vocode_mel.c -- vocode mel spectrograms through the C ABI alone: include/wavernn_b200.h, libwavernn_b200.so and
  * libc; no Python, no PyTorch.  Built by wavernn_b200/csrc/Makefile into wavernn_b200/wrnn_vocode_mel.
  *
- *   wrnn_vocode_mel WEIGHTS_DIR MEL OUT [name=value ...]
+ *   wrnn_vocode_mel WEIGHTS_DIR MEL OUT [MEL OUT ...] [name=value ...]
+ *
+ * One MEL OUT pair is vocoded with wrnn_vocode_host.  Several pairs are vocoded as one batch with wrnn_vocode_many_host,
+ * utterance i keyed by seed + i (each waveform is then what a single call with that seed gives on the same engine).
+ * The options are the arguments that contain '=' (so a MEL or OUT path must not).
  *
  * WEIGHTS_DIR holds one raw little-endian float32 file per state_dict key, named "<key>.f32" (INTEGRATION.md section 2:
  * `for k, v in sd.items(): v.float().numpy().astype('<f4').tofile(f'{dir}/{k}.f32')`).  MEL is raw float32 [80, T],
@@ -47,15 +51,22 @@ static int load_key(const char *dir, const char *key, wrnn_tensor *t) {
   return t->data ? 0 : -1;
 }
 
+static int first_opt = 2;            /* index of the first name=value argument */
+
 static const char *opt(int argc, char **argv, const char *name, const char *dflt) {
   size_t n = strlen(name);
-  for (int i = 4; i < argc; ++i)
+  for (int i = first_opt; i < argc; ++i)
     if (!strncmp(argv[i], name, n) && argv[i][n] == '=') return argv[i] + n + 1;
   return dflt;
 }
 
 int main(int argc, char **argv) {
-  if (argc < 4) { fprintf(stderr, "usage: %s WEIGHTS_DIR MEL OUT [name=value ...]\n", argv[0]); return 2; }
+  while (first_opt < argc && !strchr(argv[first_opt], '=')) ++first_opt;
+  const int n_utts = (first_opt - 2) / 2;
+  if (n_utts < 1 || (first_opt - 2) % 2) {
+    fprintf(stderr, "usage: %s WEIGHTS_DIR MEL OUT [MEL OUT ...] [name=value ...]\n", argv[0]);
+    return 2;
+  }
   const char *dir = argv[1];
   const int raw = !strcmp(opt(argc, argv, "mode", "MOL"), "RAW");
   const char *prec = opt(argc, argv, "precision", "fp16"), *eng = opt(argc, argv, "engine", "auto");
@@ -104,25 +115,45 @@ int main(int argc, char **argv) {
     return 1;
   }
 
-  int64_t mel_numel = 0;
-  float *mel = read_f32(argv[2], &mel_numel);
-  if (!mel || mel_numel % 80) { fprintf(stderr, "the mel file must hold [80, T] float32\n"); return 1; }
-  const int64_t T = mel_numel / 80, wave_len = (T - 1) * 275;
-  double *wav = malloc((size_t)(wave_len > 0 ? wave_len : 1) * sizeof(double));
-  wrnn_vocode_job job = {mel, T, atoi(opt(argc, argv, "batched", "1")), atoi(opt(argc, argv, "target", "11000")),
-                         atoi(opt(argc, argv, "overlap", "550")), atoi(opt(argc, argv, "mu_law", "1")),
-                         strtoull(opt(argc, argv, "seed", "0"), NULL, 10), wav};
-  if ((rc = wrnn_vocode_host(h, &job)) != WRNN_OK) {
-    fprintf(stderr, "wrnn_vocode_host: %d %s\n", rc, wrnn_last_error());
-    return 1;
+  const int batched = atoi(opt(argc, argv, "batched", "1")), target = atoi(opt(argc, argv, "target", "11000"));
+  const int overlap = atoi(opt(argc, argv, "overlap", "550")), mu_law = atoi(opt(argc, argv, "mu_law", "1"));
+  const uint64_t seed = strtoull(opt(argc, argv, "seed", "0"), NULL, 10);
+  wrnn_utterance *u = calloc((size_t)n_utts, sizeof(wrnn_utterance));
+  if (!u) { fprintf(stderr, "out of memory\n"); return 1; }
+  for (int i = 0; i < n_utts; ++i) {
+    int64_t mel_numel = 0;
+    float *mel = read_f32(argv[2 + 2 * i], &mel_numel);
+    if (!mel || mel_numel % 80) { fprintf(stderr, "the mel file %s must hold [80, T] float32\n", argv[2 + 2 * i]); return 1; }
+    const int64_t T = mel_numel / 80, wave_len = (T - 1) * 275;
+    u[i].mel = mel;
+    u[i].T = T;
+    u[i].philox_seed = seed + (uint64_t)i;
+    u[i].wav = malloc((size_t)(wave_len > 0 ? wave_len : 1) * sizeof(double));
   }
-  FILE *f = fopen(argv[3], "wb");
-  if (!f || fwrite(wav, sizeof(double), (size_t)wave_len, f) != (size_t)wave_len) { fprintf(stderr, "cannot write %s\n", argv[3]); return 1; }
-  fclose(f);
-  printf("%lld samples (%s engine)\n", (long long)wave_len, wrnn_engine_name(h));
+  if (n_utts == 1) {
+    wrnn_vocode_job job = {u[0].mel, u[0].T, batched, target, overlap, mu_law, seed, u[0].wav};
+    if ((rc = wrnn_vocode_host(h, &job)) != WRNN_OK) {
+      fprintf(stderr, "wrnn_vocode_host: %d %s\n", rc, wrnn_last_error());
+      return 1;
+    }
+  } else {
+    wrnn_vocode_batch b = {u, n_utts, batched, target, overlap, mu_law};
+    if ((rc = wrnn_vocode_many_host(h, &b)) != WRNN_OK) {
+      fprintf(stderr, "wrnn_vocode_many_host: %d %s\n", rc, wrnn_last_error());
+      return 1;
+    }
+  }
+  for (int i = 0; i < n_utts; ++i) {
+    const int64_t wave_len = (u[i].T - 1) * 275;
+    const char *out = argv[3 + 2 * i];
+    FILE *f = fopen(out, "wb");
+    if (!f || fwrite(u[i].wav, sizeof(double), (size_t)wave_len, f) != (size_t)wave_len) { fprintf(stderr, "cannot write %s\n", out); return 1; }
+    fclose(f);
+    printf("%lld samples (%s engine)\n", (long long)wave_len, wrnn_engine_name(h));
+  }
   wrnn_destroy(h);
   for (int i = 0; i < n; ++i) free((void *)t[i].data);
-  free(mel);
-  free(wav);
+  for (int i = 0; i < n_utts; ++i) { free((void *)u[i].mel); free(u[i].wav); }
+  free(u);
   return 0;
 }

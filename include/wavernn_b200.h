@@ -271,6 +271,44 @@ int wrnn_vocode(wrnn_t *h, const wrnn_vocode_job *job, void *stream);
 /* The same with HOST mel and wav: copies in, runs, copies out, synchronises and returns wrnn_check's verdict. */
 int wrnn_vocode_host(wrnn_t *h, const wrnn_vocode_job *job);
 
+/* A batch of mels as ONE job: one launch of the conditioning network, one engine job over the folds of every utterance
+ * (folds ordered by utterance, then ascending; one tile-launch per 64 folds on TCGEN05, one launch on STREAM) and one
+ * epilogue launch.  A step of the sample loop costs about the same for 1 fold as for 64, so k short utterances cost
+ * about as much as one.
+ *
+ * Contract: utterance i's waveform is bit-identical to wrnn_vocode on the same handle with {mel_i, T_i, batched,
+ * target, overlap, mu_law, philox_seed_i} whenever the batch and that single call are served by the same engine: each
+ * fold's draws are keyed by (its utterance's philox_seed, its index within the utterance), not by its place in the
+ * batch.  A handle created with a fixed engine (TCGEN05, STREAM, SIMT) always serves both with that engine.  An AUTO
+ * handle routes the batch by its TOTAL fold count with wrnn_generate's rule (MoL jobs of 257 folds or more go to the
+ * stream engine), so a batch can land on another engine than its single calls; its waveforms then agree with them
+ * to DESIGN.md section 5's tolerances, not bit for bit.
+ *
+ * Unbatched (batched = 0): each utterance is one fold and every fold runs max_i(T_i) * hop steps; a shorter
+ * utterance's fold runs past its end on zero conditioning and those samples are discarded (the recurrence is causal,
+ * so its first T_i * hop samples are unchanged).  That costs sum_i (max T - T_i) * hop wasted fold-steps.
+ *
+ * Refused (WRNN_E_INVALID, the handle stays usable): n_utts < 1 or > 65535, a null utts / mel / wav, any T_i < 21
+ * (the message names i), a batched job with target <= 0 or overlap <= 0, a laid-out stream of 2^31 samples or more
+ * (sum_i (T_i + 4) * hop), a total of 2^31 folds or more, a handle with no upsampler attached.                  */
+typedef struct {
+  const float *mel;        /* [feat, T], the layout of wrnn_vocode_job::mel */
+  int64_t T;               /* >= 21                                          */
+  uint64_t philox_seed;    /* this utterance's key                           */
+  double *wav;             /* [(T - 1) * hop] float64                        */
+} wrnn_utterance;
+
+typedef struct {
+  const wrnn_utterance *utts;   /* HOST array of n_utts descriptors (mel / wav: device or host per entry point) */
+  int32_t n_utts;
+  int32_t batched, target, overlap, mu_law;   /* shared, meaning as in wrnn_vocode_job */
+} wrnn_vocode_batch;
+
+/* DEVICE mel / wav pointers; asynchronous on `stream` (device errors: wrnn_check after a sync). */
+int wrnn_vocode_many(wrnn_t *h, const wrnn_vocode_batch *b, void *stream);
+/* The same with HOST mel / wav: copies in, runs, copies out, synchronises and returns wrnn_check's verdict. */
+int wrnn_vocode_many_host(wrnn_t *h, const wrnn_vocode_batch *b);
+
 /* Host helper for parity mode: replays torch's default CPU generator (MT19937) natively, so the
  * draws the reference makes before / inside its loop cost a few ms instead of ~30.
  *   state : the generator's 624 words and its position `pos` in [0, 624] (624 = block exhausted)

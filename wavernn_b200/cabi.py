@@ -22,7 +22,8 @@ ABI_VERSION = 5
 EXPORTS = ("wrnn_abi_version", "wrnn_last_error", "wrnn_create", "wrnn_destroy", "wrnn_generate",
            "wrnn_check", "wrnn_generate_host", "wrnn_engine_name", "wrnn_grid_ctas", "wrnn_launch_count",
            "wrnn_mt19937_uniform", "wrnn_mt19937_uniform_cols", "wrnn_epilogue", "wrnn_expand_conditioning",
-           "wrnn_attach_upsampler", "wrnn_conditioning_frames", "wrnn_vocode", "wrnn_vocode_host")
+           "wrnn_attach_upsampler", "wrnn_conditioning_frames", "wrnn_vocode", "wrnn_vocode_host",
+           "wrnn_vocode_many", "wrnn_vocode_many_host")
 
 _fp = C.POINTER(C.c_float)
 
@@ -70,6 +71,23 @@ class WrnnUpsampleCfg(C.Structure):
 class WrnnVocodeJob(C.Structure):
     _fields_ = [("mel", C.c_void_p), ("T", C.c_int64), ("batched", C.c_int32), ("target", C.c_int32),
                 ("overlap", C.c_int32), ("mu_law", C.c_int32), ("philox_seed", C.c_uint64), ("wav", C.c_void_p)]
+
+
+class WrnnUtterance(C.Structure):
+    _fields_ = [("mel", C.c_void_p), ("T", C.c_int64), ("philox_seed", C.c_uint64), ("wav", C.c_void_p)]
+
+
+class WrnnVocodeBatch(C.Structure):
+    _fields_ = [("utts", C.POINTER(WrnnUtterance)), ("n_utts", C.c_int32), ("batched", C.c_int32), ("target", C.c_int32),
+                ("overlap", C.c_int32), ("mu_law", C.c_int32)]
+
+
+def vocode_batch(utts, *, batched=True, target=11000, overlap=550, mu_law=False):
+    """A wrnn_vocode_batch over `utts`, a list of (mel address, T, philox_seed, wav address) (0 = NULL).  Returns the
+    struct and the utterance array it points to (keep both alive for the call)."""
+    arr = (WrnnUtterance * max(len(utts), 1))(*[WrnnUtterance(m or None, int(T), int(s), w or None) for m, T, s, w in utts])
+    b = WrnnVocodeBatch(arr if utts else None, len(utts), int(bool(batched)), int(target), int(overlap), int(bool(mu_law)))
+    return b, arr
 
 
 _lib = None
@@ -127,7 +145,13 @@ def load() -> C.CDLL:
     lib.wrnn_vocode.argtypes = [C.c_void_p, C.POINTER(WrnnVocodeJob), C.c_void_p]
     lib.wrnn_vocode_host.restype = C.c_int
     lib.wrnn_vocode_host.argtypes = [C.c_void_p, C.POINTER(WrnnVocodeJob)]
+    lib.wrnn_vocode_many.restype = C.c_int
+    lib.wrnn_vocode_many.argtypes = [C.c_void_p, C.POINTER(WrnnVocodeBatch), C.c_void_p]
+    lib.wrnn_vocode_many_host.restype = C.c_int
+    lib.wrnn_vocode_many_host.argtypes = [C.c_void_p, C.POINTER(WrnnVocodeBatch)]
     # test hooks (not declared in the header)
+    lib.wrnn_debug_vocode_many_plan.restype = C.c_int
+    lib.wrnn_debug_vocode_many_plan.argtypes = [C.c_int32, C.POINTER(WrnnVocodeBatch), C.c_void_p, C.c_void_p, C.c_void_p]
     lib.wrnn_debug_fold_geometry.restype = C.c_int
     lib.wrnn_debug_fold_geometry.argtypes = [C.c_int64, C.c_int32, C.c_int64, C.c_int64, C.c_void_p]
     lib.wrnn_debug_epilogue_tables.restype = C.c_int
@@ -261,6 +285,31 @@ class Engine:
                             int(philox_seed), wav.ctypes.data)
         _check(self.lib, self.lib.wrnn_vocode_host(self._h, C.byref(job)))
         return wav
+
+    def vocode_many(self, *, mels, Ts, seeds, wavs, batched: bool = True, target: int = 11000, overlap: int = 550,
+                    mu_law: bool = False, stream: int = 0):
+        """wrnn_vocode_many with raw device addresses: utterance i is mels[i] [80, Ts[i]] fp32 -> wavs[i]
+        [(Ts[i]-1)*hop] float64, keyed by seeds[i].  One job for the whole batch.  Asynchronous."""
+        b, keep = vocode_batch(list(zip(mels, Ts, seeds, wavs)), batched=batched, target=target, overlap=overlap,
+                               mu_law=mu_law)
+        _check(self.lib, self.lib.wrnn_vocode_many(self._h, C.byref(b), C.c_void_p(stream or None)))
+        del keep
+
+    def vocode_many_host(self, mels, seeds, *, batched: bool = True, target: int = 11000, overlap: int = 550,
+                         mu_law: bool = False):
+        """wrnn_vocode_many_host: a list of numpy mels (80, T_i) and one Philox seed per mel -> the list of float64
+        waveforms, each bit-identical to vocode_host(mel_i, philox_seed=seeds[i]) on a handle with a fixed engine."""
+        import numpy as np
+        mels = [np.ascontiguousarray(m[0] if m.ndim == 3 and m.shape[0] == 1 else m, dtype=np.float32) for m in mels]
+        if len(seeds) != len(mels):
+            raise ValueError("one seed per mel")
+        hop = getattr(self, "hop_length", 275)
+        wavs = [np.empty(max(m.shape[-1] - 1, 0) * hop, dtype=np.float64) for m in mels]
+        b, keep = vocode_batch([(m.ctypes.data, m.shape[-1], s, w.ctypes.data) for m, s, w in zip(mels, seeds, wavs)],
+                               batched=batched, target=target, overlap=overlap, mu_law=mu_law)
+        _check(self.lib, self.lib.wrnn_vocode_many_host(self._h, C.byref(b)))
+        del keep
+        return wavs
 
     def check(self):
         _check(self.lib, self.lib.wrnn_check(self._h))

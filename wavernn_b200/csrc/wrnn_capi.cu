@@ -169,7 +169,7 @@ int wrnn_generate(wrnn_t* h, const wrnn_job* job, void* stream) {
   Engine* e = nullptr;
   if ((rc = pick_engine(h, job, &e)) != WRNN_OK) return rc;
   h->last = e;
-  return e->generate(*job, static_cast<cudaStream_t>(stream));
+  return e->generate(*job, static_cast<cudaStream_t>(stream), nullptr);
 }
 
 int wrnn_check(wrnn_t* h) {
@@ -216,7 +216,7 @@ int wrnn_generate_host(wrnn_t* h, const wrnn_job* job) {
     cudaMemcpyAsync(t0 + B, job->fold_row_end, B * 8, cudaMemcpyHostToDevice, 0);
     dj.fold_row0 = t0; dj.fold_row_end = t0 + B;
   }
-  rc = e->generate(dj, 0);
+  rc = e->generate(dj, 0, nullptr);
   if (rc != WRNN_OK) return rc;
   WRNN_CUDA_OK(cudaMemcpyAsync(job->out, dj.out, n_out * sizeof(float), cudaMemcpyDeviceToHost, 0));
   if (n_log) WRNN_CUDA_OK(cudaMemcpyAsync(job->logits_out, dj.logits_out, n_log * sizeof(float), cudaMemcpyDeviceToHost, 0));
@@ -269,6 +269,46 @@ static int validate_vocode(const wrnn_t* h, const wrnn_vocode_job* job) {
 
 static size_t align_floats(size_t n) { return (n + 63) & ~size_t(63); }   // 256-byte aligned regions
 
+// The engine of a vocode job (frame-rate conditioning).  The SIMT engine takes per-sample rows: pick_engine refuses the
+// frame-rate job on a handle that has no other engine, and *expanded tells the caller to expand the rows into scratch.
+static int pick_vocode_engine(wrnn_t* h, wrnn_job& j, Engine** e, bool* expanded) {
+  const void* tag = h->upsampler;                      // placeholders: only tested against NULL
+  j.mel_frames = j.aux_frames = j.up_taps = static_cast<const float*>(tag);
+  *expanded = pick_engine(h, &j, e) != WRNN_OK;
+  if (!*expanded) return WRNN_OK;
+  j.mel_frames = j.aux_frames = j.up_taps = nullptr;
+  j.mels_up = j.aux = static_cast<const float*>(tag);
+  return pick_engine(h, &j, e);
+}
+
+// fade_in / fade_out / mu / tail of the epilogue on the device, rebuilt and uploaded only when (overlap, mu_law,
+// n_classes) changes.
+struct EpTables { const double *fade_in, *fade_out, *mu, *tail; };
+static int epilogue_tables(wrnn_t* h, int ov, bool mu_law, cudaStream_t st, EpTables* t) {
+  Upsampler& u = *h->upsampler;
+  const int nc = h->engine->cfg.n_classes;
+  if (u.tabs_key[0] != ov || u.tabs_key[1] != (mu_law ? 1 : 0) || u.tabs_key[2] != nc) {
+    u.tabs_key[0] = u.tabs_key[1] = u.tabs_key[2] = -1;
+    std::vector<double> fi, fo, mu, tail;
+    cond::epilogue_tables(ov, mu_law, nc, u.hop, fi, fo, mu, tail);
+    u.host_tabs.clear();
+    for (const auto* v : {&fi, &fo, &mu, &tail}) u.host_tabs.insert(u.host_tabs.end(), v->begin(), v->end());
+    if (u.host_tabs.size() > u.tabs_len) {
+      if (u.d_tabs) cudaFree(u.d_tabs);
+      u.d_tabs = nullptr; u.tabs_len = 0;
+      WRNN_CUDA_OK(cudaMalloc(&u.d_tabs, u.host_tabs.size() * sizeof(double)));
+      u.tabs_len = u.host_tabs.size();
+    }
+    WRNN_CUDA_OK(cudaMemcpyAsync(u.d_tabs, u.host_tabs.data(), u.host_tabs.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    u.tabs_key[0] = ov; u.tabs_key[1] = mu_law ? 1 : 0; u.tabs_key[2] = nc;
+  }
+  t->fade_in = ov ? u.d_tabs : nullptr;
+  t->fade_out = ov ? u.d_tabs + ov : nullptr;
+  t->mu = mu_law ? u.d_tabs + 2 * ov : nullptr;
+  t->tail = u.d_tabs + 2 * ov + (mu_law ? nc : 0);
+  return WRNN_OK;
+}
+
 static int vocode(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st) {
   Upsampler& u = *h->upsampler;
   const int hop = u.hop;
@@ -284,21 +324,15 @@ static int vocode(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st) {
   j.L = L; j.seg_stride = g.seg_stride; j.n_seg = (int32_t)g.n_seg; j.seg_len = (int32_t)g.seg_len;
   j.philox_seed = job->philox_seed;
   j.hop = hop; j.cond_mode = WRNN_COND_AUTO;
-  j.mel_frames = j.aux_frames = j.up_taps = reinterpret_cast<const float*>(&u);   // placeholders: only tested against NULL
   Engine* e = nullptr;
-  // the SIMT engine takes per-sample rows: pick_engine refuses the frame-rate job on a handle that has no other engine
-  const bool expanded = pick_engine(h, &j, &e) != WRNN_OK;
-  if (expanded) {
-    j.mel_frames = j.aux_frames = j.up_taps = nullptr;
-    j.mels_up = j.aux = reinterpret_cast<const float*>(&u);
-    const int rc = pick_engine(h, &j, &e);
-    if (rc != WRNN_OK) return rc;
-  }
+  bool expanded = false;
+  int rc = pick_vocode_engine(h, j, &e, &expanded);
+  if (rc != WRNN_OK) return rc;
 
   const size_t n_mf = align_floats((size_t)(T + 4) * FEAT), n_af = align_floats((size_t)T * cond::CD);
   const size_t n_smp = align_floats((size_t)g.n_seg * g.seg_len);
   const size_t n_rows = expanded ? align_floats((size_t)L * FEAT) + align_floats((size_t)L * 4 * AUXD) : 0;
-  int rc = grow(&u.d_scratch, &u.scratch_bytes, (n_mf + n_af + n_smp + n_rows) * sizeof(float));
+  rc = grow(&u.d_scratch, &u.scratch_bytes, (n_mf + n_af + n_smp + n_rows) * sizeof(float));
   if (rc != WRNN_OK) return rc;
   float* mel_frames = static_cast<float*>(u.d_scratch);
   float* aux_frames = mel_frames + n_mf;
@@ -306,25 +340,8 @@ static int vocode(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st) {
 
   const bool mu_law = job->mu_law && h->engine->cfg.mode == WRNN_MODE_RAW;
   const int ov = (int)g.overlap, nc = h->engine->cfg.n_classes;
-  if (u.tabs_key[0] != ov || u.tabs_key[1] != (mu_law ? 1 : 0) || u.tabs_key[2] != nc) {
-    u.tabs_key[0] = u.tabs_key[1] = u.tabs_key[2] = -1;
-    std::vector<double> fi, fo, mu, tail;
-    cond::epilogue_tables(ov, mu_law, nc, hop, fi, fo, mu, tail);
-    u.host_tabs.clear();
-    for (const auto* v : {&fi, &fo, &mu, &tail}) u.host_tabs.insert(u.host_tabs.end(), v->begin(), v->end());
-    if (u.host_tabs.size() > u.tabs_len) {
-      if (u.d_tabs) cudaFree(u.d_tabs);
-      u.d_tabs = nullptr; u.tabs_len = 0;
-      WRNN_CUDA_OK(cudaMalloc(&u.d_tabs, u.host_tabs.size() * sizeof(double)));
-      u.tabs_len = u.host_tabs.size();
-    }
-    WRNN_CUDA_OK(cudaMemcpyAsync(u.d_tabs, u.host_tabs.data(), u.host_tabs.size() * sizeof(double), cudaMemcpyHostToDevice, st));
-    u.tabs_key[0] = ov; u.tabs_key[1] = mu_law ? 1 : 0; u.tabs_key[2] = nc;
-  }
-  const double* fade_in = ov ? u.d_tabs : nullptr;
-  const double* fade_out = ov ? u.d_tabs + ov : nullptr;
-  const double* mu_table = mu_law ? u.d_tabs + 2 * ov : nullptr;
-  const double* tail = u.d_tabs + 2 * ov + (mu_law ? nc : 0);
+  EpTables tabs;
+  if ((rc = epilogue_tables(h, ov, mu_law, st, &tabs)) != WRNN_OK) return rc;
 
   if ((rc = conditioning_frames(u, job->mel, T, mel_frames, aux_frames, nullptr, st)) != WRNN_OK) return rc;
   if (expanded) {
@@ -337,9 +354,89 @@ static int vocode(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st) {
   }
   j.out = samples;
   h->last = e;
-  if ((rc = e->generate(j, st)) != WRNN_OK) return rc;
-  return wrnn_epilogue(samples, j.n_seg, j.seg_len, j.seg_stride, ov, fade_in, fade_out, mu_table, nc, tail, 20ll * hop,
-                       wave_len, job->wav, st);
+  if ((rc = e->generate(j, st, nullptr)) != WRNN_OK) return rc;
+  return wrnn_epilogue(samples, j.n_seg, j.seg_len, j.seg_stride, ov, tabs.fade_in, tabs.fade_out, tabs.mu, nc, tabs.tail,
+                       20ll * hop, wave_len, job->wav, st);
+}
+
+// wrnn_vocode_many: the batch as one job (layout: cond::batch_plan).  `b` holds DEVICE mel / wav pointers.
+static int vocode_many(wrnn_t* h, const wrnn_vocode_batch* b, const cond::BatchPlan& pl, cudaStream_t st) {
+  Upsampler& u = *h->upsampler;
+  const int hop = u.hop, n = b->n_utts;
+  const size_t nf = (size_t)pl.g.n_seg;
+  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
+
+  wrnn_job j;
+  std::memset(&j, 0, sizeof(j));
+  j.L = pl.L; j.seg_stride = pl.g.seg_stride; j.n_seg = (int32_t)nf; j.seg_len = (int32_t)pl.g.seg_len;
+  j.hop = hop; j.cond_mode = WRNN_COND_AUTO;
+  const void* tag = h->upsampler;                      // placeholders: only tested against NULL
+  j.fold_row0 = j.fold_row_end = static_cast<const int64_t*>(tag);
+  Engine* e = nullptr;
+  bool expanded = false;
+  int rc = pick_vocode_engine(h, j, &e, &expanded);
+  if (rc != WRNN_OK) return rc;
+
+  // scratch: [row0 | row_end | keys | CondUtt table | EpUtt table | mel_frames | aux_frames | samples | expanded rows]
+  // The frame regions span every utterance's T + 4 frames (aux_frames included, so that no row of the laid-out stream
+  // maps outside them); the tables go up in one copy.
+  const size_t n_frames = (size_t)pl.frame0.back();
+  const size_t b_row = align_floats(2 * nf) * 4, b_key = align_floats(4 * nf) * 4;
+  const size_t b_cu = align_floats(n * sizeof(CondUtt) / 4 + 1) * 4, b_eu = align_floats(n * sizeof(EpUtt) / 4 + 1) * 4;
+  const size_t b_tab = 2 * b_row + b_key + b_cu + b_eu;
+  const size_t n_mf = align_floats(n_frames * FEAT), n_af = align_floats(n_frames * cond::CD), n_smp = align_floats(nf * pl.g.seg_len);
+  const size_t n_rows = expanded ? align_floats((size_t)pl.L * FEAT) + align_floats((size_t)pl.L * 4 * AUXD) : 0;
+  rc = grow(&u.d_scratch, &u.scratch_bytes, b_tab + (n_mf + n_af + n_smp + n_rows) * sizeof(float));
+  if (rc != WRNN_OK) return rc;
+  unsigned char* d = static_cast<unsigned char*>(u.d_scratch);
+  float* mel_frames = reinterpret_cast<float*>(d + b_tab);
+  float* aux_frames = mel_frames + n_mf;
+  float* samples = aux_frames + n_af;
+
+  u.host_plan.assign(b_tab, 0);
+  unsigned char* hp = u.host_plan.data();
+  std::memcpy(hp, pl.row0.data(), nf * 8);
+  std::memcpy(hp + b_row, pl.row_end.data(), nf * 8);
+  std::memcpy(hp + 2 * b_row, pl.keys.data(), nf * sizeof(FoldKey));
+  CondUtt* cu = reinterpret_cast<CondUtt*>(hp + 2 * b_row + b_key);
+  EpUtt* eu = reinterpret_cast<EpUtt*>(hp + 2 * b_row + b_key + b_cu);
+  for (int i = 0; i < n; ++i) {
+    cu[i] = CondUtt{b->utts[i].mel, b->utts[i].T, pl.frame0[i]};
+    eu[i] = EpUtt{pl.fold0[i], (int)(pl.fold0[i + 1] - pl.fold0[i]), (b->utts[i].T - 1) * hop, b->utts[i].wav};
+  }
+  WRNN_CUDA_OK(cudaMemcpyAsync(d, hp, b_tab, cudaMemcpyHostToDevice, st));
+  j.fold_row0 = reinterpret_cast<const int64_t*>(d);
+  j.fold_row_end = reinterpret_cast<const int64_t*>(d + b_row);
+  const FoldKey* keys = reinterpret_cast<const FoldKey*>(d + 2 * b_row);
+  const CondUtt* d_cu = reinterpret_cast<const CondUtt*>(d + 2 * b_row + b_key);
+  const EpUtt* d_eu = reinterpret_cast<const EpUtt*>(d + 2 * b_row + b_key + b_cu);
+
+  const bool mu_law = b->mu_law && h->engine->cfg.mode == WRNN_MODE_RAW;
+  const int ov = (int)pl.g.overlap;
+  EpTables tabs;
+  if ((rc = epilogue_tables(h, ov, mu_law, st, &tabs)) != WRNN_OK) return rc;
+
+  if ((rc = conditioning_frames_batch(u, d_cu, n, pl.max_T, mel_frames, aux_frames, st)) != WRNN_OK) return rc;
+  if (expanded) {
+    // rows [0, L - 4*hop): the last utterance's 4*hop gap rows would read frames past the end and no fold reads them
+    float* mels_up = samples + n_smp;
+    float* aux = mels_up + align_floats((size_t)pl.L * FEAT);
+    if ((rc = expand_conditioning(mel_frames, aux_frames, u.d_taps, hop, 0, pl.L - 4ll * hop, mels_up, aux, st)) != WRNN_OK) return rc;
+    j.mels_up = mels_up; j.aux = aux;
+  } else {
+    j.mel_frames = mel_frames; j.aux_frames = aux_frames; j.up_taps = u.d_taps;
+  }
+  j.out = samples;
+  h->last = e;
+  if ((rc = e->generate(j, st, keys)) != WRNN_OK) return rc;
+  return epilogue_launch(samples, j.seg_len, j.seg_stride, ov, tabs.fade_in, tabs.fade_out, tabs.mu, h->engine->cfg.n_classes,
+                         tabs.tail, 20ll * hop, d_eu, EpUtt{0, 0, 0, nullptr}, n, pl.max_wave, st);
+}
+
+static int validate_many(const wrnn_t* h, const wrnn_vocode_batch* b, cond::BatchPlan& pl) {
+  if (!h || !h->engine || !b) { set_error("null handle or batch"); return WRNN_E_INVALID; }
+  if (!h->upsampler) { set_error("no upsampler attached (wrnn_attach_upsampler)"); return WRNN_E_INVALID; }
+  return cond::batch_plan(h->upsampler->hop, *b, pl);
 }
 
 extern "C" {
@@ -364,6 +461,42 @@ int wrnn_vocode_host(wrnn_t* h, const wrnn_vocode_job* job) {
   dj.mel = d_mel; dj.wav = d_wav;
   if ((rc = vocode(h, &dj, 0)) != WRNN_OK) return rc;
   WRNN_CUDA_OK(cudaMemcpyAsync(job->wav, d_wav, n_wav * sizeof(double), cudaMemcpyDeviceToHost, 0));
+  WRNN_CUDA_OK(cudaStreamSynchronize(0));
+  return h->last->check();
+}
+
+int wrnn_vocode_many(wrnn_t* h, const wrnn_vocode_batch* b, void* stream) {
+  cond::BatchPlan pl;
+  const int rc = validate_many(h, b, pl);
+  if (rc != WRNN_OK) return rc;
+  return vocode_many(h, b, pl, static_cast<cudaStream_t>(stream));
+}
+
+int wrnn_vocode_many_host(wrnn_t* h, const wrnn_vocode_batch* b) {
+  cond::BatchPlan pl;
+  int rc = validate_many(h, b, pl);
+  if (rc != WRNN_OK) return rc;
+  Upsampler& u = *h->upsampler;
+  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
+  const int n = b->n_utts;
+  std::vector<size_t> mel_off(n + 1, 0);
+  for (int i = 0; i < n; ++i) mel_off[i + 1] = mel_off[i] + align_floats((size_t)b->utts[i].T * FEAT);
+  const size_t n_wav = (size_t)pl.wav0.back();
+  if ((rc = grow(&u.d_stage, &u.stage_bytes, mel_off[n] * sizeof(float) + n_wav * sizeof(double))) != WRNN_OK) return rc;
+  float* d_mel = static_cast<float*>(u.d_stage);
+  double* d_wav = reinterpret_cast<double*>(d_mel + mel_off[n]);
+  std::vector<wrnn_utterance> du(b->utts, b->utts + n);
+  for (int i = 0; i < n; ++i) {
+    WRNN_CUDA_OK(cudaMemcpyAsync(d_mel + mel_off[i], b->utts[i].mel, (size_t)b->utts[i].T * FEAT * sizeof(float), cudaMemcpyHostToDevice, 0));
+    du[i].mel = d_mel + mel_off[i];
+    du[i].wav = d_wav + pl.wav0[i];
+  }
+  wrnn_vocode_batch db = *b;
+  db.utts = du.data();
+  if ((rc = vocode_many(h, &db, pl, 0)) != WRNN_OK) return rc;
+  for (int i = 0; i < n; ++i)
+    WRNN_CUDA_OK(cudaMemcpyAsync(b->utts[i].wav, d_wav + pl.wav0[i], (size_t)(pl.wav0[i + 1] - pl.wav0[i]) * sizeof(double),
+                                 cudaMemcpyDeviceToHost, 0));
   WRNN_CUDA_OK(cudaStreamSynchronize(0));
   return h->last->check();
 }

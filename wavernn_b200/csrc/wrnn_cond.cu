@@ -67,14 +67,27 @@ __device__ __forceinline__ void store_tile(float* X, const float (&acc)[4][8], i
   }
 }
 
-// mel [FEAT, T] -> aux_frames [T, CD]; blob as cond::blob_len describes (fp32, transposed matrices)
-__global__ void __launch_bounds__(THREADS) melresnet_kernel(const float* __restrict__ mel, long long T, const float* __restrict__ blob,
-                                                            int res_blocks, float* __restrict__ aux_frames) {
+// Utterance blockIdx.y of the batch: utts[blockIdx.y], or `one` when the batch is a single utterance (utts == NULL).
+__device__ __forceinline__ CondUtt utt_of(const CondUtt* __restrict__ utts, const CondUtt& one, unsigned i) {
+  return utts ? utts[i] : one;
+}
+
+// mel [FEAT, T] -> aux_frames [T, CD] of each utterance (rows frame0 .. frame0 + T - 1); blob as cond::blob_len describes
+// (fp32, transposed matrices).  Grid: (tiles of TF frames of the longest utterance, utterances); a CTA serves one tile
+// of one utterance, and the CTAs past the end of a shorter utterance return at once.
+__global__ void __launch_bounds__(THREADS) melresnet_kernel(const CondUtt* __restrict__ utts, const CondUtt one,
+                                                            const float* __restrict__ blob, int res_blocks,
+                                                            float* __restrict__ aux_frames_all) {
   extern __shared__ __align__(16) float smem[];
   float* X = smem;                      // [CD][XS] activations of the tile
   float* Y = smem + CD * XS;            // [CD][XS] inner activations of a residual block
   float* M = Y;                         // [FEAT][XS] mel frames t0-2 .. t0+TF+1 (conv_in's receptive field)
+  const CondUtt ut = utt_of(utts, one, blockIdx.y);
+  const float* __restrict__ mel = ut.mel;
+  const long long T = ut.T;
   const long long t0 = (long long)blockIdx.x * TF;
+  if (t0 >= T) return;
+  float* __restrict__ aux_frames = aux_frames_all + (size_t)ut.frame0 * CD;
   const int o0 = (threadIdx.x & 31) * 4, f0 = (threadIdx.x >> 5) * 8;
 
   for (int e = threadIdx.x; e < FEAT * XS; e += THREADS) {
@@ -137,10 +150,18 @@ __global__ void __launch_bounds__(THREADS) melresnet_kernel(const float* __restr
   }
 }
 
-// mel [FEAT, T] -> mel_frames [T + 4, FEAT]: the zero-padded mel, transposed through a 32 x 32 shared tile
-__global__ void __launch_bounds__(256) pad_transpose_kernel(const float* __restrict__ mel, long long T, float* __restrict__ mel_frames) {
+// mel [FEAT, T] -> mel_frames [T + 4, FEAT] of each utterance (rows frame0 .. frame0 + T + 3): the zero-padded mel,
+// transposed through a 32 x 32 shared tile.  Grid: (32-frame tiles of the longest padded utterance, channel tiles,
+// utterances).
+__global__ void __launch_bounds__(256) pad_transpose_kernel(const CondUtt* __restrict__ utts, const CondUtt one,
+                                                            float* __restrict__ mel_frames_all) {
   __shared__ float tile[32][33];
+  const CondUtt ut = utt_of(utts, one, blockIdx.z);
+  const float* __restrict__ mel = ut.mel;
+  const long long T = ut.T;
   const long long r0 = (long long)blockIdx.x * 32;            // padded frame
+  if (r0 >= T + 4) return;
+  float* __restrict__ mel_frames = mel_frames_all + (size_t)ut.frame0 * FEAT;
   const int c0 = blockIdx.y * 32;                             // channel
   for (int i = threadIdx.y; i < 32; i += 8) {
     const int c = c0 + i;
@@ -318,6 +339,53 @@ Geometry fold_geometry(int64_t total_len, bool batched, int64_t target, int64_t 
   return Geometry{n, target + 2 * overlap, target + overlap, overlap, padded};
 }
 
+int batch_plan(int hop, const wrnn_vocode_batch& b, BatchPlan& out) {
+  if (b.n_utts < 1 || b.n_utts > 65535 || !b.utts) { set_error("a batch needs 1 to 65535 utterances and a non-null utts array"); return WRNN_E_INVALID; }
+  if (b.batched && (b.target <= 0 || b.overlap <= 0)) { set_error("a batched job needs target > 0 and overlap > 0"); return WRNN_E_INVALID; }
+  out = BatchPlan();
+  int64_t frames = 0, waves = 0;
+  for (int i = 0; i < b.n_utts; ++i) {
+    const wrnn_utterance& u = b.utts[i];
+    const std::string at = "utterance " + std::to_string(i) + ": ";
+    if (!u.mel || !u.wav) { set_error(at + "mel and wav are required"); return WRNN_E_INVALID; }
+    if (u.T < 21) { set_error(at + "T must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples"); return WRNN_E_INVALID; }
+    if (u.T >= (1ll << 31) / hop) { set_error(at + "stream longer than 2^31 samples"); return WRNN_E_INVALID; }
+    out.frame0.push_back(frames); out.wav0.push_back(waves);
+    frames += u.T + 4; waves += (u.T - 1) * hop;
+    if (frames * hop >= (1ll << 31)) { set_error("the laid-out stream of the batch is 2^31 samples or longer"); return WRNN_E_INVALID; }
+    if (u.T > out.max_T) out.max_T = u.T;
+  }
+  out.frame0.push_back(frames); out.wav0.push_back(waves);
+  out.L = frames * hop;
+  out.max_wave = (out.max_T - 1) * hop;
+  if (b.batched) {
+    out.g = Geometry{0, (int64_t)b.target + 2ll * b.overlap, (int64_t)b.target + b.overlap, b.overlap, 0};   // fold_with_overlap's
+    if (out.g.seg_len >= (1ll << 31)) { set_error("target + 2 * overlap must be below 2^31"); return WRNN_E_INVALID; }
+  } else {
+    out.g = Geometry{0, out.max_T * hop, out.max_T * hop, 0, 0};
+  }
+  int64_t folds = 0;
+  for (int i = 0; i < b.n_utts; ++i) {
+    const int64_t Ti = b.utts[i].T, n = b.batched ? fold_geometry(Ti * hop, true, b.target, b.overlap).n_seg : 1;
+    if (n < 1) { set_error("utterance " + std::to_string(i) + ": target / overlap give no fold"); return WRNN_E_INVALID; }
+    out.fold0.push_back(folds);
+    folds += n;
+    if (folds >= (1ll << 31)) { set_error("the batch has 2^31 folds or more"); return WRNN_E_INVALID; }
+  }
+  out.fold0.push_back(folds);
+  out.g.n_seg = folds;
+  out.row0.reserve(folds); out.row_end.reserve(folds); out.keys.reserve(folds);
+  for (int i = 0; i < b.n_utts; ++i) {
+    const int64_t R = out.frame0[i] * hop, end = R + b.utts[i].T * hop;
+    for (int64_t j = 0; j < out.fold0[i + 1] - out.fold0[i]; ++j) {
+      out.row0.push_back(R + (b.batched ? j * out.g.seg_stride : 0));
+      out.row_end.push_back(end);
+      out.keys.push_back(FoldKey{b.utts[i].philox_seed, (uint32_t)j, 0u});
+    }
+  }
+  return WRNN_OK;
+}
+
 void epilogue_tables(int overlap, bool mu_law, int n_classes, int hop, std::vector<double>& fade_in,
                      std::vector<double>& fade_out, std::vector<double>& mu, std::vector<double>& tail) {
   fade_in.clear(); fade_out.clear(); mu.clear();
@@ -383,15 +451,31 @@ int make_upsampler(const cond::HostUpsampler& hu, int device, Upsampler** out) {
   return WRNN_OK;
 }
 
+// Both kernels over a batch: the utterance table `utts` (device) or, for one utterance, `one` passed by value.
+static int launch_conditioning(const Upsampler& u, const CondUtt* utts, const CondUtt& one, int n_utts, long long max_T,
+                               float* mel_frames, float* aux_frames, cudaStream_t stream) {
+  using namespace cond;
+  pad_transpose_kernel<<<dim3((unsigned)((max_T + 4 + 31) / 32), (FEAT + 31) / 32, (unsigned)n_utts), dim3(32, 8), 0, stream>>>(
+      utts, one, mel_frames);
+  WRNN_CUDA_OK(cudaGetLastError());
+  melresnet_kernel<<<dim3((unsigned)((max_T + TF - 1) / TF), (unsigned)n_utts), THREADS, SMEM, stream>>>(utts, one, u.d_blob,
+                                                                                                      u.res_blocks, aux_frames);
+  WRNN_CUDA_OK(cudaGetLastError());
+  return WRNN_OK;
+}
+
 int conditioning_frames(const Upsampler& u, const float* mel, long long T, float* mel_frames, float* aux_frames, float* up_taps,
                         cudaStream_t stream) {
-  using namespace cond;
-  pad_transpose_kernel<<<dim3((unsigned)((T + 4 + 31) / 32), (FEAT + 31) / 32), dim3(32, 8), 0, stream>>>(mel, T, mel_frames);
-  WRNN_CUDA_OK(cudaGetLastError());
-  melresnet_kernel<<<(unsigned)((T + TF - 1) / TF), THREADS, SMEM, stream>>>(mel, T, u.d_blob, u.res_blocks, aux_frames);
-  WRNN_CUDA_OK(cudaGetLastError());
-  if (up_taps) WRNN_CUDA_OK(cudaMemcpyAsync(up_taps, u.d_taps, (size_t)u.hop * TAPS * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  const CondUtt one{mel, T, 0};
+  const int rc = launch_conditioning(u, nullptr, one, 1, T, mel_frames, aux_frames, stream);
+  if (rc != WRNN_OK) return rc;
+  if (up_taps) WRNN_CUDA_OK(cudaMemcpyAsync(up_taps, u.d_taps, (size_t)u.hop * cond::TAPS * sizeof(float), cudaMemcpyDeviceToDevice, stream));
   return WRNN_OK;
+}
+
+int conditioning_frames_batch(const Upsampler& u, const CondUtt* utts, int n_utts, long long max_T, float* mel_frames,
+                              float* aux_frames, cudaStream_t stream) {
+  return launch_conditioning(u, utts, CondUtt{nullptr, 0, 0}, n_utts, max_T, mel_frames, aux_frames, stream);
 }
 
 }  // namespace wrnn
@@ -430,6 +514,27 @@ int wrnn_debug_fold_geometry(int64_t total_len, int32_t batched, int64_t target,
   if (!out) { set_error("null argument"); return WRNN_E_INVALID; }
   const cond::Geometry g = cond::fold_geometry(total_len, batched != 0, target, overlap);
   out[0] = g.n_seg; out[1] = g.seg_len; out[2] = g.seg_stride; out[3] = g.overlap; out[4] = g.padded_len;
+  return WRNN_OK;
+}
+
+// The layout wrnn_vocode_many runs for batch b at this hop (cond::batch_plan), or its refusal.  geo[7] = n_seg, seg_len,
+// seg_stride, overlap, L (rows of the laid-out stream), max_T, total waveform samples; utt [n_utts][3] = frame0, fold0,
+// wav0 per utterance; folds [n_seg][4] = fold_row0, fold_row_end, key seed (bits of the uint64), key fold.  utt and
+// folds may be NULL (sizes first).  mel / wav are only tested against NULL.
+int wrnn_debug_vocode_many_plan(int32_t hop, const wrnn_vocode_batch* b, int64_t* geo, int64_t* utt, int64_t* folds) {
+  if (!b || !geo || hop <= 0) { set_error("null argument"); return WRNN_E_INVALID; }
+  cond::BatchPlan pl;
+  const int rc = cond::batch_plan(hop, *b, pl);
+  if (rc != WRNN_OK) return rc;
+  const int64_t g[7] = {pl.g.n_seg, pl.g.seg_len, pl.g.seg_stride, pl.g.overlap, pl.L, pl.max_T, pl.wav0.back()};
+  std::memcpy(geo, g, sizeof(g));
+  if (utt)
+    for (int i = 0; i < b->n_utts; ++i) { utt[3 * i] = pl.frame0[i]; utt[3 * i + 1] = pl.fold0[i]; utt[3 * i + 2] = pl.wav0[i]; }
+  if (folds)
+    for (int64_t f = 0; f < pl.g.n_seg; ++f) {
+      folds[4 * f] = pl.row0[f]; folds[4 * f + 1] = pl.row_end[f];
+      folds[4 * f + 2] = (int64_t)pl.keys[f].seed; folds[4 * f + 3] = pl.keys[f].fold;
+    }
   return WRNN_OK;
 }
 

@@ -40,6 +40,22 @@ struct Geometry {
 // fold_with_overlap's index math (fatchord_version.py:319-330); unbatched: one fold of total_len samples
 Geometry fold_geometry(int64_t total_len, bool batched, int64_t target, int64_t overlap);
 
+// The job wrnn_vocode_many runs, laid out on the host after the batch has been checked.  Utterance i's frames start
+// at frame0[i] = sum_{j<i} (T_j + 4) of mel_frames / aux_frames, its conditioning rows at hop * frame0[i]; its folds
+// are fold0[i] .. fold0[i+1] - 1 (batched: its own fold_with_overlap geometry; unbatched: one fold of max_T * hop steps),
+// with the fold tables of wrnn_job and the Philox key (philox_seed_i, index within the utterance).  wav0[i] is its
+// offset in the concatenation of the waveforms.
+struct BatchPlan {
+  Geometry g;                                 // seg_len, seg_stride, overlap shared; n_seg = folds of the whole batch
+  int64_t L = 0;                              // rows of the laid-out stream: hop * sum (T_i + 4)
+  int64_t max_T = 0, max_wave = 0;
+  std::vector<int64_t> frame0, fold0, wav0;   // [n_utts + 1] each (last entry: the totals)
+  std::vector<int64_t> row0, row_end;         // [n_seg]
+  std::vector<FoldKey> keys;                  // [n_seg]
+};
+// Checks the batch (WRNN_E_INVALID with a message naming the bad utterance) and lays it out.
+int batch_plan(int hop, const wrnn_vocode_batch& b, BatchPlan& out);
+
 // generate()'s float64 epilogue tables, with numpy's arithmetic (linspace = i*step + start, last element = stop):
 //   fade_in / fade_out [overlap] (xfade_and_unfold, :379-391; empty when overlap == 0), tail [20*hop] (:255),
 //   mu [n_classes] (decode_mu_law of the fp32 class values, utils/dsp.py:98-103; empty without mu_law)
@@ -56,6 +72,7 @@ struct Upsampler {
   void* d_scratch = nullptr;
   size_t scratch_bytes = 0;
   std::vector<double> host_tabs;        // [fade_in | fade_out | mu | tail], kept alive for the asynchronous upload
+  std::vector<unsigned char> host_plan; // wrnn_vocode_many: fold tables, keys and utterance tables, uploaded in one copy
   double* d_tabs = nullptr;
   size_t tabs_len = 0;
   long long tabs_key[3] = {-1, -1, -1}; // overlap, mu_law, n_classes of the tables in d_tabs
@@ -65,9 +82,21 @@ struct Upsampler {
   ~Upsampler();
 };
 
+// One utterance of a conditioning batch: mel [FEAT, T] (device); its padded mel and its MelResNet output are rows
+// frame0 .. frame0 + T + 3 of mel_frames and frame0 .. frame0 + T - 1 of aux_frames.
+struct CondUtt {
+  const float* mel;
+  long long T;
+  long long frame0;
+};
+
 int make_upsampler(const cond::HostUpsampler& hu, int device, Upsampler** out);
 // mel [FEAT, T] -> mel_frames [T + 4, FEAT], aux_frames [T, 128] (and up_taps [hop, 5] when not NULL); device, async
 int conditioning_frames(const Upsampler& u, const float* mel, long long T, float* mel_frames, float* aux_frames,
                         float* up_taps, cudaStream_t stream);
+// The same for n_utts utterances in one launch of each kernel: utts [n_utts] is a DEVICE table, max_T the longest T.
+// Each utterance's frames are bit-identical to its own conditioning_frames.
+int conditioning_frames_batch(const Upsampler& u, const CondUtt* utts, int n_utts, long long max_T, float* mel_frames,
+                              float* aux_frames, cudaStream_t stream);
 
 }  // namespace wrnn

@@ -7,6 +7,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "wrnn_fold.h"
+
 namespace wrnn {
 
 // -------------------------------------------------------------------------------------
@@ -104,6 +106,17 @@ __device__ __forceinline__ float u01_open(unsigned x) { return fminf(u01(x), 0x1
 // the reference's uniform_(1e-5, 1 - 1e-5): rand*(to-from)+from, contracted to one FFMA.  u01 = 1 maps to
 // 1 - 1e-5 (rounded), inside the reference's range, so the MoL draws keep the closed u01.
 __device__ __forceinline__ float u_ref_range(unsigned x) { return u01(x) * (1.0f - 2e-5f) + 1e-5f; }
+
+// Philox counter fold and key words of job fold f: the per-fold table when present (one 16-byte read-only load),
+// else (seg_first + f, philox_seed).
+struct FoldPhilox { unsigned fold, k0, k1; };
+__device__ __forceinline__ FoldPhilox fold_philox(const FoldKey* keys, int f, int seg_first, unsigned long long seed) {
+  if (keys) {
+    const ulonglong2 k = __ldg(reinterpret_cast<const ulonglong2*>(keys + f));
+    return FoldPhilox{(unsigned)k.y, (unsigned)k.x, (unsigned)(k.x >> 32)};
+  }
+  return FoldPhilox{(unsigned)(seg_first + f), (unsigned)seed, (unsigned)(seed >> 32)};
+}
 
 // -------------------------------------------------------------------------------------
 // samplers

@@ -32,7 +32,8 @@ inline int grid_stride_blocks(long long blocks) {
 class Engine {
  public:
   virtual ~Engine() {}
-  virtual int generate(const wrnn_job& job, cudaStream_t stream) = 0;   // async
+  // async; keys: optional per-fold Philox keys ([job.n_seg], device; NULL = keyed by seg_first + fold, philox_seed)
+  virtual int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) = 0;
   virtual int check() = 0;                                              // after stream sync
   virtual bool supports(const wrnn_job& job) const { (void)job; return true; }   // job inside this engine's envelope?
   virtual const char* name() const = 0;
@@ -51,6 +52,20 @@ int make_stream_engine(const wrnn_cfg& cfg, const HostWeights& w, int device, En
 // conditioning pre-pass (wrnn_tc.cu): rows [row_lo, row_lo + n_rows) of the per-sample stream from frame-rate tensors
 int expand_conditioning(const float* mel_frames, const float* aux_frames, const float* up_taps, int hop, long long row_lo,
                         long long n_rows, float* mels_up, float* aux, cudaStream_t stream);
+
+// One utterance of an epilogue batch: folds [fold0, fold0 + n_seg) of the sample block unfold into wav [wave_len].
+struct EpUtt {
+  long long fold0;
+  int n_seg;
+  long long wave_len;
+  double* wav;
+};
+// The epilogue (wrnn_epilogue.cu) over n_utts utterances in one launch: the table `utts` (device) or, with utts == NULL
+// and n_utts == 1, `one`.  max_wave_len: the longest wave_len.  Every utterance's samples are bit-identical to its own
+// wrnn_epilogue call.  Arguments are checked by the callers.
+int epilogue_launch(const float* samples, int seg_len, long long seg_stride, int overlap, const double* fade_in,
+                    const double* fade_out, const double* mu_table, int n_classes, const double* tail, long long tail_len,
+                    const EpUtt* utts, const EpUtt& one, int n_utts, long long max_wave_len, cudaStream_t stream);
 
 struct Upsampler;                                // conditioning network on the device (wrnn_cond.h)
 void destroy_upsampler(Upsampler* u);

@@ -19,15 +19,15 @@ namespace wrnn {
 namespace {
 
 struct EpParams {
-  const float* samples; int n_seg; int seg_len; long long seg_stride; int overlap;
+  const float* samples; int seg_len; long long seg_stride; int overlap;   // samples: [folds of every utterance, seg_len]
   const double* fade_in; const double* fade_out;      // [overlap] each (NULL when overlap == 0: unbatched)
   const double* mu_table; int n_classes;               // RAW + mu_law: expansion of label k (NULL = none)
-  const double* tail; long long tail_len;              // final fade-out over the last tail_len samples
-  long long wave_len; double* wav;
+  const double* tail; long long tail_len;              // final fade-out over the last tail_len samples of each utterance
+  const EpUtt* utts; EpUtt one;                        // utterance table (device), or the one utterance when utts == NULL
 };
 
-__device__ __forceinline__ double fold_value(const EpParams& p, int i, long long k) {
-  const float xf = __ldg(p.samples + (size_t)i * p.seg_len + k);
+__device__ __forceinline__ double fold_value(const EpParams& p, const float* s, int i, long long k) {
+  const float xf = __ldg(s + (size_t)i * p.seg_len + k);
   double y = (double)xf;
   if (p.mu_table) {                                     // x = 2k/(n-1) - 1  ->  label k (exact: labels are 2/(n-1) apart)
     int lbl = __float2int_rn((xf + 1.0f) * (0.5f * (float)(p.n_classes - 1)));
@@ -39,20 +39,36 @@ __device__ __forceinline__ double fold_value(const EpParams& p, int i, long long
   return y;
 }
 
+// Grid: (grid-stride blocks over the longest waveform, utterances); blockIdx.y unfolds utterance blockIdx.y alone.
 __global__ void __launch_bounds__(256) wrnn_epilogue_kernel(const EpParams p) {
-  for (long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x; n < p.wave_len; n += (long long)gridDim.x * blockDim.x) {
+  const EpUtt u = p.utts ? p.utts[blockIdx.y] : p.one;
+  const float* s = p.samples + (size_t)u.fold0 * p.seg_len;
+  for (long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x; n < u.wave_len; n += (long long)gridDim.x * blockDim.x) {
     long long i_hi = n / p.seg_stride;
-    if (i_hi > p.n_seg - 1) i_hi = p.n_seg - 1;
+    if (i_hi > u.n_seg - 1) i_hi = u.n_seg - 1;
     const long long k_hi = n - i_hi * p.seg_stride;
     double v = 0.0;                                      // unfolded = zeros; unfolded[...] += y[i], i ascending (:397-403)
-    if (i_hi >= 1 && k_hi + p.seg_stride < p.seg_len) v = __dadd_rn(v, fold_value(p, (int)i_hi - 1, k_hi + p.seg_stride));
-    if (k_hi < p.seg_len) v = __dadd_rn(v, fold_value(p, (int)i_hi, k_hi));
-    if (p.tail && n >= p.wave_len - p.tail_len) v = __dmul_rn(v, __ldg(p.tail + (n - (p.wave_len - p.tail_len))));   // (:255-258)
-    p.wav[n] = v;
+    if (i_hi >= 1 && k_hi + p.seg_stride < p.seg_len) v = __dadd_rn(v, fold_value(p, s, (int)i_hi - 1, k_hi + p.seg_stride));
+    if (k_hi < p.seg_len) v = __dadd_rn(v, fold_value(p, s, (int)i_hi, k_hi));
+    if (p.tail && n >= u.wave_len - p.tail_len) v = __dmul_rn(v, __ldg(p.tail + (n - (u.wave_len - p.tail_len))));   // (:255-258)
+    u.wav[n] = v;
   }
 }
 
 }  // namespace
+
+// Shared by wrnn_epilogue (one utterance, passed by value) and wrnn_vocode_many (a device table of n_utts utterances).
+int epilogue_launch(const float* samples, int seg_len, long long seg_stride, int overlap, const double* fade_in,
+                    const double* fade_out, const double* mu_table, int n_classes, const double* tail, long long tail_len,
+                    const EpUtt* utts, const EpUtt& one, int n_utts, long long max_wave_len, cudaStream_t stream) {
+  EpParams p{samples, seg_len, seg_stride, overlap, fade_in, fade_out, mu_table, n_classes, tail, tail_len, utts, one};
+  const long long blocks = (max_wave_len + 255) / 256;
+  const int grid = grid_stride_blocks(blocks);
+  wrnn_epilogue_kernel<<<dim3(grid, n_utts), 256, 0, stream>>>(p);
+  WRNN_CUDA_OK(cudaGetLastError());
+  return WRNN_OK;
+}
+
 }  // namespace wrnn
 
 extern "C" int wrnn_epilogue(const float* samples, int32_t n_seg, int32_t seg_len, int64_t seg_stride, int32_t overlap,
@@ -67,10 +83,6 @@ extern "C" int wrnn_epilogue(const float* samples, int32_t n_seg, int32_t seg_le
   if (wave_len > (int64_t)(n_seg - 1) * seg_stride + seg_len) { set_error("wrnn_epilogue: wave_len exceeds the unfolded length"); return WRNN_E_INVALID; }
   if (tail && (tail_len <= 0 || tail_len > wave_len)) { set_error("wrnn_epilogue: tail_len must be in (0, wave_len]"); return WRNN_E_INVALID; }
   if (mu_table && n_classes < 2) { set_error("wrnn_epilogue: n_classes"); return WRNN_E_INVALID; }
-  EpParams p{samples, n_seg, seg_len, seg_stride, overlap, fade_in, fade_out, mu_table, n_classes, tail, tail_len, wave_len, wav};
-  const long long blocks = (wave_len + 255) / 256;
-  const int grid = grid_stride_blocks(blocks);
-  wrnn_epilogue_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
-  WRNN_CUDA_OK(cudaGetLastError());
-  return WRNN_OK;
+  return epilogue_launch(samples, seg_len, seg_stride, overlap, fade_in, fade_out, mu_table, n_classes, tail, tail_len, nullptr,
+                         EpUtt{0, n_seg, wave_len, wav}, 1, wave_len, static_cast<cudaStream_t>(stream));
 }

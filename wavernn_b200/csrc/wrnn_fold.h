@@ -41,6 +41,15 @@ struct HostWeights {   // fp32 copies of the state_dict tensors, row-major [out,
   int n_classes = 0;
 };
 
+// Optional per-fold key of the in-kernel Philox draws (device table of n_seg entries, indexed by the job's fold).
+// Without the table, fold f of a job draws with (counter fold = seg_first + f, key = philox_seed); with it, with
+// (key[f].fold, key[f].seed) -- so a fold's draws follow its utterance, not its place in a batch (wrnn_vocode_many).
+struct alignas(16) FoldKey {
+  uint64_t seed;
+  uint32_t fold;
+  uint32_t pad;
+};
+
 // Dense folded model in double precision; row order is the reference's ([r,z,n] gate blocks).
 struct Folded {
   std::vector<double> v1, k1, v2, k2, v3, k3;        // G3, G3, G3, G3, H, H

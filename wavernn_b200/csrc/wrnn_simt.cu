@@ -53,6 +53,7 @@ struct SimtParams {
   const float* uniforms; const float* expo; unsigned long long seed, offset;
   float* out; const float* x_force; float* logits_out;
   const long long* fold_row0; const long long* fold_row_end;
+  const FoldKey* keys;   // optional per-fold Philox keys [n_seg]
   float* xch;      // 4 x [H][Bp]: h1', h2', y1, y2
   float* xs;       // [Bp] previous sample per fold
   float* state;    // [P][NSTATE][Bp]
@@ -278,8 +279,8 @@ __global__ void __launch_bounds__(NT, 1) wrnn_simt_kernel(const SimtParams p) {
               const float* ur = p.uniforms + (size_t)t * 11 * B;
               s = mol_sample(lget, [&](int i) { return i < 10 ? __ldg(ur + b * 10 + i) : __ldg(ur + 10 * B + b); });
             } else {
-              const unsigned g = (unsigned)(p.seg_first + b);
-              const unsigned k0 = (unsigned)p.seed, k1 = (unsigned)(p.seed >> 32);
+              const FoldPhilox k = fold_philox(p.keys, b, p.seg_first, p.seed);
+              const unsigned g = k.fold, k0 = k.k0, k1 = k.k1;
               const unsigned o0 = (unsigned)p.offset;
               const Philox4 r0 = philox4x32_10((unsigned)t, g, 0u, o0, k0, k1);
               const Philox4 r1 = philox4x32_10((unsigned)t, g, 1u, o0, k0, k1);
@@ -325,14 +326,14 @@ __global__ void __launch_bounds__(NT, 1) wrnn_simt_kernel(const SimtParams p) {
           for (int i = lane; i < NC; i += 32) sum += expf(__ldcg(p.xlog + (size_t)i * Bp + b) - mx);
           for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
           float bestq = -1.f; int besti = 0x7fffffff;
+          const FoldPhilox key = p.expo ? FoldPhilox{0u, 0u, 0u} : fold_philox(p.keys, b, p.seg_first, p.seed);
           for (int i = lane; i < NC; i += 32) {
             const float l = __ldcg(p.xlog + (size_t)i * Bp + b);
             const float pr = expf(l - mx) / sum;
             float e;
             if (p.expo) e = __ldg(p.expo + ((size_t)t * B + b) * NC + i);
             else {
-              const Philox4 r = philox4x32_10((unsigned)t, (unsigned)(p.seg_first + b), 16u + (unsigned)(i >> 2),
-                                              (unsigned)p.offset, (unsigned)p.seed, (unsigned)(p.seed >> 32));
+              const Philox4 r = philox4x32_10((unsigned)t, key.fold, 16u + (unsigned)(i >> 2), (unsigned)p.offset, key.k0, key.k1);
               const unsigned rv[4] = {r.x, r.y, r.z, r.w};
               e = -logf(u01_open(rv[i & 3]));
             }
@@ -441,7 +442,7 @@ class SimtEngine : public Engine {
 
   bool supports(const wrnn_job& job) const override { return job.mel_frames == nullptr; }   // upsampled streams only
 
-  int generate(const wrnn_job& job, cudaStream_t stream) override {
+  int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) override {
     if (job.mel_frames) { set_error("the SIMT engine takes the upsampled conditioning streams (mels_up / aux)"); return WRNN_E_INVALID; }
     if (job.uniforms_ready) { set_error("the SIMT engine needs all draws resident (no uniforms_ready)"); return WRNN_E_INVALID; }
     WRNN_CUDA_OK(cudaSetDevice(device));
@@ -465,6 +466,7 @@ class SimtEngine : public Engine {
     p.uniforms = job.uniforms; p.expo = job.expo; p.seed = job.philox_seed; p.offset = job.philox_offset;
     p.out = job.out; p.x_force = job.x_force; p.logits_out = job.logits_out;
     p.fold_row0 = reinterpret_cast<const long long*>(job.fold_row0); p.fold_row_end = reinterpret_cast<const long long*>(job.fold_row_end);
+    p.keys = keys;
     float* s = static_cast<float*>(d_scratch_);
     p.xch = s; s += (size_t)4 * H * Bp;
     p.xs = s; s += Bp;

@@ -102,6 +102,7 @@ struct StreamParams {
   const float* uniforms; const unsigned* uniforms_ready; unsigned long long seed, offset;
   float* out; const float* x_force; float* logits_out;
   const long long* fold_row0; const long long* fold_row_end;
+  const FoldKey* keys;          // optional per-fold Philox keys [n_total]
   const float* mel_frames; const float* aux_frames; const float* up_taps; int hop;
   float* state;                 // [tiles][2][H][NF] fp32 hidden state
   int* abort_flag;
@@ -337,7 +338,8 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
           for (int i = 0; i < 10; ++i) ur[i] = __ldca(u + gf * 10 + i);
           ur[10] = __ldca(u + 10 * p.n_total + gf);
         } else {
-          const unsigned gg = (unsigned)(p.seg_first + gf), k0 = (unsigned)p.seed, k1 = (unsigned)(p.seed >> 32), o0 = (unsigned)p.offset;
+          const FoldPhilox k = fold_philox(p.keys, gf, p.seg_first, p.seed);
+          const unsigned gg = k.fold, k0 = k.k0, k1 = k.k1, o0 = (unsigned)p.offset;
           const Philox4 r0 = philox4x32_10((unsigned)t, gg, 0u, o0, k0, k1), r1 = philox4x32_10((unsigned)t, gg, 1u, o0, k0, k1),
                         r2 = philox4x32_10((unsigned)t, gg, 2u, o0, k0, k1);
           ur[0] = u_ref_range(r0.x); ur[1] = u_ref_range(r0.y); ur[2] = u_ref_range(r0.z); ur[3] = u_ref_range(r0.w);
@@ -409,13 +411,15 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
           // the pick is the best score, ties to the lowest class.  This thread holds rows rw, rw + 8 of folds 8j + fc (+1):
           // two words of two different Philox blocks per fold, each block computed for the one word it gives.
           uint2* cw = reinterpret_cast<uint2*>(smem + SM::OFF_LOG) + (blk & 1) * 8 * NF;      // [warp][fold] best of the warp's 16 rows
-          const unsigned k0 = (unsigned)p.seed, k1 = (unsigned)(p.seed >> 32), o0 = (unsigned)p.offset;
+          const unsigned o0 = (unsigned)p.offset;
 #pragma unroll
           for (int j = 0; j < NF / 8; ++j) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               const int f = 8 * j + fc + e;
               const size_t row_out = ((size_t)t * p.n_total + f0 + f) * NCLS_RAW;
+              FoldPhilox key{0u, 0u, 0u};
+              if (f < B && !p.expo) key = fold_philox(p.keys, f0 + f, p.seg_first, p.seed);
               float best = 0.f;
               int bk = 0;
 #pragma unroll
@@ -427,7 +431,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
                   if (p.expo) {
                     ex = __ldg(p.expo + row_out + k);
                   } else {
-                    const Philox4 r = philox4x32_10((unsigned)t, (unsigned)(p.seg_first + f0 + f), 16u + (unsigned)(k >> 2), o0, k0, k1);
+                    const Philox4 r = philox4x32_10((unsigned)t, key.fold, 16u + (unsigned)(k >> 2), o0, key.k0, key.k1);
                     const unsigned w = (k & 3) == 0 ? r.x : (k & 3) == 1 ? r.y : (k & 3) == 2 ? r.z : r.w;
                     ex = -logf(u01_open(w));
                   }
@@ -754,7 +758,7 @@ class StreamEngine : public Engine {
     if (const char* e = getenv("WRNN_STREAM_CL")) { const int v = atoi(e); if (v == 1 || v == 4) cl = v; }
   }
 
-  int generate(const wrnn_job& job, cudaStream_t stream) override {
+  int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) override {
     WRNN_CUDA_OK(cudaSetDevice(device));
     int nf = 16, cl = 1;
     choose(job.n_seg, nf, cl);
@@ -779,6 +783,7 @@ class StreamEngine : public Engine {
     p.uniforms = job.uniforms; p.uniforms_ready = job.uniforms_ready; p.seed = job.philox_seed; p.offset = job.philox_offset;
     p.out = job.out; p.x_force = job.x_force; p.logits_out = job.logits_out; p.expo = raw() ? job.expo : nullptr;
     p.fold_row0 = reinterpret_cast<const long long*>(job.fold_row0); p.fold_row_end = reinterpret_cast<const long long*>(job.fold_row_end);
+    p.keys = keys;
     p.mel_frames = job.mel_frames; p.aux_frames = job.aux_frames; p.up_taps = job.up_taps; p.hop = job.hop;
     p.state = static_cast<float*>(d_state_);
     p.abort_flag = reinterpret_cast<int*>(static_cast<unsigned*>(d_sync_) + 8);

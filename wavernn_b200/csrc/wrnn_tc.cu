@@ -100,6 +100,7 @@ struct TcParams {
   const unsigned* uniforms_ready;   // optional: rows of `uniforms` uploaded so far (draws streamed in while the kernel runs)
   float* out; const float* x_force; float* logits_out;
   const long long* fold_row0; const long long* fold_row_end;   // optional per-fold conditioning windows (job-wide, [n_total])
+  const FoldKey* keys;       // optional per-fold Philox keys (job-wide, [n_total])
   const float* mel_frames; const float* aux_frames; const float* up_taps; int hop;   // optional frame-rate conditioning
   unsigned char* xch;        // [4 vectors][2 parities][n_groups * SBO_H] activation images
   unsigned char* xch5;       // RAW: [2 parities][128 CTAs][n_groups * 8 folds] (score, class) candidates
@@ -297,8 +298,8 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
 #pragma unroll
               for (int i = 0; i < UT; ++i) ex[i] = __ldg(p.expo + ((size_t)t * p.n_total + p.f0 + fold) * NCLS + u0 + j0 + i);
             } else {                                        // same keying as the SIMT engine: block 16 + class/4
-              const Philox4 r = philox4x32_10((unsigned)t, (unsigned)(p.seg_first + p.f0 + fold), 16u + (unsigned)cta,
-                                              (unsigned)p.offset, (unsigned)p.seed, (unsigned)(p.seed >> 32));
+              const FoldPhilox k = fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
+              const Philox4 r = philox4x32_10((unsigned)t, k.fold, 16u + (unsigned)cta, (unsigned)p.offset, k.k0, k.k1);
 #pragma unroll
               for (int i = 0; i < UT; ++i) {
                 const int j = j0 + i;
@@ -328,7 +329,8 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
           }
         } else if (owns_fold) {
           {
-            const unsigned g = (unsigned)(p.seg_first + p.f0 + fold), k0 = (unsigned)p.seed, k1 = (unsigned)(p.seed >> 32), o0 = (unsigned)p.offset;
+            const FoldPhilox k = fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
+            const unsigned g = k.fold, k0 = k.k0, k1 = k.k1, o0 = (unsigned)p.offset;
             const Philox4 r0 = philox4x32_10((unsigned)t, g, 0u, o0, k0, k1), r1 = philox4x32_10((unsigned)t, g, 1u, o0, k0, k1),
                           r2 = philox4x32_10((unsigned)t, g, 2u, o0, k0, k1);
             ur[0] = u_ref_range(r0.x); ur[1] = u_ref_range(r0.y); ur[2] = u_ref_range(r0.z); ur[3] = u_ref_range(r0.w);
@@ -790,7 +792,7 @@ class TcEngine : public Engine {
   }
   bool supports(const wrnn_job&) const override { return true; }   // any fold count: tiles of 64 folds, one launch each
 
-  int generate(const wrnn_job& job, cudaStream_t stream) override {
+  int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) override {
     WRNN_CUDA_OK(cudaSetDevice(device));
     TcParams p{};
     p.blob = static_cast<const unsigned char*>(d_blob_);
@@ -801,6 +803,7 @@ class TcEngine : public Engine {
     p.uniforms_ready = job.uniforms_ready;
     p.out = job.out; p.x_force = job.x_force; p.logits_out = job.logits_out;
     p.fold_row0 = reinterpret_cast<const long long*>(job.fold_row0); p.fold_row_end = reinterpret_cast<const long long*>(job.fold_row_end);
+    p.keys = keys;
     p.mel_frames = job.mel_frames; p.aux_frames = job.aux_frames; p.up_taps = job.up_taps; p.hop = job.hop;
     p.xch = static_cast<unsigned char*>(d_scratch_);
     p.xch5 = p.xch + xch5_off_;
