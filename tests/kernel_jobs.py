@@ -8,11 +8,16 @@ Every job is teacher-forced with explicit draws and has the edges where the kern
   - fold tables (frame-rate jobs): starts that are not multiples of the stride, windows that end mid-frame and before
     `steps`, one window shorter than 8 rows.
 Rows come from frame-rate tensors through the 5-tap table, in float64 (`contract.expand_rows`); the materialised jobs
-read those rows rounded to float32."""
+read those rows rounded to float32.
+
+Every job is made at the reference's hop of 275 (upsample factors (5, 5, 11)) unless given another geometry of
+GEOMETRIES, whose taps come from a WaveRNN built with those factors (`geometry_taps`).  The stride stays 271, coprime
+with every hop here, so fold windows still start at many phases."""
 from __future__ import annotations
 
 import numpy as np
 
+import helpers
 from oracle import contract as C
 from oracle import philox as P
 from test_gpu_sampling import forced_inputs
@@ -29,47 +34,78 @@ SMALL_TILE = 24
 # another CPU's float32 summation order; fp16 stays under the suite's 1e-3.
 LOGIT_TOL = {("fp16", "MOL"): 6e-4, ("fp16", "RAW"): 6e-4, ("bf16", "MOL"): 4e-3, ("bf16", "RAW"): 4e-3}
 
+# upsampling geometries other than (5, 5, 11) whose impulse response fits the 5-tap table: hop -> upsample factors.
+# Hop 1 wraps the phase on every row; at hop <= 8 every 8-row staging group crosses a frame boundary; at 600 a window
+# of STEPS rows lies within one or two frames.  200, 256 and 300 are the hops of common 16 / 24 kHz checkpoints.
+GEOMETRIES = {1: (1,), 3: (3,), 8: (8,), 9: (3, 3), 200: (5, 5, 8), 256: (4, 8, 8), 300: (5, 6, 10), 600: (600,)}
+KERNEL_HOPS = (1, 3, 200, 256, 600)      # the hops besides 275 at which the GPU runs every job (tests/test_gpu_geometries.py)
 
-def geometry(n):
+
+def geometry_model(hop, mode="MOL", seed=0, **kw):
+    """helpers.make_model's network with the upsample factors of GEOMETRIES[hop] (hop 275: helpers.CTOR's)."""
+    import contextlib
+    import io
+
+    import torch
+    from wavernn_b200 import WaveRNN
+    factors = helpers.CTOR["upsample_factors"] if hop == HOP else GEOMETRIES[hop]
+    torch.manual_seed(seed)
+    with contextlib.redirect_stdout(io.StringIO()):
+        m = WaveRNN(mode=mode, **dict(helpers.CTOR, upsample_factors=factors, hop_length=hop, **kw))
+    m.gen_verbose = False
+    return m
+
+
+def geometry_taps(hop):
+    """(hop, 5) float32 interpolation table of the geometry (WaveRNN.upsample_taps on the CPU)."""
+    import torch
+    m = geometry_model(hop, rnn_dims=32, fc_dims=32)
+    taps = m.upsample_taps(torch.device("cpu")).numpy()
+    assert m._taps_exact and taps.shape == (hop, 5)
+    return taps
+
+
+def geometry(n, hop=HOP):
     """(L, T): the stream ends half way into the last fold's window; T frames cover it."""
     L = (SEG_FIRST + n - 1) * STRIDE + STEPS // 2
-    return L, L // HOP + 1
+    return L, L // hop + 1
 
 
-def frames(n, seed):
+def frames(n, seed, hop=HOP):
     """Padded mel frames (T + 4, 80) and aux frames (T + 4, 128), float32."""
-    _, T = geometry(n)
+    _, T = geometry(n, hop)
     rs = np.random.RandomState(seed)
     return rs.rand(T + 4, 80).astype(np.float32), rs.randn(T + 4, 128).astype(np.float32)
 
 
-def fold_tables(n, seed):
+def fold_tables(n, seed, hop=HOP):
     """fold_row0 / fold_row_end (int64, absolute rows of the stream) for n folds."""
-    L, _ = geometry(n)
+    L, _ = geometry(n, hop)
     rs = np.random.RandomState(seed)
     row0 = rs.randint(0, L - 2 * STEPS, n).astype(np.int64)
     row0[row0 % STRIDE == 0] += 1
     length = rs.randint(STEPS // 2, 2 * STEPS, n)          # about a third end before `steps`
     length[1] = 5                                          # shorter than one 8-row group
     end = np.minimum(row0 + length, L)
-    end[end % HOP == 0] -= 1                               # every window ends mid-frame
+    if hop > 1:                                            # (at hop 1 every row starts a frame)
+        end[end % hop == 0] -= 1                           # every window ends mid-frame
     return row0, end.astype(np.int64)
 
 
-def make_job(n, mode, taps, tables=False):
-    """Everything a kernel and the emulation need for one job of n folds.  Strided: `m_up` / `aux` are the job's rows
-    from its first fold on (row SEG_FIRST * STRIDE of the stream), as the materialised path indexes them.  Tables:
-    the whole stream, indexed by the absolute fold_row0."""
-    L, T = geometry(n)
+def make_job(n, mode, taps, tables=False, hop=HOP):
+    """Everything a kernel and the emulation need for one job of n folds at `hop` (taps: that geometry's (hop, 5)
+    table).  Strided: `m_up` / `aux` are the job's rows from its first fold on (row SEG_FIRST * STRIDE of the stream), as
+    the materialised path indexes them.  Tables: the whole stream, indexed by the absolute fold_row0."""
+    L, T = geometry(n, hop)
     seed = 1000 * n + (2 if tables else 0) + (mode == "RAW")
-    mel_fr, aux_fr = frames(n, seed)
+    mel_fr, aux_fr = frames(n, seed, hop)
     row_lo = 0 if tables else SEG_FIRST * STRIDE
-    m, a = C.expand_rows(mel_fr, aux_fr, taps, HOP, row_lo, L - row_lo)
-    job = dict(n=n, mode=mode, tables=tables, L=L, T=T, mel_frames=mel_fr, aux_frames=aux_fr, taps=np.asarray(taps, np.float32),
+    m, a = C.expand_rows(mel_fr, aux_fr, taps, hop, row_lo, L - row_lo)
+    job = dict(n=n, mode=mode, tables=tables, hop=hop, L=L, T=T, mel_frames=mel_fr, aux_frames=aux_fr, taps=np.asarray(taps, np.float32),
                row_lo=row_lo, m_up=m.astype(np.float32), aux=a.astype(np.float32), x_force=forced_inputs(n, STEPS, seed + 7),
                fold_row0=None, fold_row_end=None, uniforms=None, expo=None)
     if tables:
-        job["fold_row0"], job["fold_row_end"] = fold_tables(n, seed + 3)
+        job["fold_row0"], job["fold_row_end"] = fold_tables(n, seed + 3, hop)
     if mode == "MOL":
         job["uniforms"] = P.mol_uniforms(SEED, OFFSET, SEG_FIRST, n, STEPS)
     else:

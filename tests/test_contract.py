@@ -1,5 +1,7 @@
 """The engine-arithmetic emulation (folded order, fp16/bf16 operand rounding) against the
 reference-order oracle.  States the FP tolerance of the product path on the CPU."""
+import hashlib
+
 import numpy as np
 import pytest
 import torch
@@ -105,3 +107,107 @@ def test_accumulation_spread_predicts_the_kernel_matrix_tolerances(mode, precisi
     assert spread <= tol / 4
     if precision == "fp16":
         assert tol <= 1e-3
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the kernel matrix's jobs at upsampling geometries other than (5, 5, 11)
+# ---------------------------------------------------------------------------------------------------------------------
+# sha256 (first 16 hex digits) of every hop-275 job as kernel_jobs made it before it took a hop, on fixed taps
+HOP_275_JOBS = {
+    (24, False, "MOL"): "40284be60d698699", (24, True, "MOL"): "7b6044de4f34e70f", (25, False, "MOL"): "505c9cd82b995bd1",
+    (25, True, "MOL"): "813469b9decfc47d", (73, False, "MOL"): "673e009efd4e8a23", (73, True, "MOL"): "eaa21d3279c97b0e",
+    (17, False, "MOL"): "85e557183166e59d", (17, True, "MOL"): "ad48a914fe80806f", (33, False, "MOL"): "a419ac708f3dfe86",
+    (33, True, "MOL"): "c660abc597a4baf5", (24, False, "RAW"): "0428ae144e970448", (24, True, "RAW"): "584be791aeffad2d",
+    (25, False, "RAW"): "b4b71983da14b850", (25, True, "RAW"): "40c3e97ef1aa4ad3", (73, False, "RAW"): "fe0a79ad2934b78e",
+    (73, True, "RAW"): "3658f95c8a9ebb88", (17, False, "RAW"): "531433ebe116c2f5", (17, True, "RAW"): "60e7f0412296b061",
+    (33, False, "RAW"): "6cc976dfd0bc9ab1", (33, True, "RAW"): "c72f6f6e4ef28d67",
+}
+
+
+def _job_digest(job):
+    h = hashlib.sha256()
+    for k in sorted(job):
+        v = job[k]
+        if isinstance(v, np.ndarray):
+            h.update(k.encode()); h.update(str(v.dtype).encode()); h.update(str(v.shape).encode())
+            h.update(np.ascontiguousarray(v).tobytes())
+        elif k != "hop":
+            h.update(f"{k}={v!r}".encode())
+    return h.hexdigest()[:16]
+
+
+def test_hop_275_jobs_are_unchanged():
+    """Every job of the hop-275 kernel matrix, bit for bit, by default and with hop=275 spelled out (fixed taps, so that
+    the digests do not depend on torch's CPU convolutions)."""
+    taps = np.random.RandomState(275).rand(275, 5).astype(np.float32)
+    for mode in ("MOL", "RAW"):
+        for n, tables in K.all_jobs():
+            job = K.make_job(n, mode, taps, tables)
+            assert job["hop"] == K.HOP and _job_digest(job) == HOP_275_JOBS[(n, tables, mode)], (n, tables, mode)
+            assert _job_digest(K.make_job(n, mode, taps, tables, hop=K.HOP)) == HOP_275_JOBS[(n, tables, mode)]
+
+
+@pytest.mark.parametrize("hop", sorted(K.GEOMETRIES))
+def test_jobs_at_other_hops_have_the_edges(hop):
+    """The jobs at another hop keep the edges of the 275 ones: fold windows that start at many phases, windows of the
+    tables that end mid-frame, frames that cover the stream's last row (mel frames up to T + 3)."""
+    for n, tables in K.all_jobs():
+        job = K.make_job(n, "MOL", K.geometry_taps(hop), tables, hop=hop)
+        L, T = job["L"], job["T"]
+        assert job["hop"] == hop and job["mel_frames"].shape == (T + 4, 80) and (L - 1) // hop + 4 <= T + 3
+        row0 = job["fold_row0"] if tables else (K.SEG_FIRST + np.arange(n)) * K.STRIDE
+        assert len(set((row0 % hop).tolist())) >= min(hop, n) // (2 if tables else 1), "fold windows start at few phases"
+        if tables and hop > 1:
+            assert (job["fold_row_end"] % hop != 0).all()
+        rows = job["m_up"].shape[0]
+        assert rows == L - job["row_lo"] and job["aux"].shape == (rows, 128)
+
+
+def _spread(w, job, precision):
+    _, l32 = K.emulate(w, job, precision)
+    _, l64 = K.emulate(w, job, precision, accumulate="f64")
+    assert np.isfinite(l32).all() and np.abs(l64).max() > 0.1
+    return float(np.abs(l32 - l64).max())
+
+
+@pytest.mark.parametrize("precision", ["fp16", "bf16"])
+@pytest.mark.parametrize("mode", ["MOL", "RAW"])
+@pytest.mark.parametrize("hop", K.KERNEL_HOPS)
+def test_accumulation_spread_predicts_the_tolerances_at_other_hops(hop, mode, precision):
+    """test_accumulation_spread_predicts_the_kernel_matrix_tolerances on the jobs of tests/test_gpu_geometries.py: the
+    same model and LOGIT_TOL, rows formed at another hop with that geometry's taps."""
+    w = O.hot_weights(helpers.state_numpy(helpers.make_model(0, mode)))
+    taps = K.geometry_taps(hop)
+    spread = max(_spread(w, K.make_job(n, mode, taps, tables, hop=hop), precision) for n, tables in K.all_jobs())
+    tol = K.LOGIT_TOL[(precision, mode)]
+    print(f"hop {hop} {precision} {mode}: predicted accumulation spread of the teacher-forced logits {spread:.3e}; "
+          f"GPU tolerance {tol:.1e}")
+    assert spread <= tol / 4
+
+
+@pytest.mark.parametrize("mode", ["MOL", "RAW"])
+@pytest.mark.parametrize("hop", K.KERNEL_HOPS)
+def test_rows_formed_at_the_wrong_hop_move_the_logits_past_the_tolerance(hop, mode):
+    """Negative control of the GPU comparison at another hop: the emulation on the rows a kernel would form with the
+    hop-275 table, or at the right hop one phase late, moves the teacher-forced logits by more than 10 x LOGIT_TOL
+    (the larger, bf16 one), so a kernel that used a stale hop or phase would fail the comparison."""
+    w = O.hot_weights(helpers.state_numpy(helpers.make_model(0, mode)))
+    taps, taps_275 = K.geometry_taps(hop), K.geometry_taps(K.HOP)
+    bound = 10 * max(K.LOGIT_TOL[(p, mode)] for p in ("fp16", "bf16"))
+    shifts = {"hop 275": 0.0, "phase + 1": 0.0}
+    for n, tables in ((24, False), (25, True)):
+        job = K.make_job(n, mode, taps, tables, hop=hop)
+        _, want = K.emulate(w, job, "fp16")
+        lo, n_rows = job["row_lo"], job["L"] - job["row_lo"]
+        T_275 = job["L"] // K.HOP + 1
+        mel = np.zeros((max(T_275, job["T"]) + 4, 80), np.float32)
+        aux = np.zeros((max(T_275, job["T"]) + 4, 128), np.float32)
+        mel[:job["T"] + 4], aux[:job["T"] + 4] = job["mel_frames"], job["aux_frames"]
+        wrong = {"hop 275": C.expand_rows(mel, aux, taps_275, K.HOP, lo, n_rows),
+                 "phase + 1": C.expand_rows(job["mel_frames"], job["aux_frames"], taps, hop, lo + 1, n_rows)}
+        for what, (m, a) in wrong.items():
+            _, lg = K.emulate(w, dict(job, m_up=m.astype(np.float32), aux=a.astype(np.float32)), "fp16")
+            shifts[what] = max(shifts[what], float(np.abs(lg.astype(np.float64) - want).max()))
+    print(f"hop {hop} {mode}: logit shift on rows formed at hop 275 {shifts['hop 275']:.3e}, one phase late "
+          f"{shifts['phase + 1']:.3e}; 10 x tolerance {bound:.1e}")
+    assert shifts["hop 275"] > bound and shifts["phase + 1"] > bound

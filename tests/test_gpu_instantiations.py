@@ -97,7 +97,7 @@ def launch(eng, job, source, *, a=0, b=None, cond_mode=cabi.COND_AUTO, form=None
     kw = dict(mels_up=0, aux=0, mel_frames=0, aux_frames=0, up_taps=0, hop=0)
     if source == "frames":
         mel_fr, aux_fr, taps = t(job["mel_frames"]), t(job["aux_frames"]), t(job["taps"])
-        kw.update(mel_frames=p(mel_fr), aux_frames=p(aux_fr), up_taps=p(taps), hop=K.HOP)
+        kw.update(mel_frames=p(mel_fr), aux_frames=p(aux_fr), up_taps=p(taps), hop=job["hop"])
         L = job["L"]
     else:
         n_rows = job["L"] - job["row_lo"]
@@ -107,7 +107,7 @@ def launch(eng, job, source, *, a=0, b=None, cond_mode=cabi.COND_AUTO, form=None
             mel_fr, aux_fr, taps = t(job["mel_frames"]), t(job["aux_frames"]), t(job["taps"])
             m_up = torch.empty((n_rows, 80), device=dev)
             aux = torch.empty((n_rows, 128), device=dev)
-            cabi.expand_conditioning(mel_frames=p(mel_fr), aux_frames=p(aux_fr), up_taps=p(taps), hop=K.HOP, row_lo=job["row_lo"],
+            cabi.expand_conditioning(mel_frames=p(mel_fr), aux_frames=p(aux_fr), up_taps=p(taps), hop=job["hop"], row_lo=job["row_lo"],
                                      n_rows=n_rows, mels_up=p(m_up), aux=p(aux), stream=torch.cuda.current_stream(dev).cuda_stream)
         if not tables:                                    # the sub-job's rows start at its first fold
             m_up, aux, n_rows = m_up[a * K.STRIDE:], aux[a * K.STRIDE:], n_rows - a * K.STRIDE
@@ -177,6 +177,11 @@ def logit_error(lg, emu_lg, precision, head, what):
 @pytest.mark.parametrize("precision,head,frames,big", PERSISTENT,
                          ids=[f"tc-{p}-{h}-{'frames' if fr else 'rows'}-{'big' if big else 'small'}" for p, h, fr, big in PERSISTENT])
 def test_persistent_kernel(mx, precision, head, frames, big):
+    check_persistent_kernel(mx, precision, head, frames, big)
+
+
+def check_persistent_kernel(mx, precision, head, frames, big, tag=""):
+    """The checks of one persistent kernel on mx's jobs; prints one line (prefixed by `tag`)."""
     eng = mx.engine("persistent", precision, head)
     errs = []
 
@@ -214,7 +219,7 @@ def test_persistent_kernel(mx, precision, head, frames, big):
                 parts = [run(job, source, a=a, b=b, cond_mode=cond) for a, b in ((0, 24), (24, 25))]
                 assert np.array_equal(out, np.concatenate([parts[0][0], parts[1][0]], 0)), "BIG != small (samples)"
                 assert np.array_equal(lg, np.concatenate([parts[0][1], parts[1][1]], 1)), "BIG != small (logits)"
-    print(f"persistent {'BIG' if big else 'small'} {'FRAMES' if frames else 'rows'} {precision} {head}: "
+    print(f"{tag}persistent {'BIG' if big else 'small'} {'FRAMES' if frames else 'rows'} {precision} {head}: "
           f"max logit error vs emulation {max(errs):.2e} (tolerance {K.LOGIT_TOL[(precision, head)]:.1e})")
 
 
@@ -224,6 +229,11 @@ def test_persistent_kernel(mx, precision, head, frames, big):
 @pytest.mark.parametrize("precision,head,frames,nf,cl", STREAM,
                          ids=[f"stream-{p}-{h}-{'frames' if fr else 'rows'}-{nf}x{cl}" for p, h, fr, nf, cl in STREAM])
 def test_stream_kernel(mx, precision, head, frames, nf, cl):
+    check_stream_kernel(mx, precision, head, frames, nf, cl)
+
+
+def check_stream_kernel(mx, precision, head, frames, nf, cl, tag=""):
+    """The checks of one stream kernel form on mx's jobs; prints one line (prefixed by `tag`)."""
     eng = mx.engine("stream", precision, head)
     n = K.STREAM_FOLDS[nf]
     errs = []
@@ -250,7 +260,7 @@ def test_stream_kernel(mx, precision, head, frames, nf, cl):
             assert np.array_equal(out, out_1) and np.array_equal(lg, lg_1), "cluster form != one-CTA form"
         errs.append(logit_error(lg, emu_lg, precision, head, tables))
         check_samples(job, out, lg)
-    print(f"stream {nf}x{cl} {'FRAMES' if frames else 'rows'} {precision} {head}: "
+    print(f"{tag}stream {nf}x{cl} {'FRAMES' if frames else 'rows'} {precision} {head}: "
           f"max logit error vs emulation {max(errs):.2e} (tolerance {K.LOGIT_TOL[(precision, head)]:.1e})")
 
 
@@ -261,15 +271,19 @@ def test_conditioning_pre_pass_against_the_float64_rows():
     """cabi.expand_conditioning against contract.expand_rows: mel within the error bound of the kernel's 5-fmaf chain
     (2^-21 of the sum of |tap x mel|), aux bit for bit.  Short runs at a non-zero phase, a run long enough for the
     grid-stride loop to go round more than once, and the last row of the stream (mel frames up to T + 3)."""
-    dev = torch.device("cuda", 0)
     model = helpers.make_model(0, "MOL")
-    taps = model.upsample_taps(torch.device("cpu")).numpy()
-    hop, T = 275, 80
+    check_pre_pass(model.upsample_taps(torch.device("cpu")).numpy(), 275, 80)
+
+
+def check_pre_pass(taps, hop, T):
+    """The pre-pass on T frames at `hop` with that geometry's taps: runs of 1, 7, 8 and 9 rows from row 3 hop + 101 %
+    hop, all rows but the first 57, and the last row."""
+    dev = torch.device("cuda", 0)
     rs = np.random.RandomState(9)
     mel_fr, aux_fr = rs.rand(T + 4, 80).astype(np.float32), rs.randn(T, 128).astype(np.float32)
     d_mel, d_aux, d_taps = (torch.as_tensor(x, device=dev) for x in (mel_fr, aux_fr, taps))
     n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
-    cases = [(3 * hop + 101, k) for k in (1, 7, 8, 9)] + [(57, T * hop - 57), (T * hop - 1, 1)]
+    cases = [(3 * hop + 101 % hop, k) for k in (1, 7, 8, 9)] + [(57, T * hop - 57), (T * hop - 1, 1)]
     assert T * hop - 57 > 2 * 8 * 8 * n_sm                # more than two passes of the capped grid (8 rows per block)
     for row_lo, n_rows in cases:
         m = torch.full((n_rows, 80), float("nan"), device=dev)
@@ -283,7 +297,7 @@ def test_conditioning_pre_pass_against_the_float64_rows():
         r = np.arange(row_lo, row_lo + n_rows)
         bound = 2.0 ** -21 * sum(np.abs(taps[r % hop, dd].astype(np.float64)[:, None] * mel_fr[r // hop + dd]) for dd in range(5))
         e = np.abs(m - want_m)
-        print(f"pre-pass rows [{row_lo}, {row_lo + n_rows}): max mel error {e.max():.2e}, max error / bound {(e / np.maximum(bound, 1e-300)).max():.3f}")
+        print(f"pre-pass hop {hop} rows [{row_lo}, {row_lo + n_rows}): max mel error {e.max():.2e}, max error / bound {(e / np.maximum(bound, 1e-300)).max():.3f}")
         assert (e <= bound).all() and np.array_equal(a, want_a.astype(np.float32)), (row_lo, n_rows)
 
 

@@ -43,7 +43,7 @@ def _frames(eng, mel):
     d = torch.as_tensor(mel, dtype=torch.float32, device=DEV).contiguous()
     mf = torch.full((T + 4, 80), float("nan"), device=DEV)
     af = torch.full((T, 128), float("nan"), device=DEV)
-    tp = torch.full((275, 5), float("nan"), device=DEV)
+    tp = torch.full((eng.hop_length, 5), float("nan"), device=DEV)
     eng.conditioning_frames(mel=d.data_ptr(), T=T, mel_frames=mf.data_ptr(), aux_frames=af.data_ptr(), up_taps=tp.data_ptr(),
                             stream=_stream())
     torch.cuda.synchronize(DEV)
@@ -54,7 +54,7 @@ def _frames(eng, mel):
 def _vocode(eng, mel, **kw):
     T = mel.shape[1]
     d = torch.as_tensor(mel, dtype=torch.float32, device=DEV).contiguous()
-    wav = torch.full(((T - 1) * 275,), float("nan"), dtype=torch.float64, device=DEV)
+    wav = torch.full(((T - 1) * eng.hop_length,), float("nan"), dtype=torch.float64, device=DEV)
     eng.vocode(mel=d.data_ptr(), T=T, wav=wav.data_ptr(), stream=_stream(), **kw)
     torch.cuda.synchronize(DEV)
     eng.check()

@@ -105,6 +105,27 @@ def test_plan_matches_restatement(lib, Ts, batched, target, overlap):
         assert (f[:, 0] >= utt[i, 0] * HOP).all() and (f[:, 1] == (utt[i, 0] + T) * HOP).all()
 
 
+@pytest.mark.parametrize("hop", [1, 3, 256, 600])
+def test_plan_matches_restatement_at_other_hops(lib, hop):
+    """The batch layout at hops other than 275: frame0 * hop rows per utterance, 4 * hop gap rows between them, folds
+    scaled to the hop (a padded last fold per utterance), and one fold per utterance unbatched."""
+    Ts = (26, 21, 40, 33)
+    seeds = [(0x9E3779B97F4A7C15 * (i + 3)) % 2 ** 64 for i in range(len(Ts))]
+    for batched, target, overlap in ((True, 8 * hop, max(2, 4 * hop // 5)), (True, 3 * hop, hop), (False, 0, 0)):
+        rc, msg, p = _plan(lib, Ts, seeds, batched, target, overlap, hop)
+        assert rc == 0, msg
+        geo, utt, folds = _restated(Ts, seeds, batched, target, overlap, hop)
+        assert tuple(p["geo"]) == geo and np.array_equal(p["utt"], utt) and np.array_equal(p["folds"], folds), (batched, target)
+        ends = list(utt[1:, 1]) + [geo[0]]
+        for i, T in enumerate(Ts):
+            f = p["folds"][utt[i, 1]:ends[i]]
+            assert (f[:, 0] >= utt[i, 0] * hop).all() and (f[:, 1] == (utt[i, 0] + T) * hop).all()
+            assert i + 1 == len(Ts) or utt[i + 1, 0] * hop - f[0, 1] == 4 * hop          # the gap rows
+        if batched:
+            assert geo[0] >= 3 * len(Ts)
+            assert any(fold_geometry(T * hop, target, overlap).padded_len != T * hop for T in Ts)
+
+
 @pytest.mark.parametrize("batched", [True, False])
 def test_one_utterance_is_the_single_job(lib, batched):
     """A one-utterance batch is wrnn_vocode's job: its fold_geometry, fold b at row b * seg_stride, key (seed, b)."""
