@@ -54,12 +54,27 @@ template <> __device__ __forceinline__ void wgmma_ss<8, 1>(float* d, uint64_t da
                    "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])    \
                  : "l"(da), "l"(db), "r"(s) : "memory");                                                                     \
   }
+#define WRNN_WGMMA_N64(FMT, TY)                                                                                              \
+  template <> __device__ __forceinline__ void wgmma_ss<64, FMT>(float* d, uint64_t da, uint64_t db, uint32_t s) {          \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"                                                      \
+                 "wgmma.mma_async.sync.aligned.m64n64k16" TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, "  \
+                 "%14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, "       \
+                 "p, 1, 1, 0, 0;\n\t}\n"                                                                                      \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),          \
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),    \
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),  \
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])   \
+                 : "l"(da), "l"(db), "r"(s) : "memory");                                                                     \
+  }
 WRNN_WGMMA_N16(0, ".f32.f16.f16")
 WRNN_WGMMA_N16(1, ".f32.bf16.bf16")
 WRNN_WGMMA_N32(0, ".f32.f16.f16")
 WRNN_WGMMA_N32(1, ".f32.bf16.bf16")
+WRNN_WGMMA_N64(0, ".f32.f16.f16")
+WRNN_WGMMA_N64(1, ".f32.bf16.bf16")
 #undef WRNN_WGMMA_N16
 #undef WRNN_WGMMA_N32
+#undef WRNN_WGMMA_N64
 
 // TMA 1-D bulk copy global -> shared, completion counted in bytes on an mbarrier (whole warp, one lane elected)
 __device__ __forceinline__ void tma_bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t mbar) {
