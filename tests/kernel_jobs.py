@@ -1,5 +1,6 @@
-"""The job matrix that runs every compiled tensor-core kernel (tests/test_gpu_instantiations.py), the emulation of
-each job (oracle/contract.py) and the logit tolerances, which the CPU predicts (tests/test_contract.py).
+"""The job matrix that runs every compiled tensor-core kernel (tests/test_gpu_instantiations.py) and every SIMT engine
+path (tests/test_gpu_simt.py), the emulation of each job (oracle/contract.py) and the logit tolerances, which the CPU
+predicts (tests/test_contract.py).
 
 Every job is teacher-forced with explicit draws and has the edges where the kernels' per-instantiation code differs:
   - seg_stride 271 against a hop of 275: fold windows start at many phases of the hop and cross frame boundaries;
@@ -30,9 +31,20 @@ SMALL_TILE = 24
 
 # Teacher-forced logits of a kernel against contract.generate_segments at the kernel's operand precision.  Each bound is
 # at least 4 x the largest float32-vs-float64 accumulation spread of the emulation on these jobs (asserted on the CPU in
-# tests/test_contract.py, which prints the spreads: fp16 8.9e-5 MoL / 1.1e-4 RAW, bf16 6.9e-4 / 7.5e-4), with room for
-# another CPU's float32 summation order; fp16 stays under the suite's 1e-3.
-LOGIT_TOL = {("fp16", "MOL"): 6e-4, ("fp16", "RAW"): 6e-4, ("bf16", "MOL"): 4e-3, ("bf16", "RAW"): 4e-3}
+# tests/test_contract.py, which prints the spreads: fp16 8.9e-5 MoL / 1.1e-4 RAW, bf16 6.9e-4 / 7.5e-4, fp32 (the SIMT
+# engine's strict mode) 1.6e-7 / 1.8e-7), with room for another CPU's float32 summation order; fp16 stays under the
+# suite's 1e-3.
+LOGIT_TOL = {("fp16", "MOL"): 6e-4, ("fp16", "RAW"): 6e-4, ("bf16", "MOL"): 4e-3, ("bf16", "RAW"): 4e-3,
+             ("fp32", "MOL"): 1.2e-6, ("fp32", "RAW"): 1.2e-6}
+# fp32 logits against wavernn_oracle.generate_segments (the reference's own operation order, unfolded): at least 4 x
+# the largest difference between the fp32 emulation (float32 or float64 sums) and that order on these jobs
+# (tests/test_contract.py: 1.8e-7 MoL / 2.1e-7 RAW).
+ORACLE_TOL = {"MOL": 1.5e-6, "RAW": 1.5e-6}
+# A 16-bit kernel's mean logit error against the emulation at its own precision must be at most 1 / ROUNDING_SEPARATION
+# of its mean error against the other 16-bit precision's emulation.  The max-error bounds above cannot tell bf16 from
+# fp16 rounding on these jobs; the means can (tests/test_contract.py: the float64-summed emulation, standing in for a
+# kernel with another sum order, is 14 x (bf16) and 22 x (fp16) closer to its own precision).
+ROUNDING_SEPARATION = 4
 
 # upsampling geometries other than (5, 5, 11) whose impulse response fits the 5-tap table: hop -> upsample factors.
 # Hop 1 wraps the phase on every row; at hop <= 8 every 8-row staging group crosses a frame boundary; at 600 a window
@@ -119,6 +131,28 @@ def emulate(w, job, precision, accumulate="f32"):
                                mode=job["mode"], uniforms=job["uniforms"], expo=job["expo"], x_force=job["x_force"],
                                fold_row0=job["fold_row0"], fold_row_end=job["fold_row_end"], want_logits=True,
                                precision=precision, accumulate=accumulate)
+
+
+def oracle_rows(job):
+    """The job's rows re-laid out as STEPS-row windows, one per fold, zero past each window's end: the rows fold f reads
+    at step t are rows f * STEPS + t, so that wavernn_oracle.generate_segments (which has no fold tables) runs every job
+    at seg_stride = STEPS."""
+    n, t = job["n"], np.arange(STEPS)
+    if job["tables"]:
+        row, end = job["fold_row0"][:, None] + t, job["fold_row_end"][:, None]
+    else:
+        row, end = np.arange(n)[:, None] * STRIDE + t, job["m_up"].shape[0]
+    ok = (row < end).reshape(-1, 1)
+    r = np.where(ok[:, 0], row.reshape(-1), 0)
+    return np.where(ok, job["m_up"][r], 0).astype(np.float32), np.where(ok, job["aux"][r], 0).astype(np.float32)
+
+
+def emulate_oracle(w, job):
+    """wavernn_oracle.generate_segments on the job (its rows by oracle_rows): (samples, logits) as emulate returns them."""
+    from oracle import wavernn_oracle as O
+    m, a = oracle_rows(job)
+    return O.generate_segments(w, m, a, n_seg=job["n"], seg_len=STEPS, seg_stride=STEPS, steps=STEPS, mode=job["mode"],
+                               uniforms=job["uniforms"], expo=job["expo"], x_force=job["x_force"], want_logits=True)
 
 
 def all_jobs():

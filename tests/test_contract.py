@@ -86,12 +86,12 @@ def test_expand_rows_restates_the_upsample_network():
     assert np.array_equal(m2, m[3 * hop + 101:3 * hop + 801]) and np.array_equal(a2, a[3 * hop + 101:3 * hop + 801])
 
 
-@pytest.mark.parametrize("precision", ["fp16", "bf16"])
+@pytest.mark.parametrize("precision", ["fp16", "bf16", "fp32"])
 @pytest.mark.parametrize("mode", ["MOL", "RAW"])
 def test_accumulation_spread_predicts_the_kernel_matrix_tolerances(mode, precision):
-    """Teacher-forced logits of every job of tests/test_gpu_instantiations.py, summed in float32 and in float64 at the
-    same operand precision: their largest difference estimates the accumulation-order noise a kernel may show, and the
-    GPU tolerance must be at least 4 x that (fp16: at most the suite's 1e-3)."""
+    """Teacher-forced logits of every job of tests/test_gpu_instantiations.py and tests/test_gpu_simt.py, summed in
+    float32 and in float64 at the same operand precision: their largest difference estimates the accumulation-order
+    noise a kernel may show, and the GPU tolerance must be at least 4 x that (fp16: at most the suite's 1e-3)."""
     model = helpers.make_model(0, mode)
     w = O.hot_weights(helpers.state_numpy(model))
     taps = model.upsample_taps(torch.device("cpu")).numpy()
@@ -107,6 +107,75 @@ def test_accumulation_spread_predicts_the_kernel_matrix_tolerances(mode, precisi
     assert spread <= tol / 4
     if precision == "fp16":
         assert tol <= 1e-3
+
+
+@pytest.mark.parametrize("mode", ["MOL", "RAW"])
+def test_reference_order_spread_predicts_the_strict_engine_bound(mode):
+    """The fp32 emulation (folded order, float32 and float64 sums) against wavernn_oracle.generate_segments (the
+    reference's unfolded order) on every job of the kernel matrix: the SIMT engine's fp32 bound against that order,
+    kernel_jobs.ORACLE_TOL, must be at least 4 x their largest difference.  The oracle has no fold tables, so it reads
+    each job's windows re-laid out by kernel_jobs.oracle_rows; the emulation on those rows equals the emulation on the
+    job bit for bit (the re-layout reads exactly the job's rows)."""
+    model = helpers.make_model(0, mode)
+    w = O.hot_weights(helpers.state_numpy(model))
+    taps = model.upsample_taps(torch.device("cpu")).numpy()
+    spread = 0.0
+    for n, tables in K.all_jobs():
+        job = K.make_job(n, mode, taps, tables)
+        _, l32 = K.emulate(w, job, "fp32")
+        _, l64 = K.emulate(w, job, "fp32", accumulate="f64")
+        _, lo = K.emulate_oracle(w, job)
+        m, a = K.oracle_rows(job)
+        _, lr = C.generate_segments(w, m, a, n_seg=n, seg_len=K.STEPS, seg_stride=K.STEPS, steps=K.STEPS, mode=mode,
+                                    uniforms=job["uniforms"], expo=job["expo"], x_force=job["x_force"], want_logits=True,
+                                    precision="fp32")
+        assert np.array_equal(lr, l32), (n, tables)
+        spread = max(spread, float(np.abs(l32 - lo.astype(np.float64)).max()), float(np.abs(l64 - lo.astype(np.float64)).max()))
+    tol = K.ORACLE_TOL[mode]
+    print(f"fp32 {mode}: emulation vs the reference order {spread:.3e}; GPU bound {tol:.1e}")
+    assert spread <= tol / 4
+
+
+@pytest.mark.parametrize("mode", ["MOL", "RAW"])
+def test_operand_rounding_of_another_precision_fails_the_kernel_matrix_checks(mode):
+    """Negative control of the SIMT matrix (tests/test_gpu_simt.py): a handle that rounded its operands to another
+    type than its own must fail the comparison with its own emulation.
+
+    fp32: the fp16 and bf16 emulations differ from the fp32 one by more than 10 x the fp32 tolerance, so the strict
+    engine's max-error check catches either rounding.
+
+    fp16 / bf16: the bf16 emulation differs from the fp16 one by only ~2.5 x the fp16 tolerance (1.5e-3 MoL, 1.7e-3 RAW
+    on these small random-init logits), and by less than the bf16 tolerance.  Most of the bf16 accumulation spread is
+    an activation whose bf16 rounding flips when the sum order changes, so a bf16 max-error bound cannot be tighter than
+    the bf16-vs-fp16 shift.  The 16-bit handles are therefore also checked on the MEAN logit error: against the
+    emulation at their own precision it must be at most a quarter of that against the other 16-bit precision.  The
+    float64-summed emulation stands in for a kernel with another sum order here; it must pass that check by 10 x."""
+    model = helpers.make_model(0, mode)
+    w = O.hot_weights(helpers.state_numpy(model))
+    taps = model.upsample_taps(torch.device("cpu")).numpy()
+    shift = {("fp16", "fp32"): 0.0, ("bf16", "fp32"): 0.0, ("bf16", "fp16"): 0.0}
+    mean = {(p, q): [] for p in ("fp16", "bf16") for q in ("fp16", "bf16")}        # (stand-in precision, emulation)
+    for n, tables in K.all_jobs():
+        job = K.make_job(n, mode, taps, tables)
+        l = {p: K.emulate(w, job, p)[1].astype(np.float64) for p in ("fp32", "fp16", "bf16")}
+        for a, b in shift:
+            shift[(a, b)] = max(shift[(a, b)], float(np.abs(l[a] - l[b]).max()))
+        for p in ("fp16", "bf16"):
+            _, l64 = K.emulate(w, job, p, accumulate="f64")
+            for q in ("fp16", "bf16"):
+                mean[(p, q)].append(np.abs(l64 - l[q]).ravel())
+    mean = {k: float(np.concatenate(v).mean()) for k, v in mean.items()}
+    print(f"{mode}: max logit shift fp16 vs fp32 {shift[('fp16', 'fp32')]:.3e}, bf16 vs fp32 {shift[('bf16', 'fp32')]:.3e} "
+          f"(10 x fp32 tolerance {10 * K.LOGIT_TOL[('fp32', mode)]:.1e}); bf16 vs fp16 {shift[('bf16', 'fp16')]:.3e} "
+          f"(fp16 tolerance {K.LOGIT_TOL[('fp16', mode)]:.1e}); mean error of the float64-summed stand-in against its own / "
+          f"the other 16-bit emulation: fp16 {mean[('fp16', 'fp16')]:.2e} / {mean[('fp16', 'bf16')]:.2e}, "
+          f"bf16 {mean[('bf16', 'bf16')]:.2e} / {mean[('bf16', 'fp16')]:.2e}")
+    assert shift[("fp16", "fp32")] > 10 * K.LOGIT_TOL[("fp32", mode)]
+    assert shift[("bf16", "fp32")] > 10 * K.LOGIT_TOL[("fp32", mode)]
+    assert shift[("bf16", "fp16")] > 2 * K.LOGIT_TOL[("fp16", mode)]
+    for p, q in (("fp16", "bf16"), ("bf16", "fp16")):
+        assert mean[(p, p)] <= mean[(p, q)] / 10, (p, mean)
+    assert K.ROUNDING_SEPARATION <= 4
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -38,6 +38,7 @@ FORMS = {
     "stream-32x4": ("stream", "fp16", 40, "32", "4"),
     "simt-fp16": ("simt", "fp16", 40, None, None),
     "simt-fp32": ("simt", "fp32", 40, None, None),
+    "simt-bf16": ("simt", "bf16", 40, None, None),
 }
 MOL_FORMS = list(FORMS)
 RAW_FORMS = [f for f in FORMS if not f.startswith("stream")]     # the stream engine has no RAW head

@@ -106,6 +106,23 @@ def test_mu_law_table(lib):
     assert np.all(np.abs(mu - ref) <= np.spacing(pw_c) / (n - 1))
 
 
+def test_every_raw_label_is_recovered_from_the_sample_the_kernels_write():
+    """Host mirror of wrnn_epilogue's label recovery for the mu-law table, in float32 as the kernel evaluates it:
+    __float2int_rn((x + 1) * (0.5 * (n - 1))) returns k for the sample x = 2k / (n - 1) - 1 that the RAW samplers of
+    wrnn_tc.cu / wrnn_simt.cu / wrnn_stream.cu write for class k (`2.0f * (float)k / ((float)n - 1.0f) - 1.0f`), for
+    every k < 512.  np.rint rounds half to even, as __float2int_rn does."""
+    n = 512
+    f = np.float32
+    k = np.arange(n)
+    x = f(2) * k.astype(f) / (f(n) - f(1)) - f(1)
+    assert x.dtype == f and x[0] == -1 and x[-1] == 1 and x[(n - 1) // 2 + 1] > 0 > x[(n - 1) // 2]
+    y = (x + f(1)) * (f(0.5) * f(n - 1))
+    assert y.dtype == f
+    lbl = np.rint(y).astype(np.int64)
+    assert np.array_equal(lbl, k), k[lbl != k]
+    print(f"RAW labels: largest distance of (x + 1) (n - 1) / 2 from its label {np.abs(y.astype(np.float64) - k).max():.2e}")
+
+
 # ---------------------------------------------------------------------------------------------------- the upsampler
 def _hook(lib, state_dict, **kw):
     cfg = cabi.upsample_cfg(**kw)
