@@ -309,6 +309,45 @@ int wrnn_vocode_many(wrnn_t *h, const wrnn_vocode_batch *b, void *stream);
 /* The same with HOST mel / wav: copies in, runs, copies out, synchronises and returns wrnn_check's verdict. */
 int wrnn_vocode_many_host(wrnn_t *h, const wrnn_vocode_batch *b);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * Scoring: how likely a given waveform is under the model, on the engine that generates it.  The loss the reference
+ * trains with (train_wavernn.py:83), per sample, teacher-forced and reduced inside the kernel where the logits are:
+ *   MoL: discretized_mix_logistic_loss(reduce=False) (utils/distribution.py:16-84; num_classes 65536, log_scale_min
+ *        log(1e-14)), all of its branches, in fp32 in the reference's order;
+ *   RAW: F.cross_entropy, logsumexp(logits) - logits[label] with label = rint((y + 1)(n_classes - 1) / 2) clamped to
+ *        [0, n_classes - 1] -- pass label_2_float(label) as the target (utils/dataset.py:88).
+ * In nats, with accurate expf / logf / log1pf.  No draws are made.  The stream engine scores the MoL head only.
+ * --------------------------------------------------------------------------------------------------------------- */
+
+/* nll[t][b] (device, [seg_len, n_seg], the layout of x_force) = the loss of target x_force[t][b] given x_force[0..t-1][b]
+ * and the conditioning rows up to t.  job->x_force (device) is required and holds the targets; step t consumes
+ * x_force[t-1] exactly as wrnn_generate does.  Rows >= steps of nll are untouched.  job->out may be NULL and is never
+ * written; logits_out works as in wrnn_generate (the same chains, so the same bits); the draw fields are ignored.
+ * The engine is the one wrnn_generate would pick.  Asynchronous on `stream` (device errors: wrnn_check after a sync). */
+int wrnn_score(wrnn_t *h, const wrnn_job *job, float *nll, void *stream);
+
+/* One recording to score from its mel spectrogram.  Scored UNBATCHED, as one fold: step t conditions on row t of the
+ * T*hop-row stream wrnn_vocode would build from `mel` and on x[t-1] (0 at t = 0) -- the model's likelihood of the
+ * whole recording (folding with overlap would change it).                                                          */
+typedef struct {
+  const float *mel;        /* [feat, T], the layout of wrnn_vocode_job::mel           */
+  int64_t T;               /* mel frames                                               */
+  const float *x;          /* [n] the waveform, samples in [-1, 1] (RAW: label_2_float) */
+  int64_t n;               /* samples to score, 1 <= n <= T * hop                       */
+  float *nll;              /* [n] per-sample loss in nats                               */
+} wrnn_score_utt;
+
+/* All utterances as ONE job: one launch of the conditioning network, one engine job over n_utts folds of max_i n_i steps
+ * (rows past an utterance read as zeros; nothing is written past n_i), engine chosen as for wrnn_vocode_many (a SIMT
+ * handle expands the rows into scratch first).  Each utterance's losses are bit-identical to its own single-utterance
+ * call whenever both are served by the same engine (always on a handle created with a fixed engine).
+ * Refused (WRNN_E_INVALID, the handle stays usable): n_utts < 1 or > 65535; a null utts, mel, x or nll; n_i < 1 or
+ * n_i > T_i * hop (the message names i); a laid-out stream of 2^31 samples or more (sum_i (T_i + 4) * hop); a handle
+ * with no upsampler attached; a RAW head on the stream engine.  DEVICE mel / x / nll pointers; asynchronous.        */
+int wrnn_score_many(wrnn_t *h, const wrnn_score_utt *utts, int32_t n_utts, void *stream);
+/* The same with HOST mel / x / nll: copies in, runs, copies out, synchronises and returns wrnn_check's verdict. */
+int wrnn_score_many_host(wrnn_t *h, const wrnn_score_utt *utts, int32_t n_utts);
+
 /* Host helper for parity mode: replays torch's default CPU generator (MT19937) natively, so the
  * draws the reference makes before / inside its loop cost a few ms instead of ~30.
  *   state : the generator's 624 words and its position `pos` in [0, 624] (624 = block exhausted)

@@ -23,7 +23,7 @@ EXPORTS = ("wrnn_abi_version", "wrnn_last_error", "wrnn_create", "wrnn_destroy",
            "wrnn_check", "wrnn_generate_host", "wrnn_engine_name", "wrnn_grid_ctas", "wrnn_launch_count",
            "wrnn_mt19937_uniform", "wrnn_mt19937_uniform_cols", "wrnn_epilogue", "wrnn_expand_conditioning",
            "wrnn_attach_upsampler", "wrnn_conditioning_frames", "wrnn_vocode", "wrnn_vocode_host",
-           "wrnn_vocode_many", "wrnn_vocode_many_host")
+           "wrnn_vocode_many", "wrnn_vocode_many_host", "wrnn_score", "wrnn_score_many", "wrnn_score_many_host")
 
 _fp = C.POINTER(C.c_float)
 
@@ -80,6 +80,18 @@ class WrnnUtterance(C.Structure):
 class WrnnVocodeBatch(C.Structure):
     _fields_ = [("utts", C.POINTER(WrnnUtterance)), ("n_utts", C.c_int32), ("batched", C.c_int32), ("target", C.c_int32),
                 ("overlap", C.c_int32), ("mu_law", C.c_int32)]
+
+
+class WrnnScoreUtt(C.Structure):
+    _fields_ = [("mel", C.c_void_p), ("T", C.c_int64), ("x", C.c_void_p), ("n", C.c_int64), ("nll", C.c_void_p)]
+
+
+def score_utts(utts):
+    """A wrnn_score_utt array over `utts`, a list of (mel address, T, x address, n, nll address) (0 = NULL).  Returns
+    the array and its length (an empty list gives a NULL array)."""
+    arr = (WrnnScoreUtt * max(len(utts), 1))(*[WrnnScoreUtt(m or None, int(T), x or None, int(n), o or None)
+                                               for m, T, x, n, o in utts])
+    return (arr if utts else None), len(utts)
 
 
 def vocode_batch(utts, *, batched=True, target=11000, overlap=550, mu_law=False):
@@ -149,7 +161,15 @@ def load() -> C.CDLL:
     lib.wrnn_vocode_many.argtypes = [C.c_void_p, C.POINTER(WrnnVocodeBatch), C.c_void_p]
     lib.wrnn_vocode_many_host.restype = C.c_int
     lib.wrnn_vocode_many_host.argtypes = [C.c_void_p, C.POINTER(WrnnVocodeBatch)]
+    lib.wrnn_score.restype = C.c_int
+    lib.wrnn_score.argtypes = [C.c_void_p, C.POINTER(WrnnJob), C.c_void_p, C.c_void_p]
+    lib.wrnn_score_many.restype = C.c_int
+    lib.wrnn_score_many.argtypes = [C.c_void_p, C.POINTER(WrnnScoreUtt), C.c_int32, C.c_void_p]
+    lib.wrnn_score_many_host.restype = C.c_int
+    lib.wrnn_score_many_host.argtypes = [C.c_void_p, C.POINTER(WrnnScoreUtt), C.c_int32]
     # test hooks (not declared in the header)
+    lib.wrnn_debug_score_many_plan.restype = C.c_int
+    lib.wrnn_debug_score_many_plan.argtypes = [C.c_int32, C.POINTER(WrnnScoreUtt), C.c_int32, C.c_void_p, C.c_void_p]
     lib.wrnn_debug_vocode_many_plan.restype = C.c_int
     lib.wrnn_debug_vocode_many_plan.argtypes = [C.c_int32, C.POINTER(WrnnVocodeBatch), C.c_void_p, C.c_void_p, C.c_void_p]
     lib.wrnn_debug_fold_geometry.restype = C.c_int
@@ -310,6 +330,38 @@ class Engine:
         _check(self.lib, self.lib.wrnn_vocode_many_host(self._h, C.byref(b)))
         del keep
         return wavs
+
+    # ---- scoring (wrnn_score / wrnn_score_many): the reference's training loss per sample, teacher-forced ----
+    def score(self, *, L: int, n_seg: int, seg_len: int, seg_stride: int, x_force: int, nll: int, mels_up: int = 0, aux: int = 0,
+              seg_first: int = 0, steps: int = 0, logits_out: int = 0, fold_row0: int = 0, fold_row_end: int = 0,
+              mel_frames: int = 0, aux_frames: int = 0, up_taps: int = 0, hop: int = 0, cond_mode: int = 0, stream: int = 0):
+        """wrnn_score with raw device addresses: nll [seg_len, n_seg] fp32 = the loss of target x_force[t] (same layout)
+        given x_force[:t] and the conditioning rows up to t.  The job is wrnn_generate's without `out` or draws.
+        Asynchronous."""
+        job = WrnnJob(mels_up or None, aux or None, L, seg_stride, n_seg, seg_len, seg_first, steps, None, None, 0, 0, None,
+                      x_force or None, logits_out or None, fold_row0 or None, fold_row_end or None, mel_frames or None,
+                      aux_frames or None, up_taps or None, hop, cond_mode, None)
+        _check(self.lib, self.lib.wrnn_score(self._h, C.byref(job), nll or None, C.c_void_p(stream or None)))
+
+    def score_many(self, *, mels, Ts, xs, ns, nlls, stream: int = 0):
+        """wrnn_score_many with raw device addresses: utterance i is mels[i] [80, Ts[i]] and its waveform xs[i] [ns[i]]
+        -> nlls[i] [ns[i]] fp32, each scored unbatched (one fold).  One job for the whole batch.  Asynchronous."""
+        arr, n = score_utts(list(zip(mels, Ts, xs, ns, nlls)))
+        _check(self.lib, self.lib.wrnn_score_many(self._h, arr, n, C.c_void_p(stream or None)))
+
+    def score_many_host(self, mels, xs):
+        """wrnn_score_many_host: a list of numpy mels (80, T_i) and the waveforms xs[i] (n_i samples, n_i <= T_i * hop)
+        -> the list of per-sample losses (nats, float32), without torch."""
+        import numpy as np
+        mels = [np.ascontiguousarray(m[0] if m.ndim == 3 and m.shape[0] == 1 else m, dtype=np.float32) for m in mels]
+        xs = [np.ascontiguousarray(x, dtype=np.float32).reshape(-1) for x in xs]
+        if len(xs) != len(mels):
+            raise ValueError("one waveform per mel")
+        nlls = [np.empty(x.size, dtype=np.float32) for x in xs]
+        arr, n = score_utts([(m.ctypes.data, m.shape[-1], x.ctypes.data, x.size, o.ctypes.data)
+                             for m, x, o in zip(mels, xs, nlls)])
+        _check(self.lib, self.lib.wrnn_score_many_host(self._h, arr, n))
+        return nlls
 
     def check(self):
         _check(self.lib, self.lib.wrnn_check(self._h))

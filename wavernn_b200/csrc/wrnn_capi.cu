@@ -143,9 +143,9 @@ void wrnn_destroy(wrnn_t* h) {
   delete h;
 }
 
-static int validate(const wrnn_t* h, const wrnn_job* job, bool host) {
+static int validate(const wrnn_t* h, const wrnn_job* job, bool host, bool score = false) {
   if (!h || !h->engine || !job) { set_error("null handle or job"); return WRNN_E_INVALID; }
-  if (!job->out) { set_error("out is required"); return WRNN_E_INVALID; }
+  if (!job->out && !score) { set_error("out is required"); return WRNN_E_INVALID; }
   if (job->mel_frames) {
     if (!job->aux_frames || !job->up_taps || job->hop <= 0) { set_error("mel_frames needs aux_frames, up_taps and hop"); return WRNN_E_INVALID; }
     if (host) { set_error("frame-rate conditioning is a device-pointer feature (use wrnn_generate)"); return WRNN_E_INVALID; }
@@ -170,6 +170,19 @@ int wrnn_generate(wrnn_t* h, const wrnn_job* job, void* stream) {
   if ((rc = pick_engine(h, job, &e)) != WRNN_OK) return rc;
   h->last = e;
   return e->generate(*job, static_cast<cudaStream_t>(stream), nullptr);
+}
+
+static const char* kNoRawStreamScore = "the stream engine scores the MoL head only (RAW scoring runs on the persistent or SIMT engine)";
+
+int wrnn_score(wrnn_t* h, const wrnn_job* job, float* nll, void* stream) {
+  int rc = validate(h, job, false, true);
+  if (rc != WRNN_OK) return rc;
+  if (!job->x_force || !nll) { set_error("wrnn_score needs x_force (the targets) and nll"); return WRNN_E_INVALID; }
+  Engine* e = nullptr;
+  if ((rc = pick_engine(h, job, &e)) != WRNN_OK) return rc;
+  if (!e->scores()) { set_error(kNoRawStreamScore); return WRNN_E_INVALID; }
+  h->last = e;
+  return e->score(*job, nll, static_cast<cudaStream_t>(stream), nullptr);
 }
 
 int wrnn_check(wrnn_t* h) {
@@ -433,6 +446,107 @@ static int vocode_many(wrnn_t* h, const wrnn_vocode_batch* b, const cond::BatchP
                          tabs.tail, 20ll * hop, d_eu, EpUtt{0, 0, 0, nullptr}, n, pl.max_wave, st);
 }
 
+// wrnn_score_many: each utterance one fold (layout: cond::score_plan).  Its samples are gathered into the x_force block
+// of the job ([steps][n_utts], zeros past n_i) and its losses scattered back from the nll block, one launch each.
+struct ScoreUtt {
+  const float* x;
+  float* nll;
+  long long n;
+};
+__global__ void score_gather_kernel(const ScoreUtt* __restrict__ u, int n_utts, long long steps, float* __restrict__ xf) {
+  const long long total = steps * n_utts;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long t = i / n_utts;
+    const int b = (int)(i - t * n_utts);
+    xf[i] = t < u[b].n ? __ldg(u[b].x + t) : 0.f;
+  }
+}
+__global__ void score_scatter_kernel(const ScoreUtt* __restrict__ u, int n_utts, long long steps, const float* __restrict__ nl) {
+  const long long total = steps * n_utts;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long t = i / n_utts;
+    const int b = (int)(i - t * n_utts);
+    if (t < u[b].n) u[b].nll[t] = __ldcg(nl + i);
+  }
+}
+
+static int score_many(wrnn_t* h, const wrnn_score_utt* utts, int n, const cond::BatchPlan& pl, cudaStream_t st) {
+  Upsampler& u = *h->upsampler;
+  const int hop = u.hop;
+  const size_t steps = (size_t)pl.g.seg_len;
+  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
+
+  wrnn_job j;
+  std::memset(&j, 0, sizeof(j));
+  j.L = pl.L; j.seg_stride = pl.g.seg_stride; j.n_seg = n; j.seg_len = (int32_t)steps;
+  j.hop = hop; j.cond_mode = WRNN_COND_AUTO;
+  const void* tag = h->upsampler;                      // placeholders: only tested against NULL
+  j.fold_row0 = j.fold_row_end = static_cast<const int64_t*>(tag);
+  Engine* e = nullptr;
+  bool expanded = false;
+  int rc = pick_vocode_engine(h, j, &e, &expanded);
+  if (rc != WRNN_OK) return rc;
+  if (!e->scores()) { set_error(kNoRawStreamScore); return WRNN_E_INVALID; }
+
+  // scratch: [row0 | row_end | CondUtt table | ScoreUtt table | mel_frames | aux_frames | x_force | nll | expanded rows]
+  const size_t n_frames = (size_t)pl.frame0.back();
+  const size_t b_row = align_floats(2 * (size_t)n) * 4;
+  const size_t b_cu = align_floats(n * sizeof(CondUtt) / 4 + 1) * 4, b_su = align_floats(n * sizeof(ScoreUtt) / 4 + 1) * 4;
+  const size_t b_tab = 2 * b_row + b_cu + b_su;
+  const size_t n_mf = align_floats(n_frames * FEAT), n_af = align_floats(n_frames * cond::CD), n_xf = align_floats(steps * n);
+  const size_t n_rows = expanded ? align_floats((size_t)pl.L * FEAT) + align_floats((size_t)pl.L * 4 * AUXD) : 0;
+  rc = grow(&u.d_scratch, &u.scratch_bytes, b_tab + (n_mf + n_af + 2 * n_xf + n_rows) * sizeof(float));
+  if (rc != WRNN_OK) return rc;
+  unsigned char* d = static_cast<unsigned char*>(u.d_scratch);
+  float* mel_frames = reinterpret_cast<float*>(d + b_tab);
+  float* aux_frames = mel_frames + n_mf;
+  float* xf = aux_frames + n_af;
+  float* nl = xf + n_xf;
+
+  u.host_plan.assign(b_tab, 0);
+  unsigned char* hp = u.host_plan.data();
+  std::memcpy(hp, pl.row0.data(), n * 8);
+  std::memcpy(hp + b_row, pl.row_end.data(), n * 8);
+  CondUtt* cu = reinterpret_cast<CondUtt*>(hp + 2 * b_row);
+  ScoreUtt* su = reinterpret_cast<ScoreUtt*>(hp + 2 * b_row + b_cu);
+  for (int i = 0; i < n; ++i) {
+    cu[i] = CondUtt{utts[i].mel, utts[i].T, pl.frame0[i]};
+    su[i] = ScoreUtt{utts[i].x, utts[i].nll, utts[i].n};
+  }
+  WRNN_CUDA_OK(cudaMemcpyAsync(d, hp, b_tab, cudaMemcpyHostToDevice, st));
+  j.fold_row0 = reinterpret_cast<const int64_t*>(d);
+  j.fold_row_end = reinterpret_cast<const int64_t*>(d + b_row);
+  const CondUtt* d_cu = reinterpret_cast<const CondUtt*>(d + 2 * b_row);
+  const ScoreUtt* d_su = reinterpret_cast<const ScoreUtt*>(d + 2 * b_row + b_cu);
+
+  if ((rc = conditioning_frames_batch(u, d_cu, n, pl.max_T, mel_frames, aux_frames, st)) != WRNN_OK) return rc;
+  if (expanded) {
+    // rows [0, L - 4*hop): the last utterance's 4*hop gap rows would read frames past the end and no fold reads them
+    float* mels_up = nl + n_xf;
+    float* aux = mels_up + align_floats((size_t)pl.L * FEAT);
+    if ((rc = expand_conditioning(mel_frames, aux_frames, u.d_taps, hop, 0, pl.L - 4ll * hop, mels_up, aux, st)) != WRNN_OK) return rc;
+    j.mels_up = mels_up; j.aux = aux;
+  } else {
+    j.mel_frames = mel_frames; j.aux_frames = aux_frames; j.up_taps = u.d_taps;
+  }
+  const int grid = grid_stride_blocks(((long long)steps * n + 255) / 256);
+  score_gather_kernel<<<grid, 256, 0, st>>>(d_su, n, (long long)steps, xf);
+  WRNN_CUDA_OK(cudaGetLastError());
+  j.x_force = xf;
+  h->last = e;
+  if ((rc = e->score(j, nl, st, nullptr)) != WRNN_OK) return rc;
+  score_scatter_kernel<<<grid, 256, 0, st>>>(d_su, n, (long long)steps, nl);
+  WRNN_CUDA_OK(cudaGetLastError());
+  return WRNN_OK;
+}
+
+static int validate_score_many(const wrnn_t* h, const wrnn_score_utt* utts, int n, cond::BatchPlan& pl) {
+  if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
+  if (!h->upsampler) { set_error("no upsampler attached (wrnn_attach_upsampler)"); return WRNN_E_INVALID; }
+  if (!h->engine->scores()) { set_error(kNoRawStreamScore); return WRNN_E_INVALID; }
+  return cond::score_plan(h->upsampler->hop, utts, n, pl);
+}
+
 static int validate_many(const wrnn_t* h, const wrnn_vocode_batch* b, cond::BatchPlan& pl) {
   if (!h || !h->engine || !b) { set_error("null handle or batch"); return WRNN_E_INVALID; }
   if (!h->upsampler) { set_error("no upsampler attached (wrnn_attach_upsampler)"); return WRNN_E_INVALID; }
@@ -497,6 +611,42 @@ int wrnn_vocode_many_host(wrnn_t* h, const wrnn_vocode_batch* b) {
   for (int i = 0; i < n; ++i)
     WRNN_CUDA_OK(cudaMemcpyAsync(b->utts[i].wav, d_wav + pl.wav0[i], (size_t)(pl.wav0[i + 1] - pl.wav0[i]) * sizeof(double),
                                  cudaMemcpyDeviceToHost, 0));
+  WRNN_CUDA_OK(cudaStreamSynchronize(0));
+  return h->last->check();
+}
+
+int wrnn_score_many(wrnn_t* h, const wrnn_score_utt* utts, int32_t n_utts, void* stream) {
+  cond::BatchPlan pl;
+  const int rc = validate_score_many(h, utts, n_utts, pl);
+  if (rc != WRNN_OK) return rc;
+  return score_many(h, utts, n_utts, pl, static_cast<cudaStream_t>(stream));
+}
+
+int wrnn_score_many_host(wrnn_t* h, const wrnn_score_utt* utts, int32_t n_utts) {
+  cond::BatchPlan pl;
+  int rc = validate_score_many(h, utts, n_utts, pl);
+  if (rc != WRNN_OK) return rc;
+  Upsampler& u = *h->upsampler;
+  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
+  const int n = n_utts;
+  std::vector<size_t> mel_off(n + 1, 0), x_off(n + 1, 0);
+  for (int i = 0; i < n; ++i) {
+    mel_off[i + 1] = mel_off[i] + align_floats((size_t)utts[i].T * FEAT);
+    x_off[i + 1] = x_off[i] + align_floats((size_t)utts[i].n);
+  }
+  if ((rc = grow(&u.d_stage, &u.stage_bytes, (mel_off[n] + 2 * x_off[n]) * sizeof(float))) != WRNN_OK) return rc;
+  float* d_mel = static_cast<float*>(u.d_stage);
+  float* d_x = d_mel + mel_off[n];
+  float* d_nll = d_x + x_off[n];
+  std::vector<wrnn_score_utt> du(utts, utts + n);
+  for (int i = 0; i < n; ++i) {
+    WRNN_CUDA_OK(cudaMemcpyAsync(d_mel + mel_off[i], utts[i].mel, (size_t)utts[i].T * FEAT * sizeof(float), cudaMemcpyHostToDevice, 0));
+    WRNN_CUDA_OK(cudaMemcpyAsync(d_x + x_off[i], utts[i].x, (size_t)utts[i].n * sizeof(float), cudaMemcpyHostToDevice, 0));
+    du[i].mel = d_mel + mel_off[i]; du[i].x = d_x + x_off[i]; du[i].nll = d_nll + x_off[i];
+  }
+  if ((rc = score_many(h, du.data(), n, pl, 0)) != WRNN_OK) return rc;
+  for (int i = 0; i < n; ++i)
+    WRNN_CUDA_OK(cudaMemcpyAsync(utts[i].nll, d_nll + x_off[i], (size_t)utts[i].n * sizeof(float), cudaMemcpyDeviceToHost, 0));
   WRNN_CUDA_OK(cudaStreamSynchronize(0));
   return h->last->check();
 }

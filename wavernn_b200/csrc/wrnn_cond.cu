@@ -386,6 +386,29 @@ int batch_plan(int hop, const wrnn_vocode_batch& b, BatchPlan& out) {
   return WRNN_OK;
 }
 
+int score_plan(int hop, const wrnn_score_utt* utts, int n_utts, BatchPlan& out) {
+  if (n_utts < 1 || n_utts > 65535 || !utts) { set_error("a batch needs 1 to 65535 utterances and a non-null utts array"); return WRNN_E_INVALID; }
+  out = BatchPlan();
+  int64_t frames = 0, losses = 0, max_n = 0;
+  for (int i = 0; i < n_utts; ++i) {
+    const wrnn_score_utt& u = utts[i];
+    const std::string at = "utterance " + std::to_string(i) + ": ";
+    if (!u.mel || !u.x || !u.nll) { set_error(at + "mel, x and nll are required"); return WRNN_E_INVALID; }
+    if (u.T < 1 || u.T >= (1ll << 31) / hop) { set_error(at + "T must be >= 1 and the stream shorter than 2^31 samples"); return WRNN_E_INVALID; }
+    if (u.n < 1 || u.n > u.T * hop) { set_error(at + "n must be in [1, T * hop]: one target per conditioning row"); return WRNN_E_INVALID; }
+    out.frame0.push_back(frames); out.wav0.push_back(losses); out.fold0.push_back(i);
+    out.row0.push_back(frames * hop); out.row_end.push_back((frames + u.T) * hop);
+    frames += u.T + 4; losses += u.n;
+    if (frames * hop >= (1ll << 31)) { set_error("the laid-out stream of the batch is 2^31 samples or longer"); return WRNN_E_INVALID; }
+    if (u.T > out.max_T) out.max_T = u.T;
+    if (u.n > max_n) max_n = u.n;
+  }
+  out.frame0.push_back(frames); out.wav0.push_back(losses); out.fold0.push_back(n_utts);
+  out.L = frames * hop;
+  out.g = Geometry{n_utts, max_n, max_n, 0, 0};
+  return WRNN_OK;
+}
+
 void epilogue_tables(int overlap, bool mu_law, int n_classes, int hop, std::vector<double>& fade_in,
                      std::vector<double>& fade_out, std::vector<double>& mu, std::vector<double>& tail) {
   fade_in.clear(); fade_out.clear(); mu.clear();
@@ -534,6 +557,23 @@ int wrnn_debug_vocode_many_plan(int32_t hop, const wrnn_vocode_batch* b, int64_t
     for (int64_t f = 0; f < pl.g.n_seg; ++f) {
       folds[4 * f] = pl.row0[f]; folds[4 * f + 1] = pl.row_end[f];
       folds[4 * f + 2] = (int64_t)pl.keys[f].seed; folds[4 * f + 3] = pl.keys[f].fold;
+    }
+  return WRNN_OK;
+}
+
+// The layout wrnn_score_many runs for these utterances at this hop (cond::score_plan), or its refusal.  geo[5] = n_seg,
+// steps (max n_i), L (rows of the laid-out stream), max_T, total losses; folds [n_utts][4] = fold_row0, fold_row_end,
+// frame0, offset of the utterance's losses.  folds may be NULL.  mel / x / nll are only tested against NULL.
+int wrnn_debug_score_many_plan(int32_t hop, const wrnn_score_utt* utts, int32_t n_utts, int64_t* geo, int64_t* folds) {
+  if (!geo || hop <= 0) { set_error("null argument"); return WRNN_E_INVALID; }
+  cond::BatchPlan pl;
+  const int rc = cond::score_plan(hop, utts, n_utts, pl);
+  if (rc != WRNN_OK) return rc;
+  const int64_t g[5] = {pl.g.n_seg, pl.g.seg_len, pl.L, pl.max_T, pl.wav0.back()};
+  std::memcpy(geo, g, sizeof(g));
+  if (folds)
+    for (int i = 0; i < n_utts; ++i) {
+      folds[4 * i] = pl.row0[i]; folds[4 * i + 1] = pl.row_end[i]; folds[4 * i + 2] = pl.frame0[i]; folds[4 * i + 3] = pl.wav0[i];
     }
   return WRNN_OK;
 }

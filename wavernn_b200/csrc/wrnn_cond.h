@@ -55,6 +55,10 @@ struct BatchPlan {
 };
 // Checks the batch (WRNN_E_INVALID with a message naming the bad utterance) and lays it out.
 int batch_plan(int hop, const wrnn_vocode_batch& b, BatchPlan& out);
+// The job wrnn_score_many runs: batch_plan's unbatched layout for utterances of n_i scored samples.  Utterance i is
+// fold i, reading rows frame0[i] * hop + t (rows >= frame0[i] * hop + T_i * hop read as zeros) for max_i n_i steps
+// (g.seg_len); wav0[i] is the offset of its n_i losses in the concatenation of the nll arrays.  keys are not used.
+int score_plan(int hop, const wrnn_score_utt* utts, int n_utts, BatchPlan& out);
 
 // generate()'s float64 epilogue tables, with numpy's arithmetic (linspace = i*step + start, last element = stop):
 //   fade_in / fade_out [overlap] (xfade_and_unfold, :379-391; empty when overlap == 0), tail [20*hop] (:255),

@@ -139,4 +139,65 @@ __device__ __forceinline__ float mol_sample(LGet lget, UGet uget) {
   return fminf(fmaxf(x, -1.0f), 1.0f);                          // :121
 }
 
+// -------------------------------------------------------------------------------------
+// scoring: the reference's training loss per sample, in nats (train_wavernn.py:83).  Accurate expf / logf / log1pf
+// (never the SFU intrinsics) in fp32, in the reference's order, so that the value is a measurement of the logits.
+// -------------------------------------------------------------------------------------
+// torch.sigmoid and F.softplus (beta 1, threshold 20) as torch evaluates them in fp32
+__device__ __forceinline__ float ref_sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
+__device__ __forceinline__ float ref_softplus(float x) { return x > 20.0f ? x : log1pf(expf(x)); }
+
+// discretized_mix_logistic_loss(reduce=False) of utils/distribution.py:16-84 for target y, num_classes = 65536 and
+// log_scale_min = log(1e-14).  `lget(i)` fetches logit i of [10 mixture | 10 means | 10 log-scales].  The reference
+// blends its branches with 0/1 masks; every branch value is finite, so the blend is the selection made here.
+template <typename LGet>
+__device__ __forceinline__ float mol_nll(LGet lget, float y) {
+  const float half_bin = (float)(1.0 / 65535.0);                 // 1. / (num_classes - 1), a float32 scalar
+  const float log_half_classes = 10.397192449493701f;            // np.log((num_classes - 1) / 2)
+  float mx = lget(0);
+#pragma unroll
+  for (int k = 1; k < 10; ++k) mx = fmaxf(mx, lget(k));
+  float se = 0.f;
+#pragma unroll
+  for (int k = 0; k < 10; ++k) se += expf(lget(k) - mx);
+  const float lse_pi = logf(se);                                 // F.log_softmax(logit_probs): (x - max) - log(sum)
+  float lp[10];
+#pragma unroll
+  for (int k = 0; k < 10; ++k) {
+    const float log_scale = fmaxf(lget(20 + k), -32.23619130191664f);
+    const float centered = y - lget(10 + k);
+    const float inv_stdv = expf(-log_scale);
+    const float plus_in = inv_stdv * (centered + half_bin);
+    const float min_in = inv_stdv * (centered - half_bin);
+    const float cdf_delta = ref_sigmoid(plus_in) - ref_sigmoid(min_in);
+    float v;
+    if (y < -0.999f) v = plus_in - ref_softplus(plus_in);                       // log_cdf_plus
+    else if (y > 0.999f) v = -ref_softplus(min_in);                             // log_one_minus_cdf_min
+    else if (cdf_delta > 1e-5f) v = logf(fmaxf(cdf_delta, 1e-12f));
+    else {
+      const float mid_in = inv_stdv * centered;
+      v = __fsub_rn(__fsub_rn(mid_in, log_scale), __fmul_rn(2.0f, ref_softplus(mid_in))) - log_half_classes;   // log_pdf_mid
+    }
+    lp[k] = v + ((lget(k) - mx) - lse_pi);
+  }
+  float m = lp[0];
+#pragma unroll
+  for (int k = 1; k < 10; ++k) m = fmaxf(m, lp[k]);
+  float s = 0.f;
+#pragma unroll
+  for (int k = 0; k < 10; ++k) s += expf(lp[k] - m);
+  return -(m + logf(s));                                         // -log_sum_exp(log_probs)
+}
+
+// F.cross_entropy of one sample from the logits' maximum, the sum of exp(l - max) and the target's logit: the negated
+// log_softmax entry, -((l_y - max) - log(sum)).
+__device__ __forceinline__ float raw_nll(float mx, float sum, float l_y) { return -((l_y - mx) - logf(sum)); }
+
+// RAW head: the class of a target sample y as the reference labels it (the inverse of label_2_float,
+// utils/dataset.py:88): rint((y + 1) (n_classes - 1) / 2), clamped to [0, n_classes - 1].
+__device__ __forceinline__ int raw_label(float y, int n_classes) {
+  const float v = rintf(__fmul_rn(__fmul_rn(y + 1.0f, (float)(n_classes - 1)), 0.5f));
+  return (int)fminf(fmaxf(v, 0.0f), (float)(n_classes - 1));
+}
+
 }  // namespace wrnn

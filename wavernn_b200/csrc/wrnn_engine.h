@@ -34,8 +34,11 @@ class Engine {
   virtual ~Engine() {}
   // async; keys: optional per-fold Philox keys ([job.n_seg], device; NULL = keyed by seg_first + fold, philox_seed)
   virtual int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) = 0;
+  // The same job with the loss of target x_force[t] in the sampler's place: nll [steps][n_seg] (device), out unused.
+  virtual int score(const wrnn_job& job, float* nll, cudaStream_t stream, const FoldKey* keys) = 0;
   virtual int check() = 0;                                              // after stream sync
   virtual bool supports(const wrnn_job& job) const { (void)job; return true; }   // job inside this engine's envelope?
+  virtual bool scores() const { return true; }                          // serves wrnn_score for this handle's head?
   virtual const char* name() const = 0;
   virtual int grid_ctas() const = 0;
   int64_t launches = 0;

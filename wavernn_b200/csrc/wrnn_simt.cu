@@ -59,6 +59,7 @@ struct SimtParams {
   float* state;    // [P][NSTATE][Bp]
   float* xlog;     // RAW: [n_classes][Bp]
   unsigned* counter; int* abort_flag;
+  float* nll;      // scoring: [steps][n_seg] loss of target x_force[t] (out is not written)
 };
 
 __device__ __forceinline__ float4 load4(const float* p) { return *reinterpret_cast<const float4*>(p); }
@@ -111,7 +112,8 @@ __device__ __forceinline__ float out_row(const float* outs, int row, int f) {
   return s;
 }
 
-template <typename T>
+// SCORE: the sampler's place takes the loss of target x_force[t] (wrnn_score); no draws are made.
+template <typename T, bool SCORE>
 __global__ void __launch_bounds__(NT, 1) wrnn_simt_kernel(const SimtParams p) {
   extern __shared__ __align__(16) unsigned char smem[];
   T* wQ = reinterpret_cast<T*>(smem);
@@ -275,7 +277,10 @@ __global__ void __launch_bounds__(NT, 1) wrnn_simt_kernel(const SimtParams p) {
           if (b < B) {
             auto lget = [&](int i) { return out_row<F3ROWS>(outs, i, f) + __ldg(p.b3 + i); };
             float s;
-            if (p.uniforms) {
+            if constexpr (SCORE) {
+              s = __ldg(p.x_force + (size_t)t * B + b);
+              p.nll[(size_t)t * B + b] = mol_nll(lget, s);
+            } else if (p.uniforms) {
               const float* ur = p.uniforms + (size_t)t * 11 * B;
               s = mol_sample(lget, [&](int i) { return i < 10 ? __ldg(ur + b * 10 + i) : __ldg(ur + 10 * B + b); });
             } else {
@@ -289,7 +294,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_simt_kernel(const SimtParams p) {
               s = mol_sample(lget, [&](int i) { return u_ref_range(rv[i]); });
             }
             p.xs[b] = s;
-            p.out[(size_t)b * p.out_pitch + t] = s;
+            if (!SCORE) p.out[(size_t)b * p.out_pitch + t] = s;
             if (p.logits_out)
               for (int i = 0; i < 30; ++i) p.logits_out[((size_t)t * B + b) * 30 + i] = lget(i);
           }
@@ -325,6 +330,16 @@ __global__ void __launch_bounds__(NT, 1) wrnn_simt_kernel(const SimtParams p) {
           float sum = 0.f;
           for (int i = lane; i < NC; i += 32) sum += expf(__ldcg(p.xlog + (size_t)i * Bp + b) - mx);
           for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+          if constexpr (SCORE) {
+            const float y = __ldg(p.x_force + (size_t)t * B + b);
+            if (p.logits_out)
+              for (int i = lane; i < NC; i += 32) p.logits_out[((size_t)t * B + b) * NC + i] = __ldcg(p.xlog + (size_t)i * Bp + b);
+            if (lane == 0) {
+              p.nll[(size_t)t * B + b] = raw_nll(mx, sum, __ldcg(p.xlog + (size_t)raw_label(y, NC) * Bp + b));
+              p.xs[b] = y;
+            }
+            continue;
+          }
           float bestq = -1.f; int besti = 0x7fffffff;
           const FoldPhilox key = p.expo ? FoldPhilox{0u, 0u, 0u} : fold_philox(p.keys, b, p.seg_first, p.seed);
           for (int i = lane; i < NC; i += 32) {
@@ -408,11 +423,12 @@ class SimtEngine : public Engine {
   const char* name() const override {
     return cfg.precision == WRNN_PREC_FP32 ? "simt-fp32" : cfg.precision == WRNN_PREC_BF16 ? "simt-bf16" : "simt-fp16";
   }
-  const void* kernel() const {
-    return cfg.precision == WRNN_PREC_FP32   ? (const void*)wrnn_simt_kernel<float>
-           : cfg.precision == WRNN_PREC_BF16 ? (const void*)wrnn_simt_kernel<__nv_bfloat16>
-                                             : (const void*)wrnn_simt_kernel<__half>;
+  template <bool SCORE> const void* kernel_of() const {
+    return cfg.precision == WRNN_PREC_FP32   ? (const void*)wrnn_simt_kernel<float, SCORE>
+           : cfg.precision == WRNN_PREC_BF16 ? (const void*)wrnn_simt_kernel<__nv_bfloat16, SCORE>
+                                             : (const void*)wrnn_simt_kernel<__half, SCORE>;
   }
+  const void* kernel(bool score) const { return score ? kernel_of<true>() : kernel_of<false>(); }
   int grid_ctas() const override { return P; }
 
   int init(const HostWeights& w) {
@@ -433,7 +449,8 @@ class SimtEngine : public Engine {
     WRNN_CUDA_OK(cudaMemset(d_sync_, 0, 64));
     const size_t elem = cfg.precision == WRNN_PREC_FP32 ? 4 : 2;
     smem_bytes_ = MAT_ELEMS * elem + NVEC * 4 + (size_t)H * AP * 4 + 8 * 4 * AP * 4;
-    WRNN_CUDA_OK(cudaFuncSetAttribute(kernel(), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes_));
+    WRNN_CUDA_OK(cudaFuncSetAttribute(kernel(false), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes_));
+    WRNN_CUDA_OK(cudaFuncSetAttribute(kernel(true), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes_));
     int n_sm = 0;
     WRNN_CUDA_OK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
     if (n_sm < P) { set_error("SIMT engine needs >= 128 SMs for its co-resident weight shards"); return WRNN_E_NO_DEVICE; }
@@ -442,7 +459,11 @@ class SimtEngine : public Engine {
 
   bool supports(const wrnn_job& job) const override { return job.mel_frames == nullptr; }   // upsampled streams only
 
-  int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) override {
+  int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) override { return run(job, stream, keys, nullptr); }
+  int score(const wrnn_job& job, float* nll, cudaStream_t stream, const FoldKey* keys) override { return run(job, stream, keys, nll); }
+
+  // nll != NULL: scoring (the loss of x_force[t] in the sampler's place)
+  int run(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys, float* nll) {
     if (job.mel_frames) { set_error("the SIMT engine takes the upsampled conditioning streams (mels_up / aux)"); return WRNN_E_INVALID; }
     if (job.uniforms_ready) { set_error("the SIMT engine needs all draws resident (no uniforms_ready)"); return WRNN_E_INVALID; }
     WRNN_CUDA_OK(cudaSetDevice(device));
@@ -473,8 +494,9 @@ class SimtEngine : public Engine {
     p.state = s; s += (size_t)P * NSTATE * Bp;
     p.xlog = s;
     p.counter = static_cast<unsigned*>(d_sync_); p.abort_flag = reinterpret_cast<int*>(static_cast<unsigned*>(d_sync_) + 8);
+    p.nll = nll;
     void* args[] = {&p};
-    const void* fn = kernel();
+    const void* fn = kernel(nll != nullptr);
     // cooperative launch: all P CTAs must be co-resident for the spin barriers to be safe
     WRNN_CUDA_OK(cudaLaunchCooperativeKernel(fn, dim3(P), dim3(NT), args, smem_bytes_, stream));
     ++launches;

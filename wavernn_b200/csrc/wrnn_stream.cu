@@ -108,6 +108,7 @@ struct StreamParams {
   int* abort_flag;
   long long* prof;              // optional cycle counters of CTA 0
   const float* expo;            // RAW: optional explicit Exp(1) draws [steps][n_total][512] (else Philox)
+  float* nll;                   // scoring (MoL): [steps][n_total] loss of target x_force[t] (out is not written)
 };
 
 __device__ __forceinline__ uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
@@ -118,8 +119,11 @@ __device__ __forceinline__ uint32_t map_to_rank(uint32_t addr, uint32_t rank) {
   uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank)); return r;
 }
 
-template <int NF, int FMT, bool FRAMES, bool PROF, int CL, bool RAW>
+// SCORE (wrnn_score, MoL only): rank 0's sampler threads write the loss of target x_force[t] instead of a sample and
+// make no draws; the cluster form broadcasts x_force[t] as it broadcasts a sample.
+template <int NF, int FMT, bool FRAMES, bool PROF, int CL, bool RAW, bool SCORE>
 __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p) {
+  static_assert(!(RAW && SCORE), "the stream engine scores the MoL head only");
   using SM = Smem<NF, RAW>;
   extern __shared__ __align__(1024) unsigned char smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM::OFF_BAR);
@@ -326,11 +330,11 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
 #pragma unroll
       for (int i = 0; i < 11; ++i) ur[i] = 0.5f;
       const bool sampler = rank == 0 && tid < B;
-      if (!RAW && p.uniforms && rank == 0 && warp == 0) {      // streamed draws: read row t once rows t .. t+3 have landed (see wrnn_tc.cu)
+      if (!RAW && !SCORE && p.uniforms && rank == 0 && warp == 0) {      // streamed draws: read row t once rows t .. t+3 have landed (see wrnn_tc.cu)
         const unsigned need = min((unsigned)S, (unsigned)t + 4u);
         if (rows_known < need) rows_known = rows_wait(p.uniforms_ready, need, p.abort_flag);
       }
-      if (!RAW && sampler) {                                   // (RAW: the fc3 epilogue draws per class)
+      if (!RAW && !SCORE && sampler) {                         // (RAW: the fc3 epilogue draws per class)
         const int gf = f0 + tid;
         if (p.uniforms) {
           const float* u = p.uniforms + (size_t)t * 11 * p.n_total;
@@ -528,14 +532,19 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
               float lgo[32];
 #pragma unroll
               for (int i = 0; i < 32; ++i) lgo[i] = log_s[lane * SM::LOGP + i];
-              xnew = mol_sample_fast(lgo, ur);
               const int gf = f0 + lane;
-              p.out[(size_t)gf * p.out_pitch + t] = xnew;
+              if constexpr (SCORE) {
+                xnew = __ldg(p.x_force + (size_t)t * p.n_total + gf);
+                p.nll[(size_t)t * p.n_total + gf] = mol_nll([&](int i) { return lgo[i]; }, xnew);
+              } else {
+                xnew = mol_sample_fast(lgo, ur);
+                p.out[(size_t)gf * p.out_pitch + t] = xnew;
+              }
               if (p.logits_out) {
 #pragma unroll
                 for (int i = 0; i < 30; ++i) p.logits_out[((size_t)t * p.n_total + gf) * 30 + i] = lgo[i];
               }
-              if (p.x_force) xnew = __ldg(p.x_force + (size_t)t * p.n_total + gf);             // teacher forcing: step t+1 consumes x_force[t]
+              if (!SCORE && p.x_force) xnew = __ldg(p.x_force + (size_t)t * p.n_total + gf);   // teacher forcing: step t+1 consumes x_force[t]
             }
             __syncwarp();
             if constexpr (CL == 1) {
@@ -652,10 +661,12 @@ class StreamEngine : public Engine {
   }
   int grid_ctas() const override { return last_grid_; }
 
-  template <int NF, int CL, bool PROF, bool RAW> const void* kernel_r(bool frames) const {
-    if (cfg.precision == WRNN_PREC_BF16) return frames ? (const void*)wrnn_stream_kernel<NF, 1, true, PROF, CL, RAW> : (const void*)wrnn_stream_kernel<NF, 1, false, PROF, CL, RAW>;
-    return frames ? (const void*)wrnn_stream_kernel<NF, 0, true, PROF, CL, RAW> : (const void*)wrnn_stream_kernel<NF, 0, false, PROF, CL, RAW>;
+  template <int NF, int CL, bool PROF, bool RAW, bool SC = false> const void* kernel_r(bool frames) const {
+    if (cfg.precision == WRNN_PREC_BF16) return frames ? (const void*)wrnn_stream_kernel<NF, 1, true, PROF, CL, RAW, SC> : (const void*)wrnn_stream_kernel<NF, 1, false, PROF, CL, RAW, SC>;
+    return frames ? (const void*)wrnn_stream_kernel<NF, 0, true, PROF, CL, RAW, SC> : (const void*)wrnn_stream_kernel<NF, 0, false, PROF, CL, RAW, SC>;
   }
+  // MoL scoring (no profiling variant)
+  template <int NF, int CL> const void* kernel_score(bool frames) const { return kernel_r<NF, CL, false, false, true>(frames); }
   template <int NF, int CL, bool PROF> const void* kernel_p(bool frames) const {
     return raw() ? kernel_r<NF, CL, PROF, true>(frames) : kernel_r<NF, CL, PROF, false>(frames);
   }
@@ -721,6 +732,14 @@ class StreamEngine : public Engine {
       WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<16, 4>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<16>()));
       WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_nf<32, 4>(fr, pr), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<32>()));
     }
+    if (!raw()) {
+      for (int fr = 0; fr < 2; ++fr) {
+        WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_score<16, 1>(fr != 0), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<16>()));
+        WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_score<32, 1>(fr != 0), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<32>()));
+        WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_score<16, 4>(fr != 0), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<16>()));
+        WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_score<32, 4>(fr != 0), cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<32>()));
+      }
+    }
     WRNN_CUDA_OK(cudaDeviceGetAttribute(&n_sm_, cudaDevAttrMultiProcessorCount, device));
     // clusters of four that fit the device at once (GPC granularity); both tile sizes use the same shared memory class
     {
@@ -758,7 +777,15 @@ class StreamEngine : public Engine {
     if (const char* e = getenv("WRNN_STREAM_CL")) { const int v = atoi(e); if (v == 1 || v == 4) cl = v; }
   }
 
-  int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) override {
+  int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) override { return run(job, stream, keys, nullptr); }
+  bool scores() const override { return !raw(); }
+  int score(const wrnn_job& job, float* nll, cudaStream_t stream, const FoldKey* keys) override {
+    if (raw()) { set_error("the stream engine scores the MoL head only: score RAW jobs on the persistent or SIMT engine"); return WRNN_E_INVALID; }
+    return run(job, stream, keys, nll);
+  }
+
+  // nll != NULL: MoL scoring (the loss of x_force[t] in the sampler's place; the draws are not read)
+  int run(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys, float* nll) {
     WRNN_CUDA_OK(cudaSetDevice(device));
     int nf = 16, cl = 1;
     choose(job.n_seg, nf, cl);
@@ -787,11 +814,15 @@ class StreamEngine : public Engine {
     p.mel_frames = job.mel_frames; p.aux_frames = job.aux_frames; p.up_taps = job.up_taps; p.hop = job.hop;
     p.state = static_cast<float*>(d_state_);
     p.abort_flag = reinterpret_cast<int*>(static_cast<unsigned*>(d_sync_) + 8);
-    const bool prof = getenv("WRNN_STREAM_PROF") != nullptr;
+    p.nll = nll;
+    if (nll) { p.uniforms = nullptr; p.uniforms_ready = nullptr; p.expo = nullptr; }
+    const bool prof = !nll && getenv("WRNN_STREAM_PROF") != nullptr;
     p.prof = reinterpret_cast<long long*>(static_cast<unsigned char*>(d_sync_) + 64);
     const bool frames = job.mel_frames != nullptr;             // rows are formed by the staging warps (no scratch of size L)
-    const void* fn = cl == 4 ? (nf == 16 ? kernel_nf<16, 4>(frames, prof) : kernel_nf<32, 4>(frames, prof))
-                             : (nf == 16 ? kernel_nf<16, 1>(frames, prof) : kernel_nf<32, 1>(frames, prof));
+    const void* fn = nll ? (cl == 4 ? (nf == 16 ? kernel_score<16, 4>(frames) : kernel_score<32, 4>(frames))
+                                    : (nf == 16 ? kernel_score<16, 1>(frames) : kernel_score<32, 1>(frames)))
+                         : cl == 4 ? (nf == 16 ? kernel_nf<16, 4>(frames, prof) : kernel_nf<32, 4>(frames, prof))
+                                   : (nf == 16 ? kernel_nf<16, 1>(frames, prof) : kernel_nf<32, 1>(frames, prof));
     void* args[] = {&p};
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(tiles * cl); lc.blockDim = dim3(NT); lc.dynamicSmemBytes = V.smem; lc.stream = stream;

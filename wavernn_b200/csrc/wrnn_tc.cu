@@ -111,6 +111,7 @@ struct TcParams {
   unsigned* counters;        // [5] monotonically increasing arrival counters
   int* abort_flag;
   long long* prof;           // cycle counters of CTA 0 (fold thread 0: [0..4], driver lane 0: [5..7])
+  float* nll;                // scoring: [steps, n_total] loss of target x_force[t] (job-wide; out is not written)
 };
 
 // ------------------------------------------------------------------------------------------
@@ -150,7 +151,10 @@ __global__ void __launch_bounds__(XP_THREADS) wrnn_expand_rows_kernel(const floa
 // ------------------------------------------------------------------------------------------
 // the kernel
 // ------------------------------------------------------------------------------------------
-template <int FMT, bool FRAMES, bool RAW, bool BIG>
+// SCORE (wrnn_score): the loss of target x_force[t] in the sampler's place, written by CTA 0; no draws are made.  MoL:
+// from the replicated logits.  RAW: the fifth exchange carries, in the candidate's 8 B, each CTA's log-sum-exp of its 4
+// classes and the target's logit from the CTA that owns the target class (-inf from the others).
+template <int FMT, bool FRAMES, bool RAW, bool BIG, bool SCORE>
 __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const float* fv = reinterpret_cast<const float*>(smem + OFF_VEC);
@@ -290,66 +294,68 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
         // This step's draws and everything computed from them alone, while the h1' exchange is in flight: at the top of
         // the step or in the sampler they sit between x_{t-1} and the h1' publish, on the critical path of every step.
         // Every thread of a fold draws the fold's MoL uniforms (the same values, so all compute the same sample).
-        float ur[11];
+        if constexpr (!SCORE) {                             // scoring makes no draws
+          float ur[11];
 #pragma unroll
-        for (int i = 0; i < 11; ++i) ur[i] = 0.5f;
-        float ex[UT];                                       // RAW: Exp(1) draws of this thread's classes
+          for (int i = 0; i < 11; ++i) ur[i] = 0.5f;
+          float ex[UT];                                       // RAW: Exp(1) draws of this thread's classes
 #pragma unroll
-        for (int i = 0; i < UT; ++i) ex[i] = 1.f;
-        if constexpr (RAW) {
-          if (owns_fold) {
-            if (p.expo) {
+          for (int i = 0; i < UT; ++i) ex[i] = 1.f;
+          if constexpr (RAW) {
+            if (owns_fold) {
+              if (p.expo) {
 #pragma unroll
-              for (int i = 0; i < UT; ++i) ex[i] = __ldg(p.expo + ((size_t)t * p.n_total + p.f0 + fold) * NCLS + u0 + j0 + i);
-            } else {                                        // same keying as the SIMT engine: block 16 + class/4
-              const FoldPhilox k = fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
-              const Philox4 r = philox4x32_10((unsigned)t, k.fold, 16u + (unsigned)cta, (unsigned)p.offset, k.k0, k.k1);
+                for (int i = 0; i < UT; ++i) ex[i] = __ldg(p.expo + ((size_t)t * p.n_total + p.f0 + fold) * NCLS + u0 + j0 + i);
+              } else {                                        // same keying as the SIMT engine: block 16 + class/4
+                const FoldPhilox k = fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
+                const Philox4 r = philox4x32_10((unsigned)t, k.fold, 16u + (unsigned)cta, (unsigned)p.offset, k.k0, k.k1);
 #pragma unroll
-              for (int i = 0; i < UT; ++i) {
-                const int j = j0 + i;
-                ex[i] = -logf(u01_open(j == 0 ? r.x : j == 1 ? r.y : j == 2 ? r.z : r.w));
+                for (int i = 0; i < UT; ++i) {
+                  const int j = j0 + i;
+                  ex[i] = -logf(u01_open(j == 0 ? r.x : j == 1 ? r.y : j == 2 ? r.z : r.w));
+                }
               }
             }
-          }
-        } else if (p.uniforms) {
-          if (p.uniforms_ready) {
-            // Streamed draws: rows land (DMA) while the kernel runs.  All 128 CTAs read the same row, so the loads must stay
-            // L1-cached (as L2 loads they cost 1 us per step: 27 k requests on a few hot lines, measured) -- which is safe
-            // only if no line is ever cached before all of it has landed: a row is >= 44 B, a 128 B line spans at most four
-            // rows, so row t is read once rows t .. t+3 are in (the host uploads in chunks of ~1000 rows: free).
-            const unsigned need = min((unsigned)S, (unsigned)t + 4u);
-            if (rows_known < need) rows_known = rows_wait(p.uniforms_ready, need, p.abort_flag);
-            if (owns_fold) {
+          } else if (p.uniforms) {
+            if (p.uniforms_ready) {
+              // Streamed draws: rows land (DMA) while the kernel runs.  All 128 CTAs read the same row, so the loads must stay
+              // L1-cached (as L2 loads they cost 1 us per step: 27 k requests on a few hot lines, measured) -- which is safe
+              // only if no line is ever cached before all of it has landed: a row is >= 44 B, a 128 B line spans at most four
+              // rows, so row t is read once rows t .. t+3 are in (the host uploads in chunks of ~1000 rows: free).
+              const unsigned need = min((unsigned)S, (unsigned)t + 4u);
+              if (rows_known < need) rows_known = rows_wait(p.uniforms_ready, need, p.abort_flag);
+              if (owns_fold) {
+                const float* u = p.uniforms + (size_t)t * 11 * p.n_total;
+#pragma unroll
+                for (int i = 0; i < 10; ++i) ur[i] = __ldca(u + (p.f0 + fold) * 10 + i);
+                ur[10] = __ldca(u + 10 * p.n_total + p.f0 + fold);
+              }
+            } else if (owns_fold) {                            // resident draws: read-only path (11 values = 2 lines per fold)
               const float* u = p.uniforms + (size_t)t * 11 * p.n_total;
 #pragma unroll
-              for (int i = 0; i < 10; ++i) ur[i] = __ldca(u + (p.f0 + fold) * 10 + i);
-              ur[10] = __ldca(u + 10 * p.n_total + p.f0 + fold);
+              for (int i = 0; i < 10; ++i) ur[i] = __ldg(u + (p.f0 + fold) * 10 + i);
+              ur[10] = __ldg(u + 10 * p.n_total + p.f0 + fold);
             }
-          } else if (owns_fold) {                            // resident draws: read-only path (11 values = 2 lines per fold)
-            const float* u = p.uniforms + (size_t)t * 11 * p.n_total;
-#pragma unroll
-            for (int i = 0; i < 10; ++i) ur[i] = __ldg(u + (p.f0 + fold) * 10 + i);
-            ur[10] = __ldg(u + 10 * p.n_total + p.f0 + fold);
+          } else if (owns_fold) {
+            {
+              const FoldPhilox k = fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
+              const unsigned g = k.fold, k0 = k.k0, k1 = k.k1, o0 = (unsigned)p.offset;
+              const Philox4 r0 = philox4x32_10((unsigned)t, g, 0u, o0, k0, k1), r1 = philox4x32_10((unsigned)t, g, 1u, o0, k0, k1),
+                            r2 = philox4x32_10((unsigned)t, g, 2u, o0, k0, k1);
+              ur[0] = u_ref_range(r0.x); ur[1] = u_ref_range(r0.y); ur[2] = u_ref_range(r0.z); ur[3] = u_ref_range(r0.w);
+              ur[4] = u_ref_range(r1.x); ur[5] = u_ref_range(r1.y); ur[6] = u_ref_range(r1.z); ur[7] = u_ref_range(r1.w);
+              ur[8] = u_ref_range(r2.x); ur[9] = u_ref_range(r2.y); ur[10] = u_ref_range(r2.z);
+            }
           }
-        } else if (owns_fold) {
-          {
-            const FoldPhilox k = fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
-            const unsigned g = k.fold, k0 = k.k0, k1 = k.k1, o0 = (unsigned)p.offset;
-            const Philox4 r0 = philox4x32_10((unsigned)t, g, 0u, o0, k0, k1), r1 = philox4x32_10((unsigned)t, g, 1u, o0, k0, k1),
-                          r2 = philox4x32_10((unsigned)t, g, 2u, o0, k0, k1);
-            ur[0] = u_ref_range(r0.x); ur[1] = u_ref_range(r0.y); ur[2] = u_ref_range(r0.z); ur[3] = u_ref_range(r0.w);
-            ur[4] = u_ref_range(r1.x); ur[5] = u_ref_range(r1.y); ur[6] = u_ref_range(r1.z); ur[7] = u_ref_range(r1.w);
-            ur[8] = u_ref_range(r2.x); ur[9] = u_ref_range(r2.y); ur[10] = u_ref_range(r2.z);
+          if constexpr (RAW) {
+#pragma unroll
+            for (int i = 0; i < UT; ++i) { lex[i] = __logf(ex[i]); settle(lex[i]); }
+          } else {
+            mol_noise_fast(ur, gn, lu);
+#pragma unroll
+            for (int i = 0; i < 10; ++i) settle(gn[i]);
+            settle(lu);
           }
-        }
-        if constexpr (RAW) {
-#pragma unroll
-          for (int i = 0; i < UT; ++i) { lex[i] = __logf(ex[i]); settle(lex[i]); }
-        } else {
-          mol_noise_fast(ur, gn, lu);
-#pragma unroll
-          for (int i = 0; i < 10; ++i) settle(gn[i]);
-          settle(lu);
         }
       }
       if (profiling) { const long long c = clock64(); tprof[0] += c - tp0; tp0 = c; }
@@ -408,7 +414,88 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
       if (profiling) { const long long c = clock64(); tprof[3] += c - tp0; tp0 = c; }
 
       // ---- E: logits = F3 y2 + b3, sample ---------------------------------------------------------------
-      if constexpr (!RAW) {                                 // MoL: fc3 + sampler replicated in every CTA
+      if constexpr (!RAW && SCORE) {                        // MoL scoring: CTA 0's fold threads
+        mbar_wait(bar_mma, n_mma & 1, p.abort_flag); ++n_mma;
+        if (active && owns_fold && slot == 0 && cta == 0) {
+          const float* lgc = acc_f + AC_F3 * ACP;
+          const size_t r = (size_t)t * p.n_total + p.f0 + fold;
+          p.nll[r] = mol_nll([&](int i) { return lgc[i * ACP] + b3[i]; }, __ldg(p.x_force + r));
+          if (p.logits_out) {
+#pragma unroll
+            for (int i = 0; i < 30; ++i) p.logits_out[r * 30 + i] = lgc[i * ACP] + b3[i];
+          }
+        }
+      } else if constexpr (RAW && SCORE) {                  // RAW scoring: partial log-sum-exps, then the exchange
+        mbar_wait(bar_mma, n_mma & 1, p.abort_flag); ++n_mma;
+        unsigned char* cand_out = p.xch5 + (size_t)par * cand_bytes;
+        const size_t r = (size_t)t * p.n_total + p.f0 + fold;
+        // The sums of exp below run in one fixed tree whatever TPF is (pairs of classes, then their sum; quarters of the
+        // CTAs, then pairs of quarters), so a fold's loss does not depend on its tile.
+        if (active) {
+          float lg[UT];
+          acc_rd(AC_F3, 0, lg);
+          const int label = owns_fold ? raw_label(__ldg(p.x_force + r), NCLS) : -1;
+          float m = -INFINITY, tl = -INFINITY;
+#pragma unroll
+          for (int i = 0; i < UT; ++i) {
+            lg[i] += b3_r[i];
+            m = fmaxf(m, lg[i]);
+            if (u0 + j0 + i == label) tl = lg[i];
+          }
+#pragma unroll
+          for (int o = 1; o < TPF; o <<= 1) {
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+            tl = fmaxf(tl, __shfl_xor_sync(0xffffffffu, tl, o));
+          }
+          float e = 0.f;
+#pragma unroll
+          for (int i = 0; i < UT; ++i) e += expf(lg[i] - m);
+#pragma unroll
+          for (int o = 1; o < TPF; o <<= 1) e += __shfl_xor_sync(0xffffffffu, e, o);
+          if (owns_fold) {
+            if (slot == 0)
+              *reinterpret_cast<uint2*>(cand_out + ((size_t)cta * n_groups * 8 + fold) * 8) = make_uint2(__float_as_uint(m + logf(e)), __float_as_uint(tl));
+            if (p.logits_out) {
+#pragma unroll
+              for (int i = 0; i < UT; ++i) p.logits_out[r * NCLS + u0 + j0 + i] = lg[i];
+            }
+          }
+        }
+        signal(4);
+        mbar_wait(bar_g, (uint32_t)((GPS * t + 4) & 1), p.abort_flag);
+        if (active && cta == 0) {
+          const uint2* cand = reinterpret_cast<const uint2*>(smem + OFF_A);
+          constexpr int QPT = 4 / TPF;                                  // quarters of the 128 CTAs per thread
+          float mx = -INFINITY, tl = -INFINITY, s = 0.f;
+          if (fold < n_groups * 8) {
+#pragma unroll 8
+            for (int c = slot * (P / TPF); c < (slot + 1) * (P / TPF); ++c) {
+              const uint2 v = cand[c * n_groups * 8 + fold];
+              mx = fmaxf(mx, __uint_as_float(v.x));
+              tl = fmaxf(tl, __uint_as_float(v.y));
+            }
+          }
+#pragma unroll
+          for (int o = 1; o < TPF; o <<= 1) {
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+            tl = fmaxf(tl, __shfl_xor_sync(0xffffffffu, tl, o));
+          }
+          if (fold < n_groups * 8) {
+            float qs[QPT];
+#pragma unroll
+            for (int qq = 0; qq < QPT; ++qq) {
+              qs[qq] = 0.f;
+              const int c0 = (slot * QPT + qq) * (P / 4);
+#pragma unroll 8
+              for (int c = c0; c < c0 + P / 4; ++c) qs[qq] += expf(__uint_as_float(cand[c * n_groups * 8 + fold].x) - mx);
+            }
+            s = QPT == 2 ? qs[0] + qs[QPT - 1] : qs[0];
+          }
+#pragma unroll
+          for (int o = 1; o < TPF; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+          if (owns_fold && slot == 0) p.nll[r] = raw_nll(mx, s, tl);
+        }
+      } else if constexpr (!RAW) {                          // MoL: fc3 + sampler replicated in every CTA
         mbar_wait(bar_mma, n_mma & 1, p.abort_flag); ++n_mma;
         if (active) {
           // every thread of a fold: the 10 mixture logits, then only the chosen component's mean and log-scale
@@ -792,16 +879,17 @@ class TcEngine : public Engine {
   const char* name() const override { return cfg.precision == WRNN_PREC_BF16 ? "tcgen05-bf16" : "tcgen05-fp16"; }
   int grid_ctas() const override { return P; }
   // FRAMES = conditioning rows built in the kernel from frame-rate tensors (wrnn_job::mel_frames)
-  template <int FMT, bool FR, bool BIG>
+  template <int FMT, bool FR, bool BIG, bool SC>
   const void* kernel_of() const {
-    return cfg.mode == WRNN_MODE_RAW ? (const void*)wrnn_tc_kernel<FMT, FR, true, BIG> : (const void*)wrnn_tc_kernel<FMT, FR, false, BIG>;
+    return cfg.mode == WRNN_MODE_RAW ? (const void*)wrnn_tc_kernel<FMT, FR, true, BIG, SC> : (const void*)wrnn_tc_kernel<FMT, FR, false, BIG, SC>;
   }
-  // frames: rows formed in the kernel from frame-rate tensors; big: tile of more than SMALL_TILE folds
-  const void* kernel(bool frames, bool big) const {
+  template <bool SC> const void* kernel_sc(bool frames, bool big) const {
     if (cfg.precision == WRNN_PREC_BF16)
-      return frames ? (big ? kernel_of<1, true, true>() : kernel_of<1, true, false>()) : (big ? kernel_of<1, false, true>() : kernel_of<1, false, false>());
-    return frames ? (big ? kernel_of<0, true, true>() : kernel_of<0, true, false>()) : (big ? kernel_of<0, false, true>() : kernel_of<0, false, false>());
+      return frames ? (big ? kernel_of<1, true, true, SC>() : kernel_of<1, true, false, SC>()) : (big ? kernel_of<1, false, true, SC>() : kernel_of<1, false, false, SC>());
+    return frames ? (big ? kernel_of<0, true, true, SC>() : kernel_of<0, true, false, SC>()) : (big ? kernel_of<0, false, true, SC>() : kernel_of<0, false, false, SC>());
   }
+  // frames: rows formed in the kernel from frame-rate tensors; big: tile of more than SMALL_TILE folds; score: wrnn_score
+  const void* kernel(bool frames, bool big, bool score) const { return score ? kernel_sc<true>(frames, big) : kernel_sc<false>(frames, big); }
   static constexpr int SMALL_TILE = 24;     // 24 folds x 26 chunks = 624 <= 5 tasks x 128 staging threads
 
   int init(const HostWeights& w) {
@@ -840,8 +928,8 @@ class TcEngine : public Engine {
     xch5_off_ = (size_t)4 * 2 * 8 * SBO_H;               // 4 vectors x 2 parities x (up to 8 row groups)
     scratch_bytes_ = xch5_off_ + (size_t)2 * P * MT * 8;   // + RAW candidates: 2 parities x 128 CTAs x 64 folds x 8 B
     WRNN_CUDA_OK(cudaMalloc(&d_scratch_, scratch_bytes_));
-    for (int v = 0; v < 4; ++v)
-      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel((v & 1) != 0, (v & 2) != 0), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    for (int v = 0; v < 8; ++v)
+      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel((v & 1) != 0, (v & 2) != 0, (v & 4) != 0), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     int n_sm = 0;
     WRNN_CUDA_OK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
     if (n_sm < P) { set_error("tcgen05 engine needs >= 128 SMs for its co-resident weight shards"); return WRNN_E_NO_DEVICE; }
@@ -854,7 +942,11 @@ class TcEngine : public Engine {
   }
   bool supports(const wrnn_job&) const override { return true; }   // any fold count: tiles of 64 folds, one launch each
 
-  int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) override {
+  int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) override { return run(job, stream, keys, nullptr); }
+  int score(const wrnn_job& job, float* nll, cudaStream_t stream, const FoldKey* keys) override { return run(job, stream, keys, nll); }
+
+  // nll != NULL: scoring (the loss of x_force[t] in the sampler's place; the draws are not read)
+  int run(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys, float* nll) {
     WRNN_CUDA_OK(cudaSetDevice(device));
     TcParams p{};
     p.blob = static_cast<const unsigned char*>(d_blob_);
@@ -872,6 +964,8 @@ class TcEngine : public Engine {
     p.counters = static_cast<unsigned*>(d_sync_);
     p.abort_flag = reinterpret_cast<int*>(static_cast<unsigned*>(d_sync_) + 8);
     p.prof = reinterpret_cast<long long*>(static_cast<unsigned char*>(d_sync_) + 64);
+    p.nll = nll;
+    if (nll) { p.uniforms = nullptr; p.expo = nullptr; p.uniforms_ready = nullptr; }
     WRNN_CUDA_OK(cudaMemsetAsync(d_sync_, 0, 256, stream));
     p.n_total = job.n_seg;
     // frame-rate conditioning: rows formed by the pre-pass into tile-local scratch (stream kernel), or in the kernel
@@ -913,7 +1007,7 @@ class TcEngine : public Engine {
       }
       WRNN_CUDA_OK(cudaMemsetAsync(d_sync_, 0, 32, stream));                       // arrival counters (the abort flag is sticky)
       void* args[] = {&p};
-      WRNN_CUDA_OK(cudaLaunchCooperativeKernel(kernel(frames && !expand, p.n_seg > SMALL_TILE), dim3(P), dim3(NT), args, SMEM_BYTES, stream));
+      WRNN_CUDA_OK(cudaLaunchCooperativeKernel(kernel(frames && !expand, p.n_seg > SMALL_TILE, nll != nullptr), dim3(P), dim3(NT), args, SMEM_BYTES, stream));
       ++launches;
     }
     last_steps_ = p.steps;
