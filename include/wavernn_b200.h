@@ -309,6 +309,36 @@ int wrnn_vocode_many(wrnn_t *h, const wrnn_vocode_batch *b, void *stream);
 /* The same with HOST mel / wav: copies in, runs, copies out, synchronises and returns wrnn_check's verdict. */
 int wrnn_vocode_many_host(wrnn_t *h, const wrnn_vocode_batch *b);
 
+/* Live unbatched vocoding ("Slow Unbatched Generation", gen_tacotron.py:31): the waveform reaches the caller while the
+ * persistent kernel is still generating it.  Unbatched generation is one fold with no cross-fade, so sample n of the
+ * waveform depends on generated sample n alone (and on the fade-out table over the last 20 hops).  The kernel stores
+ * its samples straight into a pinned host buffer the library owns and publishes how many it has stored every 64
+ * steps; each poll turns the newly published ones into float64 samples of wav with wrnn_epilogue's arithmetic.
+ *
+ * Contract: the concatenated waveform is bit-identical to wrnn_vocode_host on the same handle with the same {mel, T,
+ * batched = 0, mu_law, philox_seed}: the draws are Philox, keyed as in wrnn_vocode.
+ *
+ * Refused (WRNN_E_INVALID, the message names the cause, the handle stays usable): batched != 0 (a batched job's folds
+ * all finish at its last step); a handle whose engine for the job is not the persistent one (TCGEN05: the stream
+ * engine's cluster form is slower than real time for one fold, the SIMT engine is not timed); a null job, mel or wav;
+ * T < 21; a handle with no upsampler attached.
+ *
+ * While a live job is in flight every other entry point on the handle returns WRNN_E_BUSY (a second
+ * wrnn_vocode_live_start included); wrnn_destroy waits for the job and then frees.  A live job cannot be cancelled. */
+
+/* Starts wrnn_vocode of an UNBATCHED job (job->batched must be 0; target / overlap ignored) whose waveform is
+ * delivered while it is generated.  job->mel: host or device (UVA); job->wav: HOST, [(T - 1) * hop] float64.
+ * Enqueued on `stream`; returns without waiting for the kernel. */
+int wrnn_vocode_live_start(wrnn_t *h, const wrnn_vocode_job *job, void *stream);
+
+/* Waits up to wait_us for more samples, writes every newly final sample into job->wav and sets *n_ready to the
+ * number of leading samples of wav that are final (never decreases; never rewritten).
+ * Returns 1 while the job runs, 0 once all (T - 1) * hop samples are in wav, or a negative WRNN_E_* code
+ * (device errors as wrnn_check: samples delivered before the error stay valid).  After 0 or an error the handle is free.
+ * The wait sleeps in intervals of 100 us; wait_us <= 0 returns at once.  A null n_ready, or a handle with no live job,
+ * is refused (WRNN_E_INVALID) without touching the job. */
+int wrnn_vocode_live_poll(wrnn_t *h, int32_t wait_us, int64_t *n_ready);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Scoring: how likely a given waveform is under the model, on the engine that generates it.  The loss the reference
  * trains with (train_wavernn.py:83), per sample, teacher-forced and reduced inside the kernel where the logits are:

@@ -23,7 +23,8 @@ EXPORTS = ("wrnn_abi_version", "wrnn_last_error", "wrnn_create", "wrnn_destroy",
            "wrnn_check", "wrnn_generate_host", "wrnn_engine_name", "wrnn_grid_ctas", "wrnn_launch_count",
            "wrnn_mt19937_uniform", "wrnn_mt19937_uniform_cols", "wrnn_epilogue", "wrnn_expand_conditioning",
            "wrnn_attach_upsampler", "wrnn_conditioning_frames", "wrnn_vocode", "wrnn_vocode_host",
-           "wrnn_vocode_many", "wrnn_vocode_many_host", "wrnn_score", "wrnn_score_many", "wrnn_score_many_host")
+           "wrnn_vocode_many", "wrnn_vocode_many_host", "wrnn_score", "wrnn_score_many", "wrnn_score_many_host",
+           "wrnn_vocode_live_start", "wrnn_vocode_live_poll")
 
 _fp = C.POINTER(C.c_float)
 
@@ -167,7 +168,13 @@ def load() -> C.CDLL:
     lib.wrnn_score_many.argtypes = [C.c_void_p, C.POINTER(WrnnScoreUtt), C.c_int32, C.c_void_p]
     lib.wrnn_score_many_host.restype = C.c_int
     lib.wrnn_score_many_host.argtypes = [C.c_void_p, C.POINTER(WrnnScoreUtt), C.c_int32]
+    lib.wrnn_vocode_live_start.restype = C.c_int
+    lib.wrnn_vocode_live_start.argtypes = [C.c_void_p, C.POINTER(WrnnVocodeJob), C.c_void_p]
+    lib.wrnn_vocode_live_poll.restype = C.c_int
+    lib.wrnn_vocode_live_poll.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int64)]
     # test hooks (not declared in the header)
+    lib.wrnn_debug_live_epilogue.restype = C.c_int
+    lib.wrnn_debug_live_epilogue.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.wrnn_debug_score_many_plan.restype = C.c_int
     lib.wrnn_debug_score_many_plan.argtypes = [C.c_int32, C.POINTER(WrnnScoreUtt), C.c_int32, C.c_void_p, C.c_void_p]
     lib.wrnn_debug_vocode_many_plan.restype = C.c_int
@@ -330,6 +337,30 @@ class Engine:
         _check(self.lib, self.lib.wrnn_vocode_many_host(self._h, C.byref(b)))
         del keep
         return wavs
+
+    def vocode_live(self, mel, *, philox_seed: int, mu_law: bool = False, wait_us: int = 1000):
+        """wrnn_vocode_live_start / _poll: a generator over the float64 waveform of the unbatched vocode_host(mel,
+        batched=False, mu_law=mu_law, philox_seed=philox_seed), yielding each newly final slice while the kernel is still
+        generating (views of one array; their concatenation is bit-identical to vocode_host's).  Each poll waits up to
+        wait_us.  Closing the generator early still waits for the job, which cannot be cancelled."""
+        import numpy as np
+        mel = np.ascontiguousarray(mel[0] if mel.ndim == 3 and mel.shape[0] == 1 else mel, dtype=np.float32)
+        T = mel.shape[-1]
+        wav = np.empty(max(T - 1, 0) * getattr(self, "hop_length", 275), dtype=np.float64)
+        job = WrnnVocodeJob(mel.ctypes.data, int(T), 0, 0, 0, int(bool(mu_law)), int(philox_seed), wav.ctypes.data)
+        _check(self.lib, self.lib.wrnn_vocode_live_start(self._h, C.byref(job), None))
+        n, prev, rc = C.c_int64(0), 0, 1
+        try:
+            while rc == 1:
+                rc = self.lib.wrnn_vocode_live_poll(self._h, int(wait_us), C.byref(n))
+                if rc < 0:
+                    _check(self.lib, rc)
+                if n.value > prev:
+                    yield wav[prev:n.value]
+                    prev = n.value
+        finally:
+            while rc == 1:                               # closed early: the job runs to its end, into `wav`
+                rc = self.lib.wrnn_vocode_live_poll(self._h, 100000, C.byref(n))
 
     # ---- scoring (wrnn_score / wrnn_score_many): the reference's training loss per sample, teacher-forced ----
     def score(self, *, L: int, n_seg: int, seg_len: int, seg_stride: int, x_force: int, nll: int, mels_up: int = 0, aux: int = 0,

@@ -1,10 +1,13 @@
 // wrnn_capi.cu -- the extern "C" surface declared in include/wavernn_b200.h.
 #include <cuda_runtime.h>
 
+#include <chrono>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <new>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "wrnn_cond.h"
@@ -21,6 +24,32 @@ static int fetch(std::vector<float>& dst, const float* src, size_t n, const char
   // cudaMemcpyDefault resolves host or device pointers through UVA
   cudaError_t e = cudaMemcpy(dst.data(), src, n * sizeof(float), cudaMemcpyDefault);
   if (e != cudaSuccess) { set_error(std::string("copying ") + what + ": " + cudaGetErrorString(e)); return WRNN_E_CUDA; }
+  return WRNN_OK;
+}
+
+// wrnn_vocode_live_start's job.  The pinned buffer is mapped into the device's address space: the progress word (the
+// samples stored so far, published by the kernel), padding to 256 B, then the fp32 samples [T * hop] the kernel's
+// sample store writes.  The host reads both in place.
+struct LiveJob {
+  static constexpr size_t SAMPLES_OFF = 256;
+  void* host = nullptr;                 // cudaHostAlloc(..., cudaHostAllocMapped), grown on demand
+  void* dev = nullptr;                  // its device alias
+  size_t bytes = 0;
+  cudaEvent_t done = nullptr;           // recorded after the kernel
+  Engine* e = nullptr;
+  double* wav = nullptr;                // the caller's [wave_len]
+  long long wave_len = 0, tail_len = 0, delivered = 0;
+  int n_classes = 0;
+  std::vector<double> mu, tail;         // the epilogue tables (mu empty without mu_law)
+  unsigned long long progress() const { return __atomic_load_n(static_cast<const unsigned long long*>(host), __ATOMIC_ACQUIRE); }
+  const float* samples() const { return reinterpret_cast<const float*>(static_cast<const char*>(host) + SAMPLES_OFF); }
+};
+
+int idle_or_busy(const wrnn_handle* h) {
+  if (h && h->live_busy) {
+    set_error("a live job is in flight on this handle: wrnn_vocode_live_poll until it returns 0 or an error");
+    return WRNN_E_BUSY;
+  }
   return WRNN_OK;
 }
 }  // namespace wrnn
@@ -134,6 +163,15 @@ static int pick_engine(wrnn_t* h, const wrnn_job* job, Engine** out) {
 
 void wrnn_destroy(wrnn_t* h) {
   if (!h) return;
+  if (h->live) {                                       // a live job still in flight finishes first
+    if (h->live->done) {
+      cudaSetDevice(h->engine->device);
+      cudaEventSynchronize(h->live->done);
+      cudaEventDestroy(h->live->done);
+    }
+    if (h->live->host) cudaFreeHost(h->live->host);
+    delete h->live;
+  }
   if (h->d_stage) cudaFree(h->d_stage);
   delete h->engine;
   delete h->fallback;
@@ -164,7 +202,9 @@ static int validate(const wrnn_t* h, const wrnn_job* job, bool host, bool score 
 }
 
 int wrnn_generate(wrnn_t* h, const wrnn_job* job, void* stream) {
-  int rc = validate(h, job, false);
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  rc = validate(h, job, false);
   if (rc != WRNN_OK) return rc;
   Engine* e = nullptr;
   if ((rc = pick_engine(h, job, &e)) != WRNN_OK) return rc;
@@ -175,7 +215,9 @@ int wrnn_generate(wrnn_t* h, const wrnn_job* job, void* stream) {
 static const char* kNoRawStreamScore = "the stream engine scores the MoL head only (RAW scoring runs on the persistent or SIMT engine)";
 
 int wrnn_score(wrnn_t* h, const wrnn_job* job, float* nll, void* stream) {
-  int rc = validate(h, job, false, true);
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  rc = validate(h, job, false, true);
   if (rc != WRNN_OK) return rc;
   if (!job->x_force || !nll) { set_error("wrnn_score needs x_force (the targets) and nll"); return WRNN_E_INVALID; }
   Engine* e = nullptr;
@@ -187,11 +229,14 @@ int wrnn_score(wrnn_t* h, const wrnn_job* job, float* nll, void* stream) {
 
 int wrnn_check(wrnn_t* h) {
   if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
+  if (h->live_busy) return idle_or_busy(h);
   return h->last->check();
 }
 
 int wrnn_generate_host(wrnn_t* h, const wrnn_job* job) {
-  int rc = validate(h, job, true);
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  rc = validate(h, job, true);
   if (rc != WRNN_OK) return rc;
   Engine* e = nullptr;
   if ((rc = pick_engine(h, job, &e)) != WRNN_OK) return rc;
@@ -322,17 +367,27 @@ static int epilogue_tables(wrnn_t* h, int ov, bool mu_law, cudaStream_t st, EpTa
   return WRNN_OK;
 }
 
-static int vocode(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st) {
+// The job of wrnn_vocode up to the engine launch: fold geometry, the engine, scratch, the epilogue tables (not for a live
+// job, whose epilogue runs on the host) and the conditioning frames (or the expanded rows of a SIMT engine), enqueued on
+// st.  j.out is the sample block in scratch.
+struct VocodeJob {
+  cond::Geometry g;
+  wrnn_job j;
+  Engine* e = nullptr;
+  EpTables tabs{};
+};
+
+static int vocode_job(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st, bool live, VocodeJob* v) {
   Upsampler& u = *h->upsampler;
   const int hop = u.hop;
-  const long long T = job->T, L = T * hop, wave_len = (T - 1) * hop;
+  const long long T = job->T, L = T * hop;
   const cond::Geometry g = cond::fold_geometry(L, job->batched != 0, job->target, job->overlap);
   if (g.n_seg < 1 || g.n_seg >= (1ll << 31) || g.seg_len >= (1ll << 31)) {
     set_error("target / overlap give no fold, or folds beyond 2^31"); return WRNN_E_INVALID;
   }
   WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
 
-  wrnn_job j;
+  wrnn_job& j = v->j;
   std::memset(&j, 0, sizeof(j));
   j.L = L; j.seg_stride = g.seg_stride; j.n_seg = (int32_t)g.n_seg; j.seg_len = (int32_t)g.seg_len;
   j.philox_seed = job->philox_seed;
@@ -341,6 +396,7 @@ static int vocode(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st) {
   bool expanded = false;
   int rc = pick_vocode_engine(h, j, &e, &expanded);
   if (rc != WRNN_OK) return rc;
+  if (live && e->live_refusal()) { set_error(e->live_refusal()); return WRNN_E_INVALID; }
 
   const size_t n_mf = align_floats((size_t)(T + 4) * FEAT), n_af = align_floats((size_t)T * cond::CD);
   const size_t n_smp = align_floats((size_t)g.n_seg * g.seg_len);
@@ -352,9 +408,7 @@ static int vocode(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st) {
   float* samples = aux_frames + n_af;
 
   const bool mu_law = job->mu_law && h->engine->cfg.mode == WRNN_MODE_RAW;
-  const int ov = (int)g.overlap, nc = h->engine->cfg.n_classes;
-  EpTables tabs;
-  if ((rc = epilogue_tables(h, ov, mu_law, st, &tabs)) != WRNN_OK) return rc;
+  if (!live && (rc = epilogue_tables(h, (int)g.overlap, mu_law, st, &v->tabs)) != WRNN_OK) return rc;
 
   if ((rc = conditioning_frames(u, job->mel, T, mel_frames, aux_frames, nullptr, st)) != WRNN_OK) return rc;
   if (expanded) {
@@ -366,10 +420,21 @@ static int vocode(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st) {
     j.mel_frames = mel_frames; j.aux_frames = aux_frames; j.up_taps = u.d_taps;
   }
   j.out = samples;
+  v->g = g;
+  v->e = e;
   h->last = e;
-  if ((rc = e->generate(j, st, nullptr)) != WRNN_OK) return rc;
-  return wrnn_epilogue(samples, j.n_seg, j.seg_len, j.seg_stride, ov, tabs.fade_in, tabs.fade_out, tabs.mu, nc, tabs.tail,
-                       20ll * hop, wave_len, job->wav, st);
+  return WRNN_OK;
+}
+
+static int vocode(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st) {
+  VocodeJob v;
+  int rc = vocode_job(h, job, st, false, &v);
+  if (rc != WRNN_OK) return rc;
+  const wrnn_job& j = v.j;
+  const int hop = h->upsampler->hop;
+  if ((rc = v.e->generate(j, st, nullptr)) != WRNN_OK) return rc;
+  return wrnn_epilogue(j.out, j.n_seg, j.seg_len, j.seg_stride, (int)v.g.overlap, v.tabs.fade_in, v.tabs.fade_out, v.tabs.mu,
+                       h->engine->cfg.n_classes, v.tabs.tail, 20ll * hop, (job->T - 1) * hop, job->wav, st);
 }
 
 // wrnn_vocode_many: the batch as one job (layout: cond::batch_plan).  `b` holds DEVICE mel / wav pointers.
@@ -556,13 +621,17 @@ static int validate_many(const wrnn_t* h, const wrnn_vocode_batch* b, cond::Batc
 extern "C" {
 
 int wrnn_vocode(wrnn_t* h, const wrnn_vocode_job* job, void* stream) {
-  const int rc = validate_vocode(h, job);
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  rc = validate_vocode(h, job);
   if (rc != WRNN_OK) return rc;
   return vocode(h, job, static_cast<cudaStream_t>(stream));
 }
 
 int wrnn_vocode_host(wrnn_t* h, const wrnn_vocode_job* job) {
-  int rc = validate_vocode(h, job);
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  rc = validate_vocode(h, job);
   if (rc != WRNN_OK) return rc;
   Upsampler& u = *h->upsampler;
   WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
@@ -581,14 +650,18 @@ int wrnn_vocode_host(wrnn_t* h, const wrnn_vocode_job* job) {
 
 int wrnn_vocode_many(wrnn_t* h, const wrnn_vocode_batch* b, void* stream) {
   cond::BatchPlan pl;
-  const int rc = validate_many(h, b, pl);
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  rc = validate_many(h, b, pl);
   if (rc != WRNN_OK) return rc;
   return vocode_many(h, b, pl, static_cast<cudaStream_t>(stream));
 }
 
 int wrnn_vocode_many_host(wrnn_t* h, const wrnn_vocode_batch* b) {
   cond::BatchPlan pl;
-  int rc = validate_many(h, b, pl);
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  rc = validate_many(h, b, pl);
   if (rc != WRNN_OK) return rc;
   Upsampler& u = *h->upsampler;
   WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
@@ -617,14 +690,18 @@ int wrnn_vocode_many_host(wrnn_t* h, const wrnn_vocode_batch* b) {
 
 int wrnn_score_many(wrnn_t* h, const wrnn_score_utt* utts, int32_t n_utts, void* stream) {
   cond::BatchPlan pl;
-  const int rc = validate_score_many(h, utts, n_utts, pl);
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  rc = validate_score_many(h, utts, n_utts, pl);
   if (rc != WRNN_OK) return rc;
   return score_many(h, utts, n_utts, pl, static_cast<cudaStream_t>(stream));
 }
 
 int wrnn_score_many_host(wrnn_t* h, const wrnn_score_utt* utts, int32_t n_utts) {
   cond::BatchPlan pl;
-  int rc = validate_score_many(h, utts, n_utts, pl);
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  rc = validate_score_many(h, utts, n_utts, pl);
   if (rc != WRNN_OK) return rc;
   Upsampler& u = *h->upsampler;
   WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
@@ -650,6 +727,157 @@ int wrnn_score_many_host(wrnn_t* h, const wrnn_score_utt* utts, int32_t n_utts) 
   WRNN_CUDA_OK(cudaStreamSynchronize(0));
   return h->last->check();
 }
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------------
+// wrnn_vocode_live_start / _poll: an unbatched wrnn_vocode whose samples the host turns into the waveform while the
+// persistent kernel is still generating.  One fold, overlap 0: sample n < wave_len is final as soon as it is stored.
+// ---------------------------------------------------------------------------------------------------------------------
+// wrnn_epilogue_kernel in the unbatched geometry, on the host: samples [n0, n1) of x -> wav.  The same operations in the
+// same order: the mu-law label recovered in fp32 and rounded half to even (saturating, NaN -> 0, then clamped), 0.0 + y
+// (a -0.0 sample becomes +0.0), then the fade-out over the last tail_len samples.
+static void live_epilogue(const float* x, long long n0, long long n1, long long wave_len, long long tail_len, const double* mu,
+                          int nc, const double* tail, double* wav) {
+  for (long long n = n0; n < n1; ++n) {
+    const float xf = x[n];
+    double y = (double)xf;
+    if (mu) {
+      const float r = std::nearbyint((xf + 1.0f) * (0.5f * (float)(nc - 1)));
+      y = mu[!(r > 0.f) ? 0 : (r >= (float)(nc - 1) ? nc - 1 : (int)r)];
+    }
+    double v = 0.0 + y;
+    if (n >= wave_len - tail_len) v *= tail[n - (wave_len - tail_len)];
+    wav[n] = v;
+  }
+}
+
+static int live_grow(LiveJob& lj, size_t want) {
+  if (want <= lj.bytes) return WRNN_OK;
+  if (lj.host) cudaFreeHost(lj.host);
+  lj.host = lj.dev = nullptr; lj.bytes = 0;
+  WRNN_CUDA_OK(cudaHostAlloc(&lj.host, want, cudaHostAllocMapped));
+  WRNN_CUDA_OK(cudaHostGetDevicePointer(&lj.dev, lj.host, 0));
+  lj.bytes = want;
+  return WRNN_OK;
+}
+
+// Delivers the samples published so far (at most wave_len) into the caller's wav.
+static void live_deliver(LiveJob& lj) {
+  const unsigned long long p = lj.progress();
+  const long long ready = (long long)p < lj.wave_len ? (long long)p : lj.wave_len;
+  if (ready <= lj.delivered) return;
+  live_epilogue(lj.samples(), lj.delivered, ready, lj.wave_len, lj.tail_len, lj.mu.empty() ? nullptr : lj.mu.data(), lj.n_classes,
+                lj.tail.data(), lj.wav);
+  lj.delivered = ready;
+}
+
+extern "C" {
+
+int wrnn_vocode_live_start(wrnn_t* h, const wrnn_vocode_job* job, void* stream) {
+  if (!job) { set_error("null job"); return WRNN_E_INVALID; }
+  if (job->batched) {
+    set_error("a live job must be unbatched (batched = 0): a batched job's folds all finish at its last step, so no "
+              "sample is final before the whole job is");
+    return WRNN_E_INVALID;
+  }
+  if (!job->mel || !job->wav) { set_error("mel and wav are required"); return WRNN_E_INVALID; }
+  if (job->T < 21) { set_error("T must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples"); return WRNN_E_INVALID; }
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  if ((rc = validate_vocode(h, job)) != WRNN_OK) return rc;
+  Upsampler& u = *h->upsampler;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
+  if (!h->live && !(h->live = new (std::nothrow) LiveJob())) { set_error("out of host memory"); return WRNN_E_INVALID; }
+  LiveJob& lj = *h->live;
+
+  // the mel (host or device) into staging, so that the conditioning network reads device memory
+  const size_t n_mel = (size_t)job->T * FEAT;
+  if ((rc = grow(&u.d_stage, &u.stage_bytes, n_mel * sizeof(float))) != WRNN_OK) return rc;
+  WRNN_CUDA_OK(cudaMemcpyAsync(u.d_stage, job->mel, n_mel * sizeof(float), cudaMemcpyDefault, st));
+  wrnn_vocode_job dj = *job;
+  dj.mel = static_cast<const float*>(u.d_stage);
+  VocodeJob v;
+  if ((rc = vocode_job(h, &dj, st, true, &v)) != WRNN_OK) return rc;
+
+  const long long L = job->T * u.hop;
+  if ((rc = live_grow(lj, LiveJob::SAMPLES_OFF + (size_t)L * sizeof(float))) != WRNN_OK) return rc;
+  __atomic_store_n(static_cast<unsigned long long*>(lj.host), 0ull, __ATOMIC_RELEASE);   // no kernel of this handle runs
+  if (!lj.done) WRNN_CUDA_OK(cudaEventCreateWithFlags(&lj.done, cudaEventDisableTiming));
+  v.j.out = reinterpret_cast<float*>(static_cast<char*>(lj.dev) + LiveJob::SAMPLES_OFF);
+  if ((rc = v.e->generate_live(v.j, st, static_cast<unsigned long long*>(lj.dev))) != WRNN_OK) return rc;
+  WRNN_CUDA_OK(cudaEventRecord(lj.done, st));
+
+  const bool mu_law = job->mu_law && h->engine->cfg.mode == WRNN_MODE_RAW;
+  std::vector<double> fi, fo;
+  cond::epilogue_tables(0, mu_law, h->engine->cfg.n_classes, u.hop, fi, fo, lj.mu, lj.tail);
+  lj.e = v.e;
+  lj.wav = job->wav;
+  lj.wave_len = (job->T - 1) * u.hop;
+  lj.tail_len = 20ll * u.hop;
+  lj.delivered = 0;
+  lj.n_classes = h->engine->cfg.n_classes;
+  h->live_busy = true;
+  return WRNN_OK;
+}
+
+int wrnn_vocode_live_poll(wrnn_t* h, int32_t wait_us, int64_t* n_ready) {
+  if (!h || !h->engine || !n_ready) { set_error("null handle or n_ready"); return WRNN_E_INVALID; }
+  if (!h->live_busy) { set_error("no live job on this handle (wrnn_vocode_live_start)"); return WRNN_E_INVALID; }
+  LiveJob& lj = *h->live;
+  const auto t0 = std::chrono::steady_clock::now();
+  const auto wait = std::chrono::microseconds(wait_us > 0 ? wait_us : 0);
+  for (;;) {
+    const cudaError_t q = cudaEventQuery(lj.done);
+    if (q == cudaSuccess) {                            // the kernel has finished: every sample is published
+      h->live_busy = false;
+      int rc = lj.e->check();
+      if (rc == WRNN_OK) {
+        live_deliver(lj);
+        if (lj.delivered < lj.wave_len) {
+          set_error("live job: the kernel finished with " + std::to_string(lj.delivered) + " of " +
+                    std::to_string(lj.wave_len) + " samples published");
+          rc = WRNN_E_CUDA;
+        }
+      }
+      *n_ready = lj.delivered;
+      return rc;
+    }
+    if (q != cudaErrorNotReady) {
+      h->live_busy = false;
+      *n_ready = lj.delivered;
+      set_error(std::string("live job: ") + cudaGetErrorString(q));
+      return WRNN_E_CUDA;
+    }
+    const long long before = lj.delivered;
+    live_deliver(lj);
+    const auto left = wait - (std::chrono::steady_clock::now() - t0);
+    if (lj.delivered > before || left <= std::chrono::microseconds(0)) {
+      *n_ready = lj.delivered;
+      return 1;
+    }
+    // sleep in short intervals: a few hundred steps of the kernel each
+    std::this_thread::sleep_for(std::min<std::chrono::steady_clock::duration>(left, std::chrono::microseconds(100)));
+  }
+}
+
+// Test hook (CPU-only, no device needed): wrnn_vocode_live_poll's epilogue over samples x [n] (n <= wave_len) of an
+// unbatched job of wave_len samples at this hop, with the tables wrnn_vocode builds.  Checked in tests/test_live_abi.py.
+int wrnn_debug_live_epilogue(const float* x, int64_t n, int64_t wave_len, int32_t hop, int32_t mu_law, int32_t n_classes,
+                             double* wav) {
+  if (!x || !wav || hop <= 0 || n < 0 || n > wave_len || wave_len < 20ll * hop || (mu_law && n_classes < 2)) {
+    set_error("bad argument"); return WRNN_E_INVALID;
+  }
+  std::vector<double> fi, fo, mu, tail;
+  cond::epilogue_tables(0, mu_law != 0, n_classes, hop, fi, fo, mu, tail);
+  live_epilogue(x, 0, n, wave_len, 20ll * hop, mu_law ? mu.data() : nullptr, n_classes, tail.data(), wav);
+  return WRNN_OK;
+}
+
+}  // extern "C"
+
+extern "C" {
 
 // Test hook (CPU-only, no device needed): the stream engine's packed weight stream and step program for host-resident
 // weights, so the packing and the schedule can be interpreted and checked without a GPU (tests/test_stream_plan.py,

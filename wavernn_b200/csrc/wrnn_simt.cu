@@ -423,6 +423,9 @@ class SimtEngine : public Engine {
   const char* name() const override {
     return cfg.precision == WRNN_PREC_FP32 ? "simt-fp32" : cfg.precision == WRNN_PREC_BF16 ? "simt-bf16" : "simt-fp16";
   }
+  const char* live_refusal() const override {
+    return "live vocoding runs on the persistent engine only: the SIMT engine's step has not been timed against real time";
+  }
   template <bool SCORE> const void* kernel_of() const {
     return cfg.precision == WRNN_PREC_FP32   ? (const void*)wrnn_simt_kernel<float, SCORE>
            : cfg.precision == WRNN_PREC_BF16 ? (const void*)wrnn_simt_kernel<__nv_bfloat16, SCORE>

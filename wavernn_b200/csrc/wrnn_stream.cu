@@ -779,6 +779,10 @@ class StreamEngine : public Engine {
 
   int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) override { return run(job, stream, keys, nullptr); }
   bool scores() const override { return !raw(); }
+  const char* live_refusal() const override {
+    return "live vocoding runs on the persistent engine only: the stream engine's cluster form takes about 66 us per step, "
+           "slower than real time for one fold (DESIGN.md section 3.2)";
+  }
   int score(const wrnn_job& job, float* nll, cudaStream_t stream, const FoldKey* keys) override {
     if (raw()) { set_error("the stream engine scores the MoL head only: score RAW jobs on the persistent or SIMT engine"); return WRNN_E_INVALID; }
     return run(job, stream, keys, nll);

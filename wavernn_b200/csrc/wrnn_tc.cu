@@ -112,6 +112,7 @@ struct TcParams {
   int* abort_flag;
   long long* prof;           // cycle counters of CTA 0 (fold thread 0: [0..4], driver lane 0: [5..7])
   float* nll;                // scoring: [steps, n_total] loss of target x_force[t] (job-wide; out is not written)
+  unsigned long long* progress;   // LIVE: samples of fold 0 stored so far (mapped host memory, system-scope release)
 };
 
 // ------------------------------------------------------------------------------------------
@@ -151,10 +152,19 @@ __global__ void __launch_bounds__(XP_THREADS) wrnn_expand_rows_kernel(const floa
 // ------------------------------------------------------------------------------------------
 // the kernel
 // ------------------------------------------------------------------------------------------
+// LIVE (wrnn_vocode_live_start): one fold whose `out` is mapped host memory.  The thread that stores fold 0's sample
+// publishes progress = t + 1 every LIVE_PERIOD steps and at the last step with a system-scope release, which orders its
+// own sample stores before the word for the host's acquire load.  The release waits for those stores to reach host
+// memory, on the critical path of CTA 0's step, so it is amortised over LIVE_PERIOD steps (DESIGN §3.6).
+constexpr int LIVE_PERIOD = 64;
+__device__ __forceinline__ void live_publish(unsigned long long* progress, int t, int steps) {
+  if ((t + 1) % LIVE_PERIOD == 0 || t + 1 == steps)
+    asm volatile("st.release.sys.u64 [%0], %1;" :: "l"(progress), "l"((unsigned long long)(t + 1)) : "memory");
+}
 // SCORE (wrnn_score): the loss of target x_force[t] in the sampler's place, written by CTA 0; no draws are made.  MoL:
 // from the replicated logits.  RAW: the fifth exchange carries, in the candidate's 8 B, each CTA's log-sum-exp of its 4
 // classes and the target's logit from the CTA that owns the target class (-inf from the others).
-template <int FMT, bool FRAMES, bool RAW, bool BIG, bool SCORE>
+template <int FMT, bool FRAMES, bool RAW, bool BIG, bool SCORE, bool LIVE>
 __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const float* fv = reinterpret_cast<const float*>(smem + OFF_VEC);
@@ -511,6 +521,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
 #pragma unroll
               for (int i = 0; i < 30; ++i) p.logits_out[((size_t)t * p.n_total + p.f0 + fold) * 30 + i] = lgc[i * ACP] + b3[i];
             }
+            if constexpr (LIVE) live_publish(p.progress, t, S);
           }
         }
       } else {                                              // RAW: this CTA's 4 classes, then the candidate exchange
@@ -563,7 +574,10 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
           }
           combine_fold(best, bestk);
           x = 2.0f * (float)bestk / ((float)NCLS - 1.0f) - 1.0f;     // :235
-          if (owns_fold && slot == 0 && cta == 0) p.out[(size_t)(p.f0 + fold) * p.out_pitch + t] = x;
+          if (owns_fold && slot == 0 && cta == 0) {
+            p.out[(size_t)(p.f0 + fold) * p.out_pitch + t] = x;
+            if constexpr (LIVE) live_publish(p.progress, t, S);
+          }
         }
       }
       if (profiling) { tprof[4] += clock64() - tp0; }
@@ -879,9 +893,9 @@ class TcEngine : public Engine {
   const char* name() const override { return cfg.precision == WRNN_PREC_BF16 ? "tcgen05-bf16" : "tcgen05-fp16"; }
   int grid_ctas() const override { return P; }
   // FRAMES = conditioning rows built in the kernel from frame-rate tensors (wrnn_job::mel_frames)
-  template <int FMT, bool FR, bool BIG, bool SC>
+  template <int FMT, bool FR, bool BIG, bool SC, bool LV = false>
   const void* kernel_of() const {
-    return cfg.mode == WRNN_MODE_RAW ? (const void*)wrnn_tc_kernel<FMT, FR, true, BIG, SC> : (const void*)wrnn_tc_kernel<FMT, FR, false, BIG, SC>;
+    return cfg.mode == WRNN_MODE_RAW ? (const void*)wrnn_tc_kernel<FMT, FR, true, BIG, SC, LV> : (const void*)wrnn_tc_kernel<FMT, FR, false, BIG, SC, LV>;
   }
   template <bool SC> const void* kernel_sc(bool frames, bool big) const {
     if (cfg.precision == WRNN_PREC_BF16)
@@ -890,6 +904,10 @@ class TcEngine : public Engine {
   }
   // frames: rows formed in the kernel from frame-rate tensors; big: tile of more than SMALL_TILE folds; score: wrnn_score
   const void* kernel(bool frames, bool big, bool score) const { return score ? kernel_sc<true>(frames, big) : kernel_sc<false>(frames, big); }
+  // the live form: a one-fold tile on expanded rows (what wrnn_vocode's unbatched job runs)
+  const void* kernel_live() const {
+    return cfg.precision == WRNN_PREC_BF16 ? kernel_of<1, false, false, false, true>() : kernel_of<0, false, false, false, true>();
+  }
   static constexpr int SMALL_TILE = 24;     // 24 folds x 26 chunks = 624 <= 5 tasks x 128 staging threads
 
   int init(const HostWeights& w) {
@@ -930,6 +948,7 @@ class TcEngine : public Engine {
     WRNN_CUDA_OK(cudaMalloc(&d_scratch_, scratch_bytes_));
     for (int v = 0; v < 8; ++v)
       WRNN_CUDA_OK(cudaFuncSetAttribute(kernel((v & 1) != 0, (v & 2) != 0, (v & 4) != 0), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_live(), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     int n_sm = 0;
     WRNN_CUDA_OK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
     if (n_sm < P) { set_error("tcgen05 engine needs >= 128 SMs for its co-resident weight shards"); return WRNN_E_NO_DEVICE; }
@@ -944,9 +963,19 @@ class TcEngine : public Engine {
 
   int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) override { return run(job, stream, keys, nullptr); }
   int score(const wrnn_job& job, float* nll, cudaStream_t stream, const FoldKey* keys) override { return run(job, stream, keys, nll); }
+  const char* live_refusal() const override { return nullptr; }
+  int generate_live(const wrnn_job& job, cudaStream_t stream, unsigned long long* progress) override {
+    const bool expand = job.mel_frames && (job.cond_mode == WRNN_COND_EXPAND || (job.cond_mode == WRNN_COND_AUTO && !job.fold_row0));
+    if (job.n_seg != 1 || !expand || job.x_force || job.logits_out || !progress) {
+      set_error("live generation runs one fold on expanded frame-rate conditioning, without instrumentation");
+      return WRNN_E_INVALID;
+    }
+    return run(job, stream, nullptr, nullptr, progress);
+  }
 
-  // nll != NULL: scoring (the loss of x_force[t] in the sampler's place; the draws are not read)
-  int run(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys, float* nll) {
+  // nll != NULL: scoring (the loss of x_force[t] in the sampler's place; the draws are not read); progress != NULL: the
+  // live form (generate_live)
+  int run(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys, float* nll, unsigned long long* progress = nullptr) {
     WRNN_CUDA_OK(cudaSetDevice(device));
     TcParams p{};
     p.blob = static_cast<const unsigned char*>(d_blob_);
@@ -965,6 +994,7 @@ class TcEngine : public Engine {
     p.abort_flag = reinterpret_cast<int*>(static_cast<unsigned*>(d_sync_) + 8);
     p.prof = reinterpret_cast<long long*>(static_cast<unsigned char*>(d_sync_) + 64);
     p.nll = nll;
+    p.progress = progress;
     if (nll) { p.uniforms = nullptr; p.expo = nullptr; p.uniforms_ready = nullptr; }
     WRNN_CUDA_OK(cudaMemsetAsync(d_sync_, 0, 256, stream));
     p.n_total = job.n_seg;
@@ -1007,7 +1037,8 @@ class TcEngine : public Engine {
       }
       WRNN_CUDA_OK(cudaMemsetAsync(d_sync_, 0, 32, stream));                       // arrival counters (the abort flag is sticky)
       void* args[] = {&p};
-      WRNN_CUDA_OK(cudaLaunchCooperativeKernel(kernel(frames && !expand, p.n_seg > SMALL_TILE, nll != nullptr), dim3(P), dim3(NT), args, SMEM_BYTES, stream));
+      const void* fn = progress ? kernel_live() : kernel(frames && !expand, p.n_seg > SMALL_TILE, nll != nullptr);
+      WRNN_CUDA_OK(cudaLaunchCooperativeKernel(fn, dim3(P), dim3(NT), args, SMEM_BYTES, stream));
       ++launches;
     }
     last_steps_ = p.steps;
