@@ -339,6 +339,39 @@ int wrnn_vocode_live_start(wrnn_t *h, const wrnn_vocode_job *job, void *stream);
  * is refused (WRNN_E_INVALID) without touching the job. */
 int wrnn_vocode_live_poll(wrnn_t *h, int32_t wait_us, int64_t *n_ready);
 
+/* Live batch vocoding: up to 64 unbatched utterances in ONE persistent job, each delivered while it is generated, so
+ * that one GPU serves several listeners at once.  The layout is wrnn_vocode_many's unbatched one: utterance i is fold
+ * i, every fold runs max_i(T_i) * hop steps, and fold i's draws are keyed by (philox_seed_i, 0).  Each fold publishes
+ * its own sample count every 64 steps and at the last step, so a short utterance completes before the job ends.
+ *
+ * Contract: utterance i's concatenated waveform is bit-identical to wrnn_vocode_many_host on the same handle and batch,
+ * and so (wrnn_vocode_many's contract, fixed-engine handle) to wrnn_vocode_host with {mel_i, T_i, batched = 0, mu_law,
+ * philox_seed_i}.
+ *
+ * Refused (WRNN_E_INVALID, the message names the cause, the handle stays usable): batched != 0; n_utts < 1 or > 64
+ * (one persistent tile holds 64 folds, and a second tile would start only after the first had finished, so it would
+ * not be live); a null b, utts, mel or wav; any T_i < 21 (the message names i); a handle whose engine for the job is
+ * not the persistent one; a handle with no upsampler attached.
+ *
+ * Busy rules are those of wrnn_vocode_live_start, shared with it: while either kind of live job is in flight every other
+ * entry point returns WRNN_E_BUSY (both live starts included), and wrnn_destroy waits for the job.  Each poll serves
+ * only the jobs of its own start: the other poll refuses (WRNN_E_INVALID, naming the right poll) without touching the
+ * job. */
+
+/* Starts wrnn_vocode_many of an UNBATCHED batch (b->batched must be 0; target / overlap ignored) whose waveforms are
+ * delivered while they are generated.  utts[i].mel: host or device (UVA); utts[i].wav: HOST, [(T_i - 1) * hop] float64.
+ * Enqueued on `stream`; returns without waiting for the kernel. */
+int wrnn_vocode_many_live_start(wrnn_t *h, const wrnn_vocode_batch *b, void *stream);
+
+/* Waits up to wait_us for more samples of any utterance, writes every newly final sample into its utts[i].wav and sets
+ * n_ready[i] (an array of n_utts) to the number of leading samples of utterance i that are final (never decreases; never
+ * rewritten; utterance i is complete once n_ready[i] == (T_i - 1) * hop, possibly while the job still runs).
+ * Returns 1 while the kernel runs, 0 once every utterance is complete, or a negative WRNN_E_* code (device errors as
+ * wrnn_check: samples delivered before the error stay valid).  After 0 or an error the handle is free.  The wait is
+ * wrnn_vocode_live_poll's.  A null n_ready, or a handle with no batch live job in flight, is refused (WRNN_E_INVALID)
+ * without touching the job. */
+int wrnn_vocode_many_live_poll(wrnn_t *h, int32_t wait_us, int64_t *n_ready);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Scoring: how likely a given waveform is under the model, on the engine that generates it.  The loss the reference
  * trains with (train_wavernn.py:83), per sample, teacher-forced and reduced inside the kernel where the logits are:

@@ -24,7 +24,8 @@ EXPORTS = ("wrnn_abi_version", "wrnn_last_error", "wrnn_create", "wrnn_destroy",
            "wrnn_mt19937_uniform", "wrnn_mt19937_uniform_cols", "wrnn_epilogue", "wrnn_expand_conditioning",
            "wrnn_attach_upsampler", "wrnn_conditioning_frames", "wrnn_vocode", "wrnn_vocode_host",
            "wrnn_vocode_many", "wrnn_vocode_many_host", "wrnn_score", "wrnn_score_many", "wrnn_score_many_host",
-           "wrnn_vocode_live_start", "wrnn_vocode_live_poll")
+           "wrnn_vocode_live_start", "wrnn_vocode_live_poll", "wrnn_vocode_many_live_start",
+           "wrnn_vocode_many_live_poll")
 
 _fp = C.POINTER(C.c_float)
 
@@ -172,7 +173,14 @@ def load() -> C.CDLL:
     lib.wrnn_vocode_live_start.argtypes = [C.c_void_p, C.POINTER(WrnnVocodeJob), C.c_void_p]
     lib.wrnn_vocode_live_poll.restype = C.c_int
     lib.wrnn_vocode_live_poll.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int64)]
+    lib.wrnn_vocode_many_live_start.restype = C.c_int
+    lib.wrnn_vocode_many_live_start.argtypes = [C.c_void_p, C.POINTER(WrnnVocodeBatch), C.c_void_p]
+    lib.wrnn_vocode_many_live_poll.restype = C.c_int
+    lib.wrnn_vocode_many_live_poll.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
     # test hooks (not declared in the header)
+    lib.wrnn_debug_live_many_deliver.restype = C.c_int
+    lib.wrnn_debug_live_many_deliver.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
+                                                 C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
     lib.wrnn_debug_live_epilogue.restype = C.c_int
     lib.wrnn_debug_live_epilogue.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.wrnn_debug_score_many_plan.restype = C.c_int
@@ -361,6 +369,36 @@ class Engine:
         finally:
             while rc == 1:                               # closed early: the job runs to its end, into `wav`
                 rc = self.lib.wrnn_vocode_live_poll(self._h, 100000, C.byref(n))
+
+    def vocode_many_live(self, mels, seeds, *, mu_law: bool = False, wait_us: int = 1000):
+        """wrnn_vocode_many_live_start / _poll: a generator over the float64 waveforms of the unbatched
+        vocode_many_host(mels, seeds, batched=False, mu_law=mu_law) (up to 64 mels), yielding (i, slice) for each newly
+        final slice of waveform i while the kernel is still generating (views of one array per mel; the concatenation
+        of utterance i's slices is bit-identical to vocode_many_host's waveform i).  Each poll waits up to wait_us.
+        Closing the generator early still waits for the job, which cannot be cancelled."""
+        import numpy as np
+        mels = [np.ascontiguousarray(m[0] if m.ndim == 3 and m.shape[0] == 1 else m, dtype=np.float32) for m in mels]
+        if len(seeds) != len(mels):
+            raise ValueError("one seed per mel")
+        hop = getattr(self, "hop_length", 275)
+        wavs = [np.empty(max(m.shape[-1] - 1, 0) * hop, dtype=np.float64) for m in mels]
+        b, keep = vocode_batch([(m.ctypes.data, m.shape[-1], s, w.ctypes.data) for m, s, w in zip(mels, seeds, wavs)],
+                               batched=False, mu_law=mu_law)
+        _check(self.lib, self.lib.wrnn_vocode_many_live_start(self._h, C.byref(b), None))
+        del keep
+        n = np.zeros(len(mels), dtype=np.int64)
+        prev, rc = n.copy(), 1
+        try:
+            while rc == 1:
+                rc = self.lib.wrnn_vocode_many_live_poll(self._h, int(wait_us), n.ctypes.data)
+                if rc < 0:
+                    _check(self.lib, rc)
+                for i in np.flatnonzero(n > prev):
+                    yield int(i), wavs[i][prev[i]:n[i]]
+                    prev[i] = n[i]
+        finally:
+            while rc == 1:                               # closed early: the job runs to its end, into `wavs`
+                rc = self.lib.wrnn_vocode_many_live_poll(self._h, 100000, n.ctypes.data)
 
     # ---- scoring (wrnn_score / wrnn_score_many): the reference's training loss per sample, teacher-forced ----
     def score(self, *, L: int, n_seg: int, seg_len: int, seg_stride: int, x_force: int, nll: int, mels_up: int = 0, aux: int = 0,

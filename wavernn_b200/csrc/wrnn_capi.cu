@@ -27,27 +27,37 @@ static int fetch(std::vector<float>& dst, const float* src, size_t n, const char
   return WRNN_OK;
 }
 
-// wrnn_vocode_live_start's job.  The pinned buffer is mapped into the device's address space: the progress word (the
-// samples stored so far, published by the kernel), padding to 256 B, then the fp32 samples [T * hop] the kernel's
-// sample store writes.  The host reads both in place.
+// A live job: wrnn_vocode_live_start's one utterance or wrnn_vocode_many_live_start's n, utterance i being fold i.  The
+// pinned buffer is mapped into the device's address space: one progress word per fold (the samples of that fold stored
+// so far, published by the kernel), padded to 512 B, then the fp32 samples [n][steps] the kernel's sample store writes.
+// The host reads both in place.
 struct LiveJob {
-  static constexpr size_t SAMPLES_OFF = 256;
+  static constexpr int MAX_UTTS = 64;   // one persistent tile
+  static constexpr size_t SAMPLES_OFF = MAX_UTTS * sizeof(unsigned long long);
   void* host = nullptr;                 // cudaHostAlloc(..., cudaHostAllocMapped), grown on demand
   void* dev = nullptr;                  // its device alias
   size_t bytes = 0;
   cudaEvent_t done = nullptr;           // recorded after the kernel
   Engine* e = nullptr;
-  double* wav = nullptr;                // the caller's [wave_len]
-  long long wave_len = 0, tail_len = 0, delivered = 0;
+  bool many = false;                    // started by wrnn_vocode_many_live_start (served by its poll only)
+  long long steps = 0, tail_len = 0;    // samples per fold (the row pitch of the sample block), fade-out length
   int n_classes = 0;
+  std::vector<double*> wav;             // per utterance: the caller's [wave_len[i]]
+  std::vector<long long> wave_len, delivered;
   std::vector<double> mu, tail;         // the epilogue tables (mu empty without mu_law)
-  unsigned long long progress() const { return __atomic_load_n(static_cast<const unsigned long long*>(host), __ATOMIC_ACQUIRE); }
-  const float* samples() const { return reinterpret_cast<const float*>(static_cast<const char*>(host) + SAMPLES_OFF); }
+  int n() const { return (int)wav.size(); }
+  unsigned long long progress(int i) const {
+    return __atomic_load_n(static_cast<const unsigned long long*>(host) + i, __ATOMIC_ACQUIRE);
+  }
+  const float* samples(int i) const {
+    return reinterpret_cast<const float*>(static_cast<const char*>(host) + SAMPLES_OFF) + (size_t)i * steps;
+  }
 };
 
 int idle_or_busy(const wrnn_handle* h) {
   if (h && h->live_busy) {
-    set_error("a live job is in flight on this handle: wrnn_vocode_live_poll until it returns 0 or an error");
+    set_error(std::string("a live job is in flight on this handle: ") +
+              (h->live->many ? "wrnn_vocode_many_live_poll" : "wrnn_vocode_live_poll") + " until it returns 0 or an error");
     return WRNN_E_BUSY;
   }
   return WRNN_OK;
@@ -367,17 +377,20 @@ static int epilogue_tables(wrnn_t* h, int ov, bool mu_law, cudaStream_t st, EpTa
   return WRNN_OK;
 }
 
-// The job of wrnn_vocode up to the engine launch: fold geometry, the engine, scratch, the epilogue tables (not for a live
-// job, whose epilogue runs on the host) and the conditioning frames (or the expanded rows of a SIMT engine), enqueued on
-// st.  j.out is the sample block in scratch.
+// The job of wrnn_vocode or wrnn_vocode_many up to the engine launch: fold geometry, the engine, scratch, the epilogue
+// tables (not for a live job, whose epilogue runs on the host) and the conditioning frames (or the expanded rows of a
+// SIMT engine), enqueued on st.  j.out is the sample block in scratch.  wrnn_vocode_many's job also has per-fold Philox
+// keys and the utterance table of its epilogue, both in scratch.
 struct VocodeJob {
   cond::Geometry g;
   wrnn_job j;
   Engine* e = nullptr;
   EpTables tabs{};
+  const FoldKey* keys = nullptr;
+  const EpUtt* eu = nullptr;
 };
 
-static int vocode_job(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st, bool live, VocodeJob* v) {
+static int vocode_job(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st, VocodeJob* v) {
   Upsampler& u = *h->upsampler;
   const int hop = u.hop;
   const long long T = job->T, L = T * hop;
@@ -396,7 +409,6 @@ static int vocode_job(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st, bo
   bool expanded = false;
   int rc = pick_vocode_engine(h, j, &e, &expanded);
   if (rc != WRNN_OK) return rc;
-  if (live && e->live_refusal()) { set_error(e->live_refusal()); return WRNN_E_INVALID; }
 
   const size_t n_mf = align_floats((size_t)(T + 4) * FEAT), n_af = align_floats((size_t)T * cond::CD);
   const size_t n_smp = align_floats((size_t)g.n_seg * g.seg_len);
@@ -408,7 +420,7 @@ static int vocode_job(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st, bo
   float* samples = aux_frames + n_af;
 
   const bool mu_law = job->mu_law && h->engine->cfg.mode == WRNN_MODE_RAW;
-  if (!live && (rc = epilogue_tables(h, (int)g.overlap, mu_law, st, &v->tabs)) != WRNN_OK) return rc;
+  if ((rc = epilogue_tables(h, (int)g.overlap, mu_law, st, &v->tabs)) != WRNN_OK) return rc;
 
   if ((rc = conditioning_frames(u, job->mel, T, mel_frames, aux_frames, nullptr, st)) != WRNN_OK) return rc;
   if (expanded) {
@@ -428,7 +440,7 @@ static int vocode_job(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st, bo
 
 static int vocode(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st) {
   VocodeJob v;
-  int rc = vocode_job(h, job, st, false, &v);
+  int rc = vocode_job(h, job, st, &v);
   if (rc != WRNN_OK) return rc;
   const wrnn_job& j = v.j;
   const int hop = h->upsampler->hop;
@@ -437,14 +449,16 @@ static int vocode(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st) {
                        h->engine->cfg.n_classes, v.tabs.tail, 20ll * hop, (job->T - 1) * hop, job->wav, st);
 }
 
-// wrnn_vocode_many: the batch as one job (layout: cond::batch_plan).  `b` holds DEVICE mel / wav pointers.
-static int vocode_many(wrnn_t* h, const wrnn_vocode_batch* b, const cond::BatchPlan& pl, cudaStream_t st) {
+// wrnn_vocode_many: the batch as one job (layout: cond::batch_plan).  `b` holds DEVICE mel pointers (and DEVICE wav
+// pointers unless live).
+static int vocode_many_job(wrnn_t* h, const wrnn_vocode_batch* b, const cond::BatchPlan& pl, cudaStream_t st, bool live,
+                           VocodeJob* v) {
   Upsampler& u = *h->upsampler;
   const int hop = u.hop, n = b->n_utts;
   const size_t nf = (size_t)pl.g.n_seg;
   WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
 
-  wrnn_job j;
+  wrnn_job& j = v->j;
   std::memset(&j, 0, sizeof(j));
   j.L = pl.L; j.seg_stride = pl.g.seg_stride; j.n_seg = (int32_t)nf; j.seg_len = (int32_t)pl.g.seg_len;
   j.hop = hop; j.cond_mode = WRNN_COND_AUTO;
@@ -454,6 +468,7 @@ static int vocode_many(wrnn_t* h, const wrnn_vocode_batch* b, const cond::BatchP
   bool expanded = false;
   int rc = pick_vocode_engine(h, j, &e, &expanded);
   if (rc != WRNN_OK) return rc;
+  if (live && e->live_refusal()) { set_error(e->live_refusal()); return WRNN_E_INVALID; }
 
   // scratch: [row0 | row_end | keys | CondUtt table | EpUtt table | mel_frames | aux_frames | samples | expanded rows]
   // The frame regions span every utterance's T + 4 frames (aux_frames included, so that no row of the laid-out stream
@@ -490,9 +505,7 @@ static int vocode_many(wrnn_t* h, const wrnn_vocode_batch* b, const cond::BatchP
   const EpUtt* d_eu = reinterpret_cast<const EpUtt*>(d + 2 * b_row + b_key + b_cu);
 
   const bool mu_law = b->mu_law && h->engine->cfg.mode == WRNN_MODE_RAW;
-  const int ov = (int)pl.g.overlap;
-  EpTables tabs;
-  if ((rc = epilogue_tables(h, ov, mu_law, st, &tabs)) != WRNN_OK) return rc;
+  if (!live && (rc = epilogue_tables(h, (int)pl.g.overlap, mu_law, st, &v->tabs)) != WRNN_OK) return rc;
 
   if ((rc = conditioning_frames_batch(u, d_cu, n, pl.max_T, mel_frames, aux_frames, st)) != WRNN_OK) return rc;
   if (expanded) {
@@ -505,10 +518,23 @@ static int vocode_many(wrnn_t* h, const wrnn_vocode_batch* b, const cond::BatchP
     j.mel_frames = mel_frames; j.aux_frames = aux_frames; j.up_taps = u.d_taps;
   }
   j.out = samples;
+  v->g = pl.g;
+  v->e = e;
+  v->keys = keys;
+  v->eu = d_eu;
   h->last = e;
-  if ((rc = e->generate(j, st, keys)) != WRNN_OK) return rc;
-  return epilogue_launch(samples, j.seg_len, j.seg_stride, ov, tabs.fade_in, tabs.fade_out, tabs.mu, h->engine->cfg.n_classes,
-                         tabs.tail, 20ll * hop, d_eu, EpUtt{0, 0, 0, nullptr}, n, pl.max_wave, st);
+  return WRNN_OK;
+}
+
+static int vocode_many(wrnn_t* h, const wrnn_vocode_batch* b, const cond::BatchPlan& pl, cudaStream_t st) {
+  VocodeJob v;
+  int rc = vocode_many_job(h, b, pl, st, false, &v);
+  if (rc != WRNN_OK) return rc;
+  const wrnn_job& j = v.j;
+  if ((rc = v.e->generate(j, st, v.keys)) != WRNN_OK) return rc;
+  return epilogue_launch(j.out, j.seg_len, j.seg_stride, (int)v.g.overlap, v.tabs.fade_in, v.tabs.fade_out, v.tabs.mu,
+                         h->engine->cfg.n_classes, v.tabs.tail, 20ll * h->upsampler->hop, v.eu, EpUtt{0, 0, 0, nullptr},
+                         b->n_utts, pl.max_wave, st);
 }
 
 // wrnn_score_many: each utterance one fold (layout: cond::score_plan).  Its samples are gathered into the x_force block
@@ -733,6 +759,8 @@ int wrnn_score_many_host(wrnn_t* h, const wrnn_score_utt* utts, int32_t n_utts) 
 // ---------------------------------------------------------------------------------------------------------------------
 // wrnn_vocode_live_start / _poll: an unbatched wrnn_vocode whose samples the host turns into the waveform while the
 // persistent kernel is still generating.  One fold, overlap 0: sample n < wave_len is final as soon as it is stored.
+// wrnn_vocode_many_live_start / _poll: the same for an unbatched wrnn_vocode_many of up to 64 utterances, one fold each,
+// in one tile; each fold publishes its own progress.
 // ---------------------------------------------------------------------------------------------------------------------
 // wrnn_epilogue_kernel in the unbatched geometry, on the host: samples [n0, n1) of x -> wav.  The same operations in the
 // same order: the mu-law label recovered in fp32 and rounded half to even (saturating, NaN -> 0, then clamped), 0.0 + y
@@ -762,14 +790,135 @@ static int live_grow(LiveJob& lj, size_t want) {
   return WRNN_OK;
 }
 
-// Delivers the samples published so far (at most wave_len) into the caller's wav.
-static void live_deliver(LiveJob& lj) {
-  const unsigned long long p = lj.progress();
-  const long long ready = (long long)p < lj.wave_len ? (long long)p : lj.wave_len;
-  if (ready <= lj.delivered) return;
-  live_epilogue(lj.samples(), lj.delivered, ready, lj.wave_len, lj.tail_len, lj.mu.empty() ? nullptr : lj.mu.data(), lj.n_classes,
-                lj.tail.data(), lj.wav);
-  lj.delivered = ready;
+// Delivers, per utterance, the samples its fold has published so far (at most its wave_len) into the caller's wav.
+// Returns whether any utterance received samples.
+static bool live_deliver(LiveJob& lj) {
+  bool more = false;
+  for (int i = 0; i < lj.n(); ++i) {
+    const unsigned long long p = lj.progress(i);
+    const long long ready = (long long)p < lj.wave_len[i] ? (long long)p : lj.wave_len[i];
+    if (ready <= lj.delivered[i]) continue;
+    live_epilogue(lj.samples(i), lj.delivered[i], ready, lj.wave_len[i], lj.tail_len, lj.mu.empty() ? nullptr : lj.mu.data(),
+                  lj.n_classes, lj.tail.data(), lj.wav[i]);
+    lj.delivered[i] = ready;
+    more = true;
+  }
+  return more;
+}
+
+// The launch of a live job set up by vocode_many_job: fold i (utterance i, of T[i] frames) stores its
+// samples into row i of the pinned buffer and publishes its progress word; the poll delivers them into wav[i].
+static int live_launch(wrnn_t* h, VocodeJob& v, bool many, bool mu_law, const std::vector<double*>& wav,
+                       const std::vector<long long>& T, cudaStream_t st) {
+  if (!h->live && !(h->live = new (std::nothrow) LiveJob())) { set_error("out of host memory"); return WRNN_E_INVALID; }
+  LiveJob& lj = *h->live;
+  const int n = (int)wav.size(), hop = h->upsampler->hop;
+  const long long steps = v.j.seg_len;
+  int rc = live_grow(lj, LiveJob::SAMPLES_OFF + (size_t)n * steps * sizeof(float));
+  if (rc != WRNN_OK) return rc;
+  for (int i = 0; i < n; ++i)                                   // no kernel of this handle runs
+    __atomic_store_n(static_cast<unsigned long long*>(lj.host) + i, 0ull, __ATOMIC_RELEASE);
+  if (!lj.done) WRNN_CUDA_OK(cudaEventCreateWithFlags(&lj.done, cudaEventDisableTiming));
+  v.j.out = reinterpret_cast<float*>(static_cast<char*>(lj.dev) + LiveJob::SAMPLES_OFF);
+  if ((rc = v.e->generate_live(v.j, st, v.keys, static_cast<unsigned long long*>(lj.dev))) != WRNN_OK) return rc;
+  WRNN_CUDA_OK(cudaEventRecord(lj.done, st));
+
+  std::vector<double> fi, fo;
+  cond::epilogue_tables(0, mu_law, h->engine->cfg.n_classes, hop, fi, fo, lj.mu, lj.tail);
+  lj.e = v.e;
+  lj.many = many;
+  lj.steps = steps;
+  lj.tail_len = 20ll * hop;
+  lj.n_classes = h->engine->cfg.n_classes;
+  lj.wav = wav;
+  lj.wave_len.resize(n);
+  for (int i = 0; i < n; ++i) lj.wave_len[i] = (T[i] - 1) * hop;
+  lj.delivered.assign(n, 0);
+  h->live_busy = true;
+  return WRNN_OK;
+}
+
+// Both polls: waits up to wait_us for more samples of the job the matching start began and delivers them; n_ready[i] =
+// the final samples of utterance i.
+static int live_poll(wrnn_t* h, int32_t wait_us, bool many, int64_t* n_ready) {
+  if (!h || !h->engine || !n_ready) { set_error("null handle or n_ready"); return WRNN_E_INVALID; }
+  if (!h->live_busy) {
+    set_error(many ? "no batch live job on this handle (wrnn_vocode_many_live_start)" : "no live job on this handle (wrnn_vocode_live_start)");
+    return WRNN_E_INVALID;
+  }
+  LiveJob& lj = *h->live;
+  if (lj.many != many) {
+    set_error(many ? "the live job in flight was started by wrnn_vocode_live_start: poll it with wrnn_vocode_live_poll"
+                   : "the live job in flight was started by wrnn_vocode_many_live_start: poll it with wrnn_vocode_many_live_poll");
+    return WRNN_E_INVALID;
+  }
+  auto report = [&] { for (int i = 0; i < lj.n(); ++i) n_ready[i] = lj.delivered[i]; };
+  const auto t0 = std::chrono::steady_clock::now();
+  const auto wait = std::chrono::microseconds(wait_us > 0 ? wait_us : 0);
+  for (;;) {
+    const cudaError_t q = cudaEventQuery(lj.done);
+    if (q == cudaSuccess) {                            // the kernel has finished: every sample is published
+      h->live_busy = false;
+      int rc = lj.e->check();
+      if (rc == WRNN_OK) {
+        live_deliver(lj);
+        for (int i = 0; i < lj.n() && rc == WRNN_OK; ++i)
+          if (lj.delivered[i] < lj.wave_len[i]) {
+            set_error("live job: the kernel finished with " + std::to_string(lj.delivered[i]) + " of " +
+                      std::to_string(lj.wave_len[i]) + " samples of utterance " + std::to_string(i) + " published");
+            rc = WRNN_E_CUDA;
+          }
+      }
+      report();
+      return rc;
+    }
+    if (q != cudaErrorNotReady) {
+      h->live_busy = false;
+      report();
+      set_error(std::string("live job: ") + cudaGetErrorString(q));
+      return WRNN_E_CUDA;
+    }
+    const bool more = live_deliver(lj);
+    const auto left = wait - (std::chrono::steady_clock::now() - t0);
+    if (more || left <= std::chrono::microseconds(0)) {
+      report();
+      return 1;
+    }
+    // sleep in short intervals: a few hundred steps of the kernel each
+    std::this_thread::sleep_for(std::min<std::chrono::steady_clock::duration>(left, std::chrono::microseconds(100)));
+  }
+}
+
+// Both live starts, after their own refusals (b is unbatched, of 1 to 64 utterances with mel, wav and T >= 21): the
+// batch laid out as wrnn_vocode_many's job, launched live.
+static int live_start(wrnn_t* h, const wrnn_vocode_batch* b, bool many, cudaStream_t st) {
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  cond::BatchPlan pl;
+  if ((rc = validate_many(h, b, pl)) != WRNN_OK) return rc;
+  Upsampler& u = *h->upsampler;
+  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
+
+  // the mels (host or device) into staging, so that the conditioning network reads device memory
+  const int n = b->n_utts;
+  std::vector<size_t> mel_off(n + 1, 0);
+  for (int i = 0; i < n; ++i) mel_off[i + 1] = mel_off[i] + align_floats((size_t)b->utts[i].T * FEAT);
+  if ((rc = grow(&u.d_stage, &u.stage_bytes, mel_off[n] * sizeof(float))) != WRNN_OK) return rc;
+  float* d_mel = static_cast<float*>(u.d_stage);
+  std::vector<wrnn_utterance> du(b->utts, b->utts + n);
+  std::vector<double*> wav(n);
+  std::vector<long long> T(n);
+  for (int i = 0; i < n; ++i) {
+    WRNN_CUDA_OK(cudaMemcpyAsync(d_mel + mel_off[i], b->utts[i].mel, (size_t)b->utts[i].T * FEAT * sizeof(float), cudaMemcpyDefault, st));
+    du[i].mel = d_mel + mel_off[i];
+    wav[i] = b->utts[i].wav;
+    T[i] = b->utts[i].T;
+  }
+  wrnn_vocode_batch db = *b;
+  db.utts = du.data();
+  VocodeJob v;
+  if ((rc = vocode_many_job(h, &db, pl, st, true, &v)) != WRNN_OK) return rc;
+  return live_launch(h, v, many, b->mu_law && h->engine->cfg.mode == WRNN_MODE_RAW, wav, T, st);
 }
 
 extern "C" {
@@ -783,84 +932,39 @@ int wrnn_vocode_live_start(wrnn_t* h, const wrnn_vocode_job* job, void* stream) 
   }
   if (!job->mel || !job->wav) { set_error("mel and wav are required"); return WRNN_E_INVALID; }
   if (job->T < 21) { set_error("T must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples"); return WRNN_E_INVALID; }
-  int rc = idle_or_busy(h);
-  if (rc != WRNN_OK) return rc;
-  if ((rc = validate_vocode(h, job)) != WRNN_OK) return rc;
-  Upsampler& u = *h->upsampler;
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
-  if (!h->live && !(h->live = new (std::nothrow) LiveJob())) { set_error("out of host memory"); return WRNN_E_INVALID; }
-  LiveJob& lj = *h->live;
-
-  // the mel (host or device) into staging, so that the conditioning network reads device memory
-  const size_t n_mel = (size_t)job->T * FEAT;
-  if ((rc = grow(&u.d_stage, &u.stage_bytes, n_mel * sizeof(float))) != WRNN_OK) return rc;
-  WRNN_CUDA_OK(cudaMemcpyAsync(u.d_stage, job->mel, n_mel * sizeof(float), cudaMemcpyDefault, st));
-  wrnn_vocode_job dj = *job;
-  dj.mel = static_cast<const float*>(u.d_stage);
-  VocodeJob v;
-  if ((rc = vocode_job(h, &dj, st, true, &v)) != WRNN_OK) return rc;
-
-  const long long L = job->T * u.hop;
-  if ((rc = live_grow(lj, LiveJob::SAMPLES_OFF + (size_t)L * sizeof(float))) != WRNN_OK) return rc;
-  __atomic_store_n(static_cast<unsigned long long*>(lj.host), 0ull, __ATOMIC_RELEASE);   // no kernel of this handle runs
-  if (!lj.done) WRNN_CUDA_OK(cudaEventCreateWithFlags(&lj.done, cudaEventDisableTiming));
-  v.j.out = reinterpret_cast<float*>(static_cast<char*>(lj.dev) + LiveJob::SAMPLES_OFF);
-  if ((rc = v.e->generate_live(v.j, st, static_cast<unsigned long long*>(lj.dev))) != WRNN_OK) return rc;
-  WRNN_CUDA_OK(cudaEventRecord(lj.done, st));
-
-  const bool mu_law = job->mu_law && h->engine->cfg.mode == WRNN_MODE_RAW;
-  std::vector<double> fi, fo;
-  cond::epilogue_tables(0, mu_law, h->engine->cfg.n_classes, u.hop, fi, fo, lj.mu, lj.tail);
-  lj.e = v.e;
-  lj.wav = job->wav;
-  lj.wave_len = (job->T - 1) * u.hop;
-  lj.tail_len = 20ll * u.hop;
-  lj.delivered = 0;
-  lj.n_classes = h->engine->cfg.n_classes;
-  h->live_busy = true;
-  return WRNN_OK;
+  // the batch of one utterance: the same fold, keyed (philox_seed, 0), as wrnn_vocode's unbatched job
+  const wrnn_utterance u{job->mel, job->T, job->philox_seed, job->wav};
+  const wrnn_vocode_batch b{&u, 1, 0, 0, 0, job->mu_law};
+  return live_start(h, &b, false, static_cast<cudaStream_t>(stream));
 }
 
-int wrnn_vocode_live_poll(wrnn_t* h, int32_t wait_us, int64_t* n_ready) {
-  if (!h || !h->engine || !n_ready) { set_error("null handle or n_ready"); return WRNN_E_INVALID; }
-  if (!h->live_busy) { set_error("no live job on this handle (wrnn_vocode_live_start)"); return WRNN_E_INVALID; }
-  LiveJob& lj = *h->live;
-  const auto t0 = std::chrono::steady_clock::now();
-  const auto wait = std::chrono::microseconds(wait_us > 0 ? wait_us : 0);
-  for (;;) {
-    const cudaError_t q = cudaEventQuery(lj.done);
-    if (q == cudaSuccess) {                            // the kernel has finished: every sample is published
-      h->live_busy = false;
-      int rc = lj.e->check();
-      if (rc == WRNN_OK) {
-        live_deliver(lj);
-        if (lj.delivered < lj.wave_len) {
-          set_error("live job: the kernel finished with " + std::to_string(lj.delivered) + " of " +
-                    std::to_string(lj.wave_len) + " samples published");
-          rc = WRNN_E_CUDA;
-        }
-      }
-      *n_ready = lj.delivered;
-      return rc;
-    }
-    if (q != cudaErrorNotReady) {
-      h->live_busy = false;
-      *n_ready = lj.delivered;
-      set_error(std::string("live job: ") + cudaGetErrorString(q));
-      return WRNN_E_CUDA;
-    }
-    const long long before = lj.delivered;
-    live_deliver(lj);
-    const auto left = wait - (std::chrono::steady_clock::now() - t0);
-    if (lj.delivered > before || left <= std::chrono::microseconds(0)) {
-      *n_ready = lj.delivered;
-      return 1;
-    }
-    // sleep in short intervals: a few hundred steps of the kernel each
-    std::this_thread::sleep_for(std::min<std::chrono::steady_clock::duration>(left, std::chrono::microseconds(100)));
+int wrnn_vocode_live_poll(wrnn_t* h, int32_t wait_us, int64_t* n_ready) { return live_poll(h, wait_us, false, n_ready); }
+
+int wrnn_vocode_many_live_start(wrnn_t* h, const wrnn_vocode_batch* b, void* stream) {
+  if (!b) { set_error("null batch"); return WRNN_E_INVALID; }
+  if (b->batched) {
+    set_error("a live batch must be unbatched (batched = 0): a batched job's folds all finish at its last step, so no "
+              "sample is final before the whole job is");
+    return WRNN_E_INVALID;
   }
+  if (b->n_utts < 1 || b->n_utts > LiveJob::MAX_UTTS) {
+    set_error("a live batch holds 1 to 64 utterances: one persistent tile holds 64 folds, and a second tile would start "
+              "only after the first has finished");
+    return WRNN_E_INVALID;
+  }
+  if (!b->utts) { set_error("utts is required"); return WRNN_E_INVALID; }
+  for (int i = 0; i < b->n_utts; ++i) {
+    const std::string at = "utterance " + std::to_string(i) + ": ";
+    if (!b->utts[i].mel || !b->utts[i].wav) { set_error(at + "mel and wav are required"); return WRNN_E_INVALID; }
+    if (b->utts[i].T < 21) {
+      set_error(at + "T must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples");
+      return WRNN_E_INVALID;
+    }
+  }
+  return live_start(h, b, true, static_cast<cudaStream_t>(stream));
 }
+
+int wrnn_vocode_many_live_poll(wrnn_t* h, int32_t wait_us, int64_t* n_ready) { return live_poll(h, wait_us, true, n_ready); }
 
 // Test hook (CPU-only, no device needed): wrnn_vocode_live_poll's epilogue over samples x [n] (n <= wave_len) of an
 // unbatched job of wave_len samples at this hop, with the tables wrnn_vocode builds.  Checked in tests/test_live_abi.py.
@@ -872,6 +976,40 @@ int wrnn_debug_live_epilogue(const float* x, int64_t n, int64_t wave_len, int32_
   std::vector<double> fi, fo, mu, tail;
   cond::epilogue_tables(0, mu_law != 0, n_classes, hop, fi, fo, mu, tail);
   live_epilogue(x, 0, n, wave_len, 20ll * hop, mu_law ? mu.data() : nullptr, n_classes, tail.data(), wav);
+  return WRNN_OK;
+}
+
+// Test hook (CPU-only, no device needed): one delivery of a poll of wrnn_vocode_many_live_poll, on a host buffer laid
+// out as the live job's pinned one.  Utterance i (T[i] frames) is fold i with samples x [n_utts][steps] and published
+// progress[i]; delivered [n_utts] holds what earlier polls delivered and receives what this one did; wav is the
+// concatenation of the n_utts waveforms.  Checked in tests/test_live_many_abi.py.
+int wrnn_debug_live_many_deliver(const float* x, int64_t steps, const uint64_t* progress, int32_t n_utts, const int64_t* T,
+                                 int32_t hop, int32_t mu_law, int32_t n_classes, int64_t* delivered, double* wav) {
+  if (!x || !progress || !T || !delivered || !wav || steps <= 0 || hop <= 0 || n_utts < 1 || n_utts > LiveJob::MAX_UTTS ||
+      (mu_law && n_classes < 2)) {
+    set_error("bad argument"); return WRNN_E_INVALID;
+  }
+  for (int i = 0; i < n_utts; ++i)
+    if (T[i] < 21 || T[i] * hop > steps || delivered[i] < 0 || delivered[i] > (T[i] - 1) * hop) { set_error("bad argument"); return WRNN_E_INVALID; }
+  std::vector<unsigned char> buf(LiveJob::SAMPLES_OFF + (size_t)n_utts * steps * sizeof(float));
+  std::memcpy(buf.data(), progress, (size_t)n_utts * sizeof(uint64_t));
+  std::memcpy(buf.data() + LiveJob::SAMPLES_OFF, x, (size_t)n_utts * steps * sizeof(float));
+  LiveJob lj;
+  lj.host = buf.data();
+  lj.steps = steps;
+  lj.tail_len = 20ll * hop;
+  lj.n_classes = n_classes;
+  std::vector<double> fi, fo;
+  cond::epilogue_tables(0, mu_law != 0, n_classes, hop, fi, fo, lj.mu, lj.tail);
+  double* w = wav;
+  for (int i = 0; i < n_utts; ++i) {
+    lj.wav.push_back(w);
+    lj.wave_len.push_back((T[i] - 1) * hop);
+    lj.delivered.push_back(delivered[i]);
+    w += (T[i] - 1) * hop;
+  }
+  live_deliver(lj);
+  for (int i = 0; i < n_utts; ++i) delivered[i] = lj.delivered[i];
   return WRNN_OK;
 }
 

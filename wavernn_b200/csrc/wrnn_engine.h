@@ -39,11 +39,12 @@ class Engine {
   virtual int check() = 0;                                              // after stream sync
   virtual bool supports(const wrnn_job& job) const { (void)job; return true; }   // job inside this engine's envelope?
   virtual bool scores() const { return true; }                          // serves wrnn_score for this handle's head?
-  // Live vocoding (wrnn_vocode_live_start): NULL when this engine serves it, else why not.  generate_live runs a one-fold
-  // job whose `out` is mapped host memory and publishes the samples stored so far to *progress (mapped host memory).
+  // Live vocoding (wrnn_vocode_live_start, wrnn_vocode_many_live_start): NULL when this engine serves it, else why not.
+  // generate_live runs a job of one tile (up to 64 folds, keyed by `keys` as generate) whose `out` is mapped host memory
+  // and publishes the samples of fold f stored so far to progress[f] (mapped host memory).
   virtual const char* live_refusal() const { return "live vocoding runs on the persistent engine only"; }
-  virtual int generate_live(const wrnn_job& job, cudaStream_t stream, unsigned long long* progress) {
-    (void)job; (void)stream; (void)progress;
+  virtual int generate_live(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys, unsigned long long* progress) {
+    (void)job; (void)stream; (void)keys; (void)progress;
     set_error(live_refusal());
     return WRNN_E_INVALID;
   }
@@ -80,7 +81,7 @@ int epilogue_launch(const float* samples, int seg_len, long long seg_stride, int
 
 struct Upsampler;                                // conditioning network on the device (wrnn_cond.h)
 void destroy_upsampler(Upsampler* u);
-struct LiveJob;                                  // wrnn_vocode_live_start's job and its pinned buffer (wrnn_capi.cu)
+struct LiveJob;                                  // a live job and its pinned buffer (wrnn_capi.cu)
 
 }  // namespace wrnn
 
@@ -97,7 +98,8 @@ struct wrnn_handle {
   size_t stage_bytes = 0;
   // wrnn_attach_upsampler: folded MelResNet, tap table and the scratch of wrnn_vocode
   wrnn::Upsampler* upsampler = nullptr;
-  // wrnn_vocode_live_start: the live job (in flight while live_busy) and its pinned, mapped host buffer
+  // wrnn_vocode_live_start / wrnn_vocode_many_live_start: the live job (in flight while live_busy) and its pinned, mapped
+  // host buffer
   wrnn::LiveJob* live = nullptr;
   bool live_busy = false;
 };

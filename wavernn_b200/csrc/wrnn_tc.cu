@@ -112,7 +112,7 @@ struct TcParams {
   int* abort_flag;
   long long* prof;           // cycle counters of CTA 0 (fold thread 0: [0..4], driver lane 0: [5..7])
   float* nll;                // scoring: [steps, n_total] loss of target x_force[t] (job-wide; out is not written)
-  unsigned long long* progress;   // LIVE: samples of fold 0 stored so far (mapped host memory, system-scope release)
+  unsigned long long* progress;   // LIVE: [n_total] samples of each fold stored so far (mapped host memory, system-scope release)
 };
 
 // ------------------------------------------------------------------------------------------
@@ -152,10 +152,11 @@ __global__ void __launch_bounds__(XP_THREADS) wrnn_expand_rows_kernel(const floa
 // ------------------------------------------------------------------------------------------
 // the kernel
 // ------------------------------------------------------------------------------------------
-// LIVE (wrnn_vocode_live_start): one fold whose `out` is mapped host memory.  The thread that stores fold 0's sample
-// publishes progress = t + 1 every LIVE_PERIOD steps and at the last step with a system-scope release, which orders its
-// own sample stores before the word for the host's acquire load.  The release waits for those stores to reach host
-// memory, on the critical path of CTA 0's step, so it is amortised over LIVE_PERIOD steps (DESIGN §3.6).
+// LIVE (wrnn_vocode_live_start, wrnn_vocode_many_live_start): a FRAMES tile whose `out` is mapped host memory.  The
+// thread that stores fold f's sample publishes progress[f] = t + 1 every LIVE_PERIOD steps and at the last step with a
+// system-scope release, which orders its own sample stores before the word for the host's acquire load.  The release
+// waits for those stores to reach host memory, on the critical path of CTA 0's step, so it is amortised over
+// LIVE_PERIOD steps (DESIGN §3.6).  Each fold's word has exactly one writer, the thread that stored all of its samples.
 constexpr int LIVE_PERIOD = 64;
 __device__ __forceinline__ void live_publish(unsigned long long* progress, int t, int steps) {
   if ((t + 1) % LIVE_PERIOD == 0 || t + 1 == steps)
@@ -521,7 +522,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
 #pragma unroll
               for (int i = 0; i < 30; ++i) p.logits_out[((size_t)t * p.n_total + p.f0 + fold) * 30 + i] = lgc[i * ACP] + b3[i];
             }
-            if constexpr (LIVE) live_publish(p.progress, t, S);
+            if constexpr (LIVE) live_publish(p.progress + p.f0 + fold, t, S);
           }
         }
       } else {                                              // RAW: this CTA's 4 classes, then the candidate exchange
@@ -576,7 +577,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
           x = 2.0f * (float)bestk / ((float)NCLS - 1.0f) - 1.0f;     // :235
           if (owns_fold && slot == 0 && cta == 0) {
             p.out[(size_t)(p.f0 + fold) * p.out_pitch + t] = x;
-            if constexpr (LIVE) live_publish(p.progress, t, S);
+            if constexpr (LIVE) live_publish(p.progress + p.f0 + fold, t, S);
           }
         }
       }
@@ -904,10 +905,12 @@ class TcEngine : public Engine {
   }
   // frames: rows formed in the kernel from frame-rate tensors; big: tile of more than SMALL_TILE folds; score: wrnn_score
   const void* kernel(bool frames, bool big, bool score) const { return score ? kernel_sc<true>(frames, big) : kernel_sc<false>(frames, big); }
-  // the live form: a one-fold tile on expanded rows (what wrnn_vocode's unbatched job runs)
-  const void* kernel_live() const {
-    return cfg.precision == WRNN_PREC_BF16 ? kernel_of<1, false, false, false, true>() : kernel_of<0, false, false, false, true>();
+  // the live form: a small or BIG tile on rows formed in the kernel from fold tables (what wrnn_vocode_many's unbatched
+  // job runs)
+  template <bool BIG> const void* kernel_lv() const {
+    return cfg.precision == WRNN_PREC_BF16 ? kernel_of<1, true, BIG, false, true>() : kernel_of<0, true, BIG, false, true>();
   }
+  const void* kernel_live(bool big) const { return big ? kernel_lv<true>() : kernel_lv<false>(); }
   static constexpr int SMALL_TILE = 24;     // 24 folds x 26 chunks = 624 <= 5 tasks x 128 staging threads
 
   int init(const HostWeights& w) {
@@ -948,7 +951,8 @@ class TcEngine : public Engine {
     WRNN_CUDA_OK(cudaMalloc(&d_scratch_, scratch_bytes_));
     for (int v = 0; v < 8; ++v)
       WRNN_CUDA_OK(cudaFuncSetAttribute(kernel((v & 1) != 0, (v & 2) != 0, (v & 4) != 0), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_live(), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    for (int v = 0; v < 2; ++v)
+      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_live(v != 0), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     int n_sm = 0;
     WRNN_CUDA_OK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
     if (n_sm < P) { set_error("tcgen05 engine needs >= 128 SMs for its co-resident weight shards"); return WRNN_E_NO_DEVICE; }
@@ -964,13 +968,14 @@ class TcEngine : public Engine {
   int generate(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys) override { return run(job, stream, keys, nullptr); }
   int score(const wrnn_job& job, float* nll, cudaStream_t stream, const FoldKey* keys) override { return run(job, stream, keys, nll); }
   const char* live_refusal() const override { return nullptr; }
-  int generate_live(const wrnn_job& job, cudaStream_t stream, unsigned long long* progress) override {
-    const bool expand = job.mel_frames && (job.cond_mode == WRNN_COND_EXPAND || (job.cond_mode == WRNN_COND_AUTO && !job.fold_row0));
-    if (job.n_seg != 1 || !expand || job.x_force || job.logits_out || !progress) {
-      set_error("live generation runs one fold on expanded frame-rate conditioning, without instrumentation");
+  int generate_live(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys, unsigned long long* progress) override {
+    const bool tables = job.mel_frames && job.fold_row0 && job.cond_mode != WRNN_COND_EXPAND;
+    if (!tables || job.n_seg > MT || job.x_force || job.logits_out || !progress) {
+      set_error("live generation runs one tile of up to 64 folds on frame-rate conditioning with fold tables, without "
+                "instrumentation");
       return WRNN_E_INVALID;
     }
-    return run(job, stream, nullptr, nullptr, progress);
+    return run(job, stream, keys, nullptr, progress);
   }
 
   // nll != NULL: scoring (the loss of x_force[t] in the sampler's place; the draws are not read); progress != NULL: the
@@ -1037,7 +1042,7 @@ class TcEngine : public Engine {
       }
       WRNN_CUDA_OK(cudaMemsetAsync(d_sync_, 0, 32, stream));                       // arrival counters (the abort flag is sticky)
       void* args[] = {&p};
-      const void* fn = progress ? kernel_live() : kernel(frames && !expand, p.n_seg > SMALL_TILE, nll != nullptr);
+      const void* fn = progress ? kernel_live(p.n_seg > SMALL_TILE) : kernel(frames && !expand, p.n_seg > SMALL_TILE, nll != nullptr);
       WRNN_CUDA_OK(cudaLaunchCooperativeKernel(fn, dim3(P), dim3(NT), args, SMEM_BYTES, stream));
       ++launches;
     }
