@@ -372,6 +372,51 @@ int wrnn_vocode_many_live_start(wrnn_t *h, const wrnn_vocode_batch *b, void *str
  * without touching the job. */
 int wrnn_vocode_many_live_poll(wrnn_t *h, int32_t wait_us, int64_t *n_ready);
 
+/* Live session: listeners that arrive at any time.  The session holds a persistent tile of `capacity` slots (1 to 64);
+ * each submitted utterance takes a free slot and is admitted into the RUNNING kernel at its next admission boundary
+ * (every 64 steps), then delivered as a wrnn_vocode_many_live utterance.  An idle session's kernel exits; the next
+ * submit relaunches it.
+ *
+ * Contract: a ticket's delivered waveform is bit-identical to wrnn_vocode_host with {mel, T, batched = 0, mu_law,
+ * philox_seed} on the same handle, whatever its slot, its admission step, the launch that served it and whatever else
+ * was in flight.  n_ready never decreases and a delivered sample is never rewritten.
+ *
+ * While a session is open every other entry point returns WRNN_E_BUSY (both live starts included; their polls refuse
+ * it); wrnn_destroy closes it.  Refused (WRNN_E_INVALID, with a message) before the handle is looked at: capacity
+ * outside 1..64, max_T < 21, null pointers, T < 21; then a null handle, a handle whose engine is not the persistent one
+ * or without an upsampler, max_T beyond 2^27 samples per utterance, T > max_T, any call but wrnn_live_open without an
+ * open session. */
+enum { WRNN_LIVE_RUNNING = 0, WRNN_LIVE_DONE = 1, WRNN_LIVE_CANCELLED = 2 };
+typedef struct {
+  int64_t ticket;
+  int64_t n_ready;    /* leading samples of the ticket's wav that are final */
+  int32_t state;      /* WRNN_LIVE_*: DONE / CANCELLED once, by the poll that releases the ticket's slot */
+  int32_t pad;
+} wrnn_live_ticket;
+
+/* Opens a session of `capacity` slots for utterances of up to max_T frames (mu_law: RAW head, as wrnn_vocode_job).
+ * Allocates a pinned, mapped buffer [progress words | mailboxes | capacity x (max_T - 1) * hop samples] and a device
+ * frame arena of `capacity` regions of max_T + 4 frames.  The kernel runs on `stream`. */
+int wrnn_live_open(wrnn_t *h, int32_t capacity, int64_t max_T, int32_t mu_law, void *stream);
+
+/* Submits one utterance (u->mel: host or device; u->wav: HOST, [(T - 1) * hop] float64, written by wrnn_live_poll) and
+ * returns its ticket (1, 2, ... in submission order).  The conditioning network runs into the slot's region on a side
+ * stream, on the SMs the kernel leaves free; the request is posted to the kernel once it is complete.  WRNN_E_BUSY when
+ * every slot holds an utterance (there is no host queue): poll until one is released. */
+int wrnn_live_submit(wrnn_t *h, const wrnn_utterance *u, int64_t *ticket);
+
+/* Cancels a ticket: its slot stops at the next boundary and is released by a later poll (state CANCELLED). */
+int wrnn_live_cancel(wrnn_t *h, int64_t ticket);
+
+/* Waits up to wait_us for progress, writes every newly final sample into its ticket's wav and reports in out[0 ..
+ * *n_out) the tickets whose slot was released since the last poll (state DONE or CANCELLED), then every ticket still
+ * held (state RUNNING).  max_out must be at least 2 * capacity.  Returns 1 while any ticket is held, 0 when none is,
+ * or a negative WRNN_E_* code (device errors as wrnn_check).  The wait is wrnn_vocode_live_poll's. */
+int wrnn_live_poll(wrnn_t *h, int32_t wait_us, wrnn_live_ticket *out, int32_t max_out, int32_t *n_out);
+
+/* Closes the session: cancels every ticket still held, waits for the kernel to exit and frees the session's buffers. */
+int wrnn_live_close(wrnn_t *h);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Scoring: how likely a given waveform is under the model, on the engine that generates it.  The loss the reference
  * trains with (train_wavernn.py:83), per sample, teacher-forced and reduced inside the kernel where the logits are:

@@ -25,7 +25,9 @@ EXPORTS = ("wrnn_abi_version", "wrnn_last_error", "wrnn_create", "wrnn_destroy",
            "wrnn_attach_upsampler", "wrnn_conditioning_frames", "wrnn_vocode", "wrnn_vocode_host",
            "wrnn_vocode_many", "wrnn_vocode_many_host", "wrnn_score", "wrnn_score_many", "wrnn_score_many_host",
            "wrnn_vocode_live_start", "wrnn_vocode_live_poll", "wrnn_vocode_many_live_start",
-           "wrnn_vocode_many_live_poll")
+           "wrnn_vocode_many_live_poll", "wrnn_live_open", "wrnn_live_submit", "wrnn_live_cancel", "wrnn_live_poll",
+           "wrnn_live_close")
+LIVE_RUNNING, LIVE_DONE, LIVE_CANCELLED = 0, 1, 2
 
 _fp = C.POINTER(C.c_float)
 
@@ -82,6 +84,10 @@ class WrnnUtterance(C.Structure):
 class WrnnVocodeBatch(C.Structure):
     _fields_ = [("utts", C.POINTER(WrnnUtterance)), ("n_utts", C.c_int32), ("batched", C.c_int32), ("target", C.c_int32),
                 ("overlap", C.c_int32), ("mu_law", C.c_int32)]
+
+
+class WrnnLiveTicket(C.Structure):
+    _fields_ = [("ticket", C.c_int64), ("n_ready", C.c_int64), ("state", C.c_int32), ("pad", C.c_int32)]
 
 
 class WrnnScoreUtt(C.Structure):
@@ -177,7 +183,25 @@ def load() -> C.CDLL:
     lib.wrnn_vocode_many_live_start.argtypes = [C.c_void_p, C.POINTER(WrnnVocodeBatch), C.c_void_p]
     lib.wrnn_vocode_many_live_poll.restype = C.c_int
     lib.wrnn_vocode_many_live_poll.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
+    lib.wrnn_live_open.restype = C.c_int
+    lib.wrnn_live_open.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_void_p]
+    lib.wrnn_live_submit.restype = C.c_int
+    lib.wrnn_live_submit.argtypes = [C.c_void_p, C.POINTER(WrnnUtterance), C.POINTER(C.c_int64)]
+    lib.wrnn_live_cancel.restype = C.c_int
+    lib.wrnn_live_cancel.argtypes = [C.c_void_p, C.c_int64]
+    lib.wrnn_live_poll.restype = C.c_int
+    lib.wrnn_live_poll.argtypes = [C.c_void_p, C.c_int32, C.POINTER(WrnnLiveTicket), C.c_int32, C.POINTER(C.c_int32)]
+    lib.wrnn_live_close.restype = C.c_int
+    lib.wrnn_live_close.argtypes = [C.c_void_p]
     # test hooks (not declared in the header)
+    lib.wrnn_debug_live_session_deliver.restype = C.c_int
+    lib.wrnn_debug_live_session_deliver.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                                    C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.wrnn_debug_live_tag.restype = C.c_uint32
+    lib.wrnn_debug_live_tag.argtypes = [C.c_int64]
+    lib.wrnn_debug_live_session_slot.restype = C.c_int
+    lib.wrnn_debug_live_session_slot.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.c_int32, C.c_uint32, C.c_uint32,
+                                                 C.c_uint64, C.c_int64, C.c_void_p]
     lib.wrnn_debug_live_many_deliver.restype = C.c_int
     lib.wrnn_debug_live_many_deliver.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
                                                  C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
@@ -400,6 +424,11 @@ class Engine:
             while rc == 1:                               # closed early: the job runs to its end, into `wavs`
                 rc = self.lib.wrnn_vocode_many_live_poll(self._h, 100000, n.ctypes.data)
 
+    def live_session(self, capacity: int, max_T: int, mu_law: bool = False):
+        """wrnn_live_open: a LiveSession of `capacity` slots (1 to 64) for mels of up to max_T frames, into whose running
+        kernel each submitted mel is admitted at the next boundary.  Use it as a context manager (close on exit)."""
+        return LiveSession(self, capacity, max_T, mu_law)
+
     # ---- scoring (wrnn_score / wrnn_score_many): the reference's training loss per sample, teacher-forced ----
     def score(self, *, L: int, n_seg: int, seg_len: int, seg_stride: int, x_force: int, nll: int, mels_up: int = 0, aux: int = 0,
               seg_first: int = 0, steps: int = 0, logits_out: int = 0, fold_row0: int = 0, fold_row_end: int = 0,
@@ -445,6 +474,72 @@ class Engine:
             self.close()
         except Exception:
             pass
+
+
+class LiveSession:
+    """wrnn_live_*: submit(mel, philox_seed) -> ticket at any time; poll() yields (ticket, slice) for each newly final
+    slice of a ticket's float64 waveform (views of one array per ticket; their concatenation is bit-identical to
+    vocode_host(mel, batched=False, mu_law=mu_law, philox_seed=philox_seed)); cancel(ticket); close().  `waves` maps
+    each ticket to its array, `states` to its last reported state (LIVE_*)."""
+
+    def __init__(self, engine: Engine, capacity: int, max_T: int, mu_law: bool = False):
+        self.engine, self.lib, self.capacity = engine, engine.lib, int(capacity)
+        self.hop = getattr(engine, "hop_length", 275)
+        _check(self.lib, self.lib.wrnn_live_open(engine._h, self.capacity, int(max_T), int(bool(mu_law)), None))
+        self.open = True
+        self.waves, self.states, self._mels, self._prev = {}, {}, {}, {}
+        self._out = (WrnnLiveTicket * (2 * self.capacity))()
+
+    def submit(self, mel, *, philox_seed: int) -> int:
+        """Submits mel (80, T) numpy; returns its ticket.  Raises EngineError(WRNN_E_BUSY) when every slot is held."""
+        import numpy as np
+        mel = np.ascontiguousarray(mel[0] if mel.ndim == 3 and mel.shape[0] == 1 else mel, dtype=np.float32)
+        T = mel.shape[-1]
+        wav = np.zeros(max(T - 1, 0) * self.hop, dtype=np.float64)
+        u = WrnnUtterance(mel.ctypes.data, int(T), int(philox_seed), wav.ctypes.data)
+        tk = C.c_int64(0)
+        _check(self.lib, self.lib.wrnn_live_submit(self.engine._h, C.byref(u), C.byref(tk)))
+        t = int(tk.value)
+        self.waves[t], self._mels[t], self._prev[t], self.states[t] = wav, mel, 0, LIVE_RUNNING
+        return t
+
+    def cancel(self, ticket: int):
+        _check(self.lib, self.lib.wrnn_live_cancel(self.engine._h, int(ticket)))
+
+    def poll_once(self, wait_us: int = 1000):
+        """One wrnn_live_poll: returns (rc, [(ticket, slice), ...]) for the slices that became final."""
+        n = C.c_int32(0)
+        rc = self.lib.wrnn_live_poll(self.engine._h, int(wait_us), self._out, len(self._out), C.byref(n))
+        if rc < 0:
+            _check(self.lib, rc)
+        got = []
+        for e in self._out[:n.value]:
+            t = int(e.ticket)
+            if int(e.n_ready) > self._prev[t]:
+                got.append((t, self.waves[t][self._prev[t]:int(e.n_ready)]))
+                self._prev[t] = int(e.n_ready)
+            self.states[t] = int(e.state)
+            if e.state != LIVE_RUNNING:
+                self._mels.pop(t, None)
+        return rc, got
+
+    def poll(self, wait_us: int = 1000):
+        """A generator of (ticket, slice) until no ticket is held."""
+        rc = 1
+        while rc == 1:
+            rc, got = self.poll_once(wait_us)
+            yield from got
+
+    def close(self):
+        if self.open:
+            self.open = False
+            _check(self.lib, self.lib.wrnn_live_close(self.engine._h))
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
 
 def _torch():

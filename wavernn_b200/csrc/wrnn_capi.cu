@@ -55,6 +55,10 @@ struct LiveJob {
 };
 
 int idle_or_busy(const wrnn_handle* h) {
+  if (h && h->session) {
+    set_error("a live session is open on this handle: wrnn_live_close it first");
+    return WRNN_E_BUSY;
+  }
   if (h && h->live_busy) {
     set_error(std::string("a live job is in flight on this handle: ") +
               (h->live->many ? "wrnn_vocode_many_live_poll" : "wrnn_vocode_live_poll") + " until it returns 0 or an error");
@@ -173,6 +177,7 @@ static int pick_engine(wrnn_t* h, const wrnn_job* job, Engine** out) {
 
 void wrnn_destroy(wrnn_t* h) {
   if (!h) return;
+  if (h->session) wrnn_live_close(h);                  // cancels every ticket and waits for the kernel
   if (h->live) {                                       // a live job still in flight finishes first
     if (h->live->done) {
       cudaSetDevice(h->engine->device);
@@ -239,7 +244,7 @@ int wrnn_score(wrnn_t* h, const wrnn_job* job, float* nll, void* stream) {
 
 int wrnn_check(wrnn_t* h) {
   if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
-  if (h->live_busy) return idle_or_busy(h);
+  if (h->live_busy || h->session) return idle_or_busy(h);
   return h->last->check();
 }
 
@@ -842,6 +847,7 @@ static int live_launch(wrnn_t* h, VocodeJob& v, bool many, bool mu_law, const st
 // the final samples of utterance i.
 static int live_poll(wrnn_t* h, int32_t wait_us, bool many, int64_t* n_ready) {
   if (!h || !h->engine || !n_ready) { set_error("null handle or n_ready"); return WRNN_E_INVALID; }
+  if (h->session) { set_error("a live session is open on this handle: poll it with wrnn_live_poll"); return WRNN_E_INVALID; }
   if (!h->live_busy) {
     set_error(many ? "no batch live job on this handle (wrnn_vocode_many_live_start)" : "no live job on this handle (wrnn_vocode_live_start)");
     return WRNN_E_INVALID;
@@ -1062,6 +1068,382 @@ int wrnn_debug_stream_plan(const wrnn_cfg* cfg, const wrnn_weights* w, uint8_t* 
     }
   }
   *blob_bytes = plan.blob.size(); *n_chunks = plan.prog.size();
+  return WRNN_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------------
+// wrnn_live_open .. wrnn_live_close: a live session.  Slot s of the persistent tile owns region s of the frame arena, row
+// s of the pinned sample block, progress word s and mailbox s.  The host picks a free slot, writes the utterance's
+// conditioning frames into its region on a side stream and, once they are complete, posts the request to the mailbox; CTA
+// 0 admits it at the next boundary (DESIGN §3.7).  A launch that has exited is relaunched with the posted requests
+// admitted at its step 0.
+// ---------------------------------------------------------------------------------------------------------------------
+namespace wrnn {
+struct LiveSession {
+  static constexpr int MAX_SLOTS = 64;
+  static constexpr size_t MAIL_OFF = MAX_SLOTS * sizeof(unsigned long long);
+  static constexpr size_t SAMPLES_OFF = 4096;     // [progress words | mailboxes | pad | samples [C][max_steps]]
+  static_assert(MAIL_OFF + MAX_SLOTS * sizeof(SesMail) <= SAMPLES_OFF, "pinned layout");
+  enum { FREE, PREP, POSTED };
+  struct Slot {
+    int state = FREE;
+    long long ticket = 0;
+    unsigned tag = 0;
+    unsigned long long seed = 0;
+    long long wave_len = 0, delivered = 0;
+    double* wav = nullptr;
+    bool cancelled = false;
+    cudaEvent_t ready = nullptr;     // the slot's conditioning frames are complete
+  };
+  int C = 0, hop = 0, n_classes = 0;
+  long long max_T = 0, max_steps = 0, tail_len = 0;
+  std::vector<double> mu, tail;      // the epilogue tables (mu empty without mu_law)
+  Engine* e = nullptr;
+  cudaStream_t st = nullptr, side = nullptr;
+  void* host = nullptr; void* dev = nullptr;         // pinned, mapped
+  void* d_ctl = nullptr;                             // [tab 2 x 64 | stop 2]
+  void* d_arena = nullptr;                           // [mel_frames C x (max_T + 4) | aux_frames C x (max_T + 4) | mel stage C x max_T]
+  float *mel_frames = nullptr, *aux_frames = nullptr, *mel_stage = nullptr;
+  const float* taps = nullptr;                       // the upsampler's [hop][5] tap table
+  size_t stage_pitch = 0;
+  cudaEvent_t done = nullptr;                        // recorded after the running launch
+  bool running = false;
+  std::vector<Slot> slots;
+  std::vector<SesEntry> tab;                         // host image of the table for a launch: [2][64], version -1 in buffer 1
+  long long next_ticket = 1;
+  std::vector<wrnn_live_ticket> released;            // tickets whose slot was released since the last poll
+  unsigned long long* progress() const { return static_cast<unsigned long long*>(host); }
+  SesMail* mail() const { return reinterpret_cast<SesMail*>(static_cast<char*>(host) + MAIL_OFF); }
+  const float* samples(int s) const {
+    return reinterpret_cast<const float*>(static_cast<const char*>(host) + SAMPLES_OFF) + (size_t)s * max_steps;
+  }
+  void release(Slot& sl) {
+    released.push_back(wrnn_live_ticket{sl.ticket, sl.delivered,
+                                        (!sl.cancelled && sl.delivered == sl.wave_len) ? WRNN_LIVE_DONE : WRNN_LIVE_CANCELLED, 0});
+    const cudaEvent_t ev = sl.ready;
+    sl = Slot();
+    sl.ready = ev;
+  }
+};
+
+// Delivers, per posted slot, the samples its occupant has published (words of an earlier occupant of the slot carry
+// another tag and are ignored) and releases the slots whose occupant CTA 0 retired.  Returns whether anything changed.
+static bool session_deliver(LiveSession& ss) {
+  bool more = false;
+  for (int s = 0; s < ss.C; ++s) {
+    LiveSession::Slot& sl = ss.slots[s];
+    if (sl.state != LiveSession::POSTED) continue;
+    const unsigned long long w = __atomic_load_n(ss.progress() + s, __ATOMIC_ACQUIRE);
+    if ((unsigned)(w >> 32) != sl.tag) continue;
+    const long long count = (long long)(w & (SES_RETIRED - 1u));
+    const long long ready = count < sl.wave_len ? count : sl.wave_len;
+    if (ready > sl.delivered && !sl.cancelled) {
+      live_epilogue(ss.samples(s), sl.delivered, ready, sl.wave_len, ss.tail_len, ss.mu.empty() ? nullptr : ss.mu.data(),
+                    ss.n_classes, ss.tail.data(), sl.wav);
+      sl.delivered = ready;
+      more = true;
+    }
+    if (w & SES_RETIRED) { ss.release(sl); more = true; }
+  }
+  return more;
+}
+
+// Posts the slots whose frames are complete, and relaunches the kernel when the last launch has exited and a posted
+// request was not admitted by it.
+static int session_pump(LiveSession& ss) {
+  if (ss.running) {
+    const cudaError_t q = cudaEventQuery(ss.done);
+    if (q == cudaSuccess) {
+      ss.running = false;
+      session_deliver(ss);                             // the launch's last words
+      const int rc = ss.e->check();
+      if (rc != WRNN_OK) return rc;
+    } else if (q != cudaErrorNotReady) {
+      set_error(std::string("live session: ") + cudaGetErrorString(q));
+      return WRNN_E_CUDA;
+    }
+  }
+  for (int s = 0; s < ss.C; ++s) {
+    LiveSession::Slot& sl = ss.slots[s];
+    if (sl.state != LiveSession::PREP) continue;
+    const cudaError_t q = cudaEventQuery(sl.ready);
+    if (q == cudaErrorNotReady) continue;
+    if (q != cudaSuccess) { set_error(std::string("live session: conditioning: ") + cudaGetErrorString(q)); return WRNN_E_CUDA; }
+    if (sl.cancelled) { ss.release(sl); continue; }
+    SesMail& m = ss.mail()[s];
+    m.seed = sl.seed;
+    m.steps = sl.wave_len;
+    __atomic_store_n(&m.req, (unsigned long long)sl.tag, __ATOMIC_RELEASE);   // the body before the tag
+    sl.state = LiveSession::POSTED;
+  }
+  if (ss.running) return WRNN_OK;
+  // No launch runs: every slot it admitted is retired and released.  A posted request it did not admit is admitted at
+  // step 0 of the next launch (version -1 of the table), or withdrawn if cancelled.
+  bool launch = false;
+  for (int s = 0; s < LiveSession::MAX_SLOTS; ++s) ss.tab[LiveSession::MAX_SLOTS + s] = SesEntry{0, 0, 0ull};
+  for (int s = 0; s < ss.C; ++s) {
+    LiveSession::Slot& sl = ss.slots[s];
+    if (sl.state != LiveSession::POSTED) continue;
+    const unsigned long long w = __atomic_load_n(ss.progress() + s, __ATOMIC_ACQUIRE);
+    if ((unsigned)(w >> 32) == sl.tag) {
+      set_error("live session: a launch exited with slot " + std::to_string(s) + " still held");
+      return WRNN_E_CUDA;
+    }
+    if (sl.cancelled) {
+      __atomic_store_n(&ss.mail()[s].req, w >> 32, __ATOMIC_RELEASE);
+      ss.release(sl);
+      continue;
+    }
+    ss.tab[LiveSession::MAX_SLOTS + s] = SesEntry{0, (int)sl.wave_len, sl.seed};
+    __atomic_store_n(ss.progress() + s, (unsigned long long)sl.tag << 32, __ATOMIC_RELEASE);
+    launch = true;
+  }
+  if (!launch) return WRNN_OK;
+  WRNN_CUDA_OK(cudaSetDevice(ss.e->device));
+  WRNN_CUDA_OK(cudaMemcpyAsync(ss.d_ctl, ss.tab.data(), ss.tab.size() * sizeof(SesEntry), cudaMemcpyHostToDevice, ss.st));
+  wrnn_job j;
+  std::memset(&j, 0, sizeof(j));
+  j.n_seg = ss.C; j.seg_len = (int32_t)ss.max_steps; j.seg_stride = (ss.max_T + 4) * ss.hop; j.L = j.seg_stride * ss.C;
+  j.mel_frames = ss.mel_frames; j.aux_frames = ss.aux_frames; j.up_taps = ss.taps; j.hop = ss.hop;
+  j.out = reinterpret_cast<float*>(static_cast<char*>(ss.dev) + LiveSession::SAMPLES_OFF);
+  SesCtl c;
+  c.tab = static_cast<SesEntry*>(ss.d_ctl);
+  c.stop = reinterpret_cast<int*>(c.tab + 2 * LiveSession::MAX_SLOTS);
+  c.mail = reinterpret_cast<const SesMail*>(static_cast<char*>(ss.dev) + LiveSession::MAIL_OFF);
+  c.progress = static_cast<unsigned long long*>(ss.dev);
+  int rc = ss.e->generate_session(j, ss.st, c);
+  if (rc != WRNN_OK) return rc;
+  WRNN_CUDA_OK(cudaEventRecord(ss.done, ss.st));
+  ss.running = true;
+  return WRNN_OK;
+}
+
+static void session_free(LiveSession* ss) {
+  if (ss->done) { cudaEventSynchronize(ss->done); cudaEventDestroy(ss->done); }
+  if (ss->side) { cudaStreamSynchronize(ss->side); cudaStreamDestroy(ss->side); }
+  for (auto& sl : ss->slots) if (sl.ready) cudaEventDestroy(sl.ready);
+  if (ss->host) cudaFreeHost(ss->host);
+  cudaFree(ss->d_ctl);
+  cudaFree(ss->d_arena);
+  delete ss;
+}
+}  // namespace wrnn
+
+extern "C" {
+
+int wrnn_live_open(wrnn_t* h, int32_t capacity, int64_t max_T, int32_t mu_law, void* stream) {
+  if (capacity < 1 || capacity > LiveSession::MAX_SLOTS) {
+    set_error("a live session holds 1 to 64 slots: one persistent tile holds 64 folds"); return WRNN_E_INVALID;
+  }
+  if (max_T < 21) { set_error("max_T must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples"); return WRNN_E_INVALID; }
+  if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  if (!h->upsampler) { set_error("no upsampler attached (wrnn_attach_upsampler)"); return WRNN_E_INVALID; }
+  if (h->engine->live_refusal()) { set_error(h->engine->live_refusal()); return WRNN_E_INVALID; }
+  const int hop = h->upsampler->hop;
+  if ((max_T - 1) * hop > SES_MAX_STEPS || (max_T + 4) * hop * capacity >= (1ll << 31)) {
+    set_error("max_T too large: an utterance is at most 2^27 samples and the session's frame arena below 2^31 rows"); return WRNN_E_INVALID;
+  }
+  LiveSession* ss = new (std::nothrow) LiveSession();
+  if (!ss) { set_error("out of host memory"); return WRNN_E_INVALID; }
+  ss->C = capacity; ss->hop = hop; ss->max_T = max_T; ss->max_steps = (max_T - 1) * hop;
+  ss->n_classes = h->engine->cfg.n_classes; ss->tail_len = 20ll * hop;
+  ss->e = h->engine; ss->st = static_cast<cudaStream_t>(stream); ss->taps = h->upsampler->d_taps;
+  ss->slots.resize(capacity);
+  ss->tab.assign(2 * LiveSession::MAX_SLOTS, SesEntry{0, 0, 0ull});
+  std::vector<double> fi, fo;
+  cond::epilogue_tables(0, mu_law && h->engine->cfg.mode == WRNN_MODE_RAW, ss->n_classes, hop, fi, fo, ss->mu, ss->tail);
+  auto fail = [&](int code) { session_free(ss); return code; };
+#define SES_OK(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { set_error(std::string(#expr) + " failed: " + cudaGetErrorString(_e)); return fail(WRNN_E_CUDA); } } while (0)
+  SES_OK(cudaSetDevice(h->engine->device));
+  const size_t host_bytes = LiveSession::SAMPLES_OFF + (size_t)capacity * ss->max_steps * sizeof(float);
+  SES_OK(cudaHostAlloc(&ss->host, host_bytes, cudaHostAllocMapped));
+  SES_OK(cudaHostGetDevicePointer(&ss->dev, ss->host, 0));
+  std::memset(ss->host, 0, LiveSession::SAMPLES_OFF);
+  SES_OK(cudaMalloc(&ss->d_ctl, 2 * LiveSession::MAX_SLOTS * sizeof(SesEntry) + 64));
+  const size_t rf = (size_t)(max_T + 4) * capacity;
+  ss->stage_pitch = align_floats((size_t)max_T * FEAT);
+  const size_t n_mf = align_floats(rf * FEAT), n_af = align_floats(rf * cond::CD);
+  SES_OK(cudaMalloc(&ss->d_arena, (n_mf + n_af + ss->stage_pitch * capacity) * sizeof(float)));
+  ss->mel_frames = static_cast<float*>(ss->d_arena);
+  ss->aux_frames = ss->mel_frames + n_mf;
+  ss->mel_stage = ss->aux_frames + n_af;
+  SES_OK(cudaStreamCreateWithFlags(&ss->side, cudaStreamNonBlocking));
+  SES_OK(cudaEventCreateWithFlags(&ss->done, cudaEventDisableTiming));
+  for (auto& sl : ss->slots) SES_OK(cudaEventCreateWithFlags(&sl.ready, cudaEventDisableTiming));
+#undef SES_OK
+  h->session = ss;
+  return WRNN_OK;
+}
+
+int wrnn_live_submit(wrnn_t* h, const wrnn_utterance* u, int64_t* ticket) {
+  if (!u || !ticket) { set_error("null utterance or ticket"); return WRNN_E_INVALID; }
+  if (!u->mel || !u->wav) { set_error("mel and wav are required"); return WRNN_E_INVALID; }
+  if (u->T < 21) { set_error("T must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples"); return WRNN_E_INVALID; }
+  if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
+  if (!h->session) { set_error("no live session is open on this handle (wrnn_live_open)"); return WRNN_E_INVALID; }
+  LiveSession& ss = *h->session;
+  if (u->T > ss.max_T) { set_error("T exceeds the session's max_T (" + std::to_string(ss.max_T) + ")"); return WRNN_E_INVALID; }
+  int rc = session_pump(ss);                           // releases what has finished, so that its slot can be reused
+  if (rc != WRNN_OK) return rc;
+  session_deliver(ss);
+  int s = 0;
+  while (s < ss.C && ss.slots[s].state != LiveSession::FREE) ++s;
+  if (s == ss.C) {
+    set_error("all " + std::to_string(ss.C) + " slots of the live session hold an utterance: poll until one is released");
+    return WRNN_E_BUSY;
+  }
+  WRNN_CUDA_OK(cudaSetDevice(ss.e->device));
+  float* stage = ss.mel_stage + (size_t)s * ss.stage_pitch;
+  const size_t frame0 = (size_t)s * (ss.max_T + 4);
+  WRNN_CUDA_OK(cudaMemcpyAsync(stage, u->mel, (size_t)u->T * FEAT * sizeof(float), cudaMemcpyDefault, ss.side));
+  if ((rc = conditioning_frames(*h->upsampler, stage, u->T, ss.mel_frames + frame0 * FEAT, ss.aux_frames + frame0 * cond::CD,
+                                nullptr, ss.side)) != WRNN_OK)
+    return rc;
+  LiveSession::Slot& sl = ss.slots[s];
+  WRNN_CUDA_OK(cudaEventRecord(sl.ready, ss.side));
+  sl.state = LiveSession::PREP;
+  sl.ticket = ss.next_ticket++;
+  sl.tag = ses_tag(sl.ticket);
+  sl.seed = u->philox_seed;
+  sl.wave_len = (u->T - 1) * ss.hop;
+  sl.delivered = 0;
+  sl.wav = u->wav;
+  sl.cancelled = false;
+  *ticket = sl.ticket;
+  return session_pump(ss);
+}
+
+int wrnn_live_cancel(wrnn_t* h, int64_t ticket) {
+  if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
+  if (!h->session) { set_error("no live session is open on this handle (wrnn_live_open)"); return WRNN_E_INVALID; }
+  LiveSession& ss = *h->session;
+  for (int s = 0; s < ss.C; ++s) {
+    LiveSession::Slot& sl = ss.slots[s];
+    if (sl.state == LiveSession::FREE || sl.ticket != ticket) continue;
+    if (!sl.cancelled) {
+      sl.cancelled = true;
+      if (sl.state == LiveSession::POSTED) __atomic_store_n(&ss.mail()[s].cancel, (unsigned long long)sl.tag, __ATOMIC_RELEASE);
+    }
+    return WRNN_OK;
+  }
+  set_error("ticket " + std::to_string(ticket) + " is not in flight in this session");
+  return WRNN_E_INVALID;
+}
+
+int wrnn_live_poll(wrnn_t* h, int32_t wait_us, wrnn_live_ticket* out, int32_t max_out, int32_t* n_out) {
+  if (!out || !n_out) { set_error("null out or n_out"); return WRNN_E_INVALID; }
+  if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
+  if (!h->session) { set_error("no live session is open on this handle (wrnn_live_open)"); return WRNN_E_INVALID; }
+  LiveSession& ss = *h->session;
+  if (max_out < 2 * ss.C) { set_error("max_out must be at least twice the session's capacity"); return WRNN_E_INVALID; }
+  *n_out = 0;
+  const auto t0 = std::chrono::steady_clock::now();
+  const auto wait = std::chrono::microseconds(wait_us > 0 ? wait_us : 0);
+  for (;;) {
+    int rc = session_pump(ss);
+    if (rc != WRNN_OK) return rc;
+    bool more = session_deliver(ss) || !ss.released.empty();
+    const auto left = wait - (std::chrono::steady_clock::now() - t0);
+    if (more || left <= std::chrono::microseconds(0)) break;
+    std::this_thread::sleep_for(std::min<std::chrono::steady_clock::duration>(left, std::chrono::microseconds(100)));
+  }
+  // released tickets first, then every ticket still held (at most C)
+  int n = 0, held = 0;
+  size_t k = 0;
+  for (; k < ss.released.size() && n < max_out - ss.C; ++k) out[n++] = ss.released[k];
+  ss.released.erase(ss.released.begin(), ss.released.begin() + k);   // the rest: next poll
+  for (const auto& sl : ss.slots) {
+    if (sl.state == LiveSession::FREE) continue;
+    ++held;
+    out[n++] = wrnn_live_ticket{sl.ticket, sl.delivered, WRNN_LIVE_RUNNING, 0};
+  }
+  *n_out = n;
+  return held > 0 ? 1 : 0;
+}
+
+int wrnn_live_close(wrnn_t* h) {
+  if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
+  if (!h->session) { set_error("no live session is open on this handle (wrnn_live_open)"); return WRNN_E_INVALID; }
+  LiveSession* ss = h->session;
+  for (int s = 0; s < ss->C; ++s) {
+    LiveSession::Slot& sl = ss->slots[s];
+    if (sl.state != LiveSession::FREE && !sl.cancelled) wrnn_live_cancel(h, sl.ticket);
+  }
+  int rc = WRNN_OK;
+  for (;;) {                                           // the launch stops once every cancelled slot is retired
+    if ((rc = session_pump(*ss)) != WRNN_OK) break;
+    session_deliver(*ss);
+    bool held = false;
+    for (const auto& sl : ss->slots) held = held || sl.state != LiveSession::FREE;
+    if (!held && !ss->running) break;
+    std::this_thread::sleep_for(std::chrono::microseconds(100));
+  }
+  h->session = nullptr;
+  session_free(ss);
+  return rc;
+}
+
+// Test hook (CPU-only, no device needed): one delivery of wrnn_live_poll on a host buffer laid out as the session's
+// pinned one.  Slot s holds ticket[s] (0: free) of T[s] frames, whose samples are x [C][max_steps], published word
+// progress[s]; delivered[s] holds what earlier polls delivered and receives what this one did, released[s] whether the
+// slot was released; wav is the concatenation of the held tickets' waveforms.  Checked in tests/test_live_session_abi.py.
+int wrnn_debug_live_session_deliver(const float* x, int64_t max_steps, const uint64_t* progress, int32_t C,
+                                    const int64_t* ticket, const int64_t* T, int32_t hop, int32_t mu_law, int32_t n_classes,
+                                    int64_t* delivered, int32_t* released, double* wav) {
+  if (!x || !progress || !ticket || !T || !delivered || !released || !wav || max_steps <= 0 || hop <= 0 || C < 1 ||
+      C > LiveSession::MAX_SLOTS || (mu_law && n_classes < 2)) {
+    set_error("bad argument"); return WRNN_E_INVALID;
+  }
+  for (int s = 0; s < C; ++s)
+    if (ticket[s] && (T[s] < 21 || (T[s] - 1) * hop > max_steps || delivered[s] < 0 || delivered[s] > (T[s] - 1) * hop)) {
+      set_error("bad argument"); return WRNN_E_INVALID;
+    }
+  std::vector<unsigned char> buf(LiveSession::SAMPLES_OFF + (size_t)C * max_steps * sizeof(float));
+  std::memcpy(buf.data(), progress, (size_t)C * sizeof(uint64_t));
+  std::memcpy(buf.data() + LiveSession::SAMPLES_OFF, x, (size_t)C * max_steps * sizeof(float));
+  LiveSession ss;
+  ss.host = buf.data();
+  ss.C = C; ss.hop = hop; ss.max_steps = max_steps; ss.tail_len = 20ll * hop; ss.n_classes = n_classes;
+  std::vector<double> fi, fo;
+  cond::epilogue_tables(0, mu_law != 0, n_classes, hop, fi, fo, ss.mu, ss.tail);
+  ss.slots.resize(C);
+  double* w = wav;
+  for (int s = 0; s < C; ++s) {
+    if (!ticket[s]) continue;
+    LiveSession::Slot& sl = ss.slots[s];
+    sl.state = LiveSession::POSTED; sl.ticket = ticket[s]; sl.tag = ses_tag(ticket[s]);
+    sl.wave_len = (T[s] - 1) * hop; sl.delivered = delivered[s]; sl.wav = w;
+    w += sl.wave_len;
+  }
+  session_deliver(ss);
+  for (int s = 0; s < C; ++s) {
+    released[s] = 0;
+    if (!ticket[s]) continue;
+    for (const auto& r : ss.released) if (r.ticket == ticket[s]) { released[s] = 1; delivered[s] = r.n_ready; }
+    if (!released[s]) delivered[s] = ss.slots[s].delivered;
+  }
+  ss.host = nullptr;
+  return WRNN_OK;
+}
+
+// Test hook (CPU-only): a ticket's 32-bit tag, and CTA 0's decision for one slot at boundary b (the functions the kernel
+// runs).  state = {tag, a, e, retired}; words[0] / words[1]: the retirement and admission words published (0: none).
+uint32_t wrnn_debug_live_tag(int64_t ticket) { return ses_tag(ticket); }
+int wrnn_debug_live_session_slot(int64_t* state, uint64_t* seed, int32_t b, uint32_t req_tag, uint32_t cancel_tag,
+                                 uint64_t req_seed, int64_t req_steps, uint64_t* words) {
+  if (!state || !seed || !words || b < 0 || b % SES_PERIOD || req_steps < 1 || req_steps > SES_MAX_STEPS) {
+    set_error("bad argument"); return WRNN_E_INVALID;
+  }
+  SesSlot s{(unsigned)state[0], (int)state[1], (int)state[2], *seed, state[3] != 0};
+  words[0] = ses_retire_cancel(s, b, cancel_tag);
+  words[1] = 0;
+  if (ses_admits(s, b, req_tag)) words[1] = ses_admit(s, b, req_tag, req_seed, req_steps);
+  state[0] = s.tag; state[1] = s.a; state[2] = s.e; state[3] = s.retired ? 1 : 0;
+  *seed = s.seed;
   return WRNN_OK;
 }
 

@@ -509,7 +509,7 @@ extern "C" {
 
 int wrnn_attach_upsampler(wrnn_t* h, const wrnn_upsample_cfg* cfg, const wrnn_tensor* t, int32_t n) {
   if (!h || !h->engine || !cfg) { set_error("null handle or cfg"); return WRNN_E_INVALID; }
-  if (h->live_busy) return idle_or_busy(h);
+  if (h->live_busy || h->session) return idle_or_busy(h);
   WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
   cond::HostUpsampler hu;
   int rc = cond::build_host_upsampler(*cfg, t, n, false, hu);
@@ -524,7 +524,7 @@ int wrnn_attach_upsampler(wrnn_t* h, const wrnn_upsample_cfg* cfg, const wrnn_te
 int wrnn_conditioning_frames(wrnn_t* h, const float* mel, int64_t T, float* mel_frames, float* aux_frames, float* up_taps,
                              void* stream) {
   if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
-  if (h->live_busy) return idle_or_busy(h);
+  if (h->live_busy || h->session) return idle_or_busy(h);
   if (!h->upsampler) { set_error("no upsampler attached (wrnn_attach_upsampler)"); return WRNN_E_INVALID; }
   if (!mel || !mel_frames || !aux_frames || T <= 0 || T >= (1ll << 31)) {
     set_error("wrnn_conditioning_frames: bad argument"); return WRNN_E_INVALID;

@@ -29,6 +29,60 @@ inline int grid_stride_blocks(long long blocks) {
   return (int)(blocks < cap ? blocks : cap);
 }
 
+// ---- live session (wrnn_live_open / _submit / _cancel / _poll / _close; DESIGN §3.7) ------------------------------------
+// A session launch runs an open-ended tile of C slots.  Slot f's utterance runs from its admission step a to its end step
+// e (global steps of the launch), at local step t - a.  Admissions, cancellations and the launch's stop are decided by
+// CTA 0 at boundaries b = k * SES_PERIOD and take effect at the next boundary.
+constexpr int SES_PERIOD = 64;
+constexpr int SES_DRAIN = 4;                        // a slot is retired at the first boundary >= e + SES_DRAIN (staging runs <= 3 steps ahead)
+constexpr int SES_ADMIT_LIMIT = 1 << 27;            // no admission at a boundary from here on: every step index stays below 2^28
+constexpr long long SES_MAX_STEPS = 1ll << 27;      // samples of one utterance: (T - 1) * hop <= 2^27
+constexpr unsigned SES_RETIRED = 1u << 31;          // progress word: (tag << 32) | [retired bit] | samples stored
+// Slot table entry (device, [2 versions][64]): version k is written at boundary k * SES_PERIOD.
+struct SesEntry {
+  int a, e;
+  unsigned long long seed;
+};
+// One slot's mailbox (mapped host memory, written by the host only): the tag of the latest request and of the latest
+// cancellation, and the request's Philox seed and step count (written before `req`).
+struct SesMail {
+  unsigned long long req, cancel, seed;
+  long long steps;
+};
+// A ticket's 32-bit tag in the progress word and the mailbox: never 0 (the tag of a slot that never held a request).
+inline unsigned ses_tag(long long ticket) { return (unsigned)((unsigned long long)(ticket - 1) % 0xffffffffull) + 1u; }
+// CTA 0's state of one slot and its decisions at boundary b, shared by the kernel and the CPU test hook.
+struct SesSlot {
+  unsigned tag;                  // the occupant's (or last occupant's) ticket tag
+  int a, e;
+  unsigned long long seed;
+  bool retired;
+};
+// Retirement (returns the progress word to publish, or 0) and cancellation at boundary b.
+__host__ __device__ inline unsigned long long ses_retire_cancel(SesSlot& s, int b, unsigned cancel_tag) {
+  unsigned long long word = 0;
+  if (!s.retired && s.e + SES_DRAIN <= b) {
+    s.retired = true;
+    word = ((unsigned long long)s.tag << 32) | SES_RETIRED | (unsigned)(s.e - s.a);
+  }
+  if (!s.retired && cancel_tag == s.tag && s.e > b + SES_PERIOD) s.e = b + SES_PERIOD;
+  return word;
+}
+__host__ __device__ inline bool ses_admits(const SesSlot& s, int b, unsigned req_tag) {
+  return s.retired && req_tag != s.tag && b < SES_ADMIT_LIMIT;
+}
+// Admission at boundary b: the utterance runs steps [b + SES_PERIOD, + steps).  Returns the progress word to publish.
+__host__ __device__ inline unsigned long long ses_admit(SesSlot& s, int b, unsigned req_tag, unsigned long long seed, long long steps) {
+  s.tag = req_tag; s.a = b + SES_PERIOD; s.e = s.a + (int)steps; s.seed = seed; s.retired = false;
+  return (unsigned long long)req_tag << 32;
+}
+struct SesCtl {
+  SesEntry* tab;                 // [2][64] (device)
+  int* stop;                     // [2]: the step at which each version stops the launch, or INT_MAX (device)
+  const SesMail* mail;           // [64] (device alias of mapped host memory)
+  unsigned long long* progress;  // [64] (device alias of mapped host memory)
+};
+
 class Engine {
  public:
   virtual ~Engine() {}
@@ -45,6 +99,13 @@ class Engine {
   virtual const char* live_refusal() const { return "live vocoding runs on the persistent engine only"; }
   virtual int generate_live(const wrnn_job& job, cudaStream_t stream, const FoldKey* keys, unsigned long long* progress) {
     (void)job; (void)stream; (void)keys; (void)progress;
+    set_error(live_refusal());
+    return WRNN_E_INVALID;
+  }
+  // One launch of a live session (same refusal): job.n_seg slots, slot f's conditioning rows from f * job.seg_stride of the
+  // frame tensors, its samples at job.out + f * job.seg_len (mapped host memory).
+  virtual int generate_session(const wrnn_job& job, cudaStream_t stream, const SesCtl& c) {
+    (void)job; (void)stream; (void)c;
     set_error(live_refusal());
     return WRNN_E_INVALID;
   }
@@ -82,6 +143,7 @@ int epilogue_launch(const float* samples, int seg_len, long long seg_stride, int
 struct Upsampler;                                // conditioning network on the device (wrnn_cond.h)
 void destroy_upsampler(Upsampler* u);
 struct LiveJob;                                  // a live job and its pinned buffer (wrnn_capi.cu)
+struct LiveSession;                              // a live session, its buffers and its slots (wrnn_capi.cu)
 
 }  // namespace wrnn
 
@@ -102,6 +164,8 @@ struct wrnn_handle {
   // host buffer
   wrnn::LiveJob* live = nullptr;
   bool live_busy = false;
+  // wrnn_live_open .. wrnn_live_close: the open live session (every other entry point is busy while it is open)
+  wrnn::LiveSession* session = nullptr;
 };
 
 namespace wrnn {

@@ -93,6 +93,9 @@ constexpr int OFF_ACC = OFF_VEC + NVEC * 4;
 constexpr int OFF_BAR = OFF_ACC + AC_COLS * ACP * 4;      // 3 mbarriers
 constexpr int SMEM_BYTES = OFF_BAR + 64;
 static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
+constexpr int OFF_SES = SMEM_BYTES;                       // SES: the staging's window (a, e) of each slot
+constexpr int SMEM_SES = OFF_SES + MT * 8;
+static_assert(SMEM_SES <= 227 * 1024, "shared memory budget");
 
 struct TcParams {
   const unsigned char* blob;
@@ -113,6 +116,7 @@ struct TcParams {
   long long* prof;           // cycle counters of CTA 0 (fold thread 0: [0..4], driver lane 0: [5..7])
   float* nll;                // scoring: [steps, n_total] loss of target x_force[t] (job-wide; out is not written)
   unsigned long long* progress;   // LIVE: [n_total] samples of each fold stored so far (mapped host memory, system-scope release)
+  SesEntry* ses_tab; int* ses_stop; const SesMail* ses_mail;   // SES: see SesCtl
 };
 
 // ------------------------------------------------------------------------------------------
@@ -162,10 +166,34 @@ __device__ __forceinline__ void live_publish(unsigned long long* progress, int t
   if ((t + 1) % LIVE_PERIOD == 0 || t + 1 == steps)
     asm volatile("st.release.sys.u64 [%0], %1;" :: "l"(progress), "l"((unsigned long long)(t + 1)) : "memory");
 }
+// SES (wrnn_live_*): a LIVE tile whose slots take utterances while it runs (DESIGN §3.7).  Slot f's occupant runs global
+// steps [a, e) as its local steps t - a; its progress word carries its tag beside the count.
+__device__ __forceinline__ void st_release_sys_u64(unsigned long long* p, unsigned long long v) {
+  asm volatile("st.release.sys.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ unsigned long long ld_volatile_u64(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("ld.volatile.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+// CTA 0's fold warps: a named barrier that also returns whether any of the 128 threads passed `pred`
+__device__ __forceinline__ bool named_bar_or(int id, int nthreads, bool pred) {
+  int r;
+  asm volatile("{ .reg .pred p, q; setp.ne.s32 p, %1, 0; bar.red.or.pred q, %2, %3, p; selp.s32 %0, 1, 0, q; }"
+               : "=r"(r) : "r"((int)pred), "r"(id), "r"(nthreads) : "memory");
+  return r != 0;
+}
+__device__ __forceinline__ SesEntry ld_ses_entry(const SesEntry* e) {   // L2, never a stale L1 line of an earlier version
+  const int2 w = __ldcg(reinterpret_cast<const int2*>(e));
+  return SesEntry{w.x, w.y, __ldcg(&e->seed)};
+}
+__device__ __forceinline__ void ses_publish(unsigned long long* progress, unsigned tag, int ts, int steps) {
+  if ((ts + 1) % LIVE_PERIOD == 0 || ts + 1 == steps) st_release_sys_u64(progress, ((unsigned long long)tag << 32) | (unsigned)(ts + 1));
+}
 // SCORE (wrnn_score): the loss of target x_force[t] in the sampler's place, written by CTA 0; no draws are made.  MoL:
 // from the replicated logits.  RAW: the fifth exchange carries, in the candidate's 8 B, each CTA's log-sum-exp of its 4
 // classes and the target's logit from the CTA that owns the target class (-inf from the others).
-template <int FMT, bool FRAMES, bool RAW, bool BIG, bool SCORE, bool LIVE>
+template <int FMT, bool FRAMES, bool RAW, bool BIG, bool SCORE, bool LIVE, bool SES = false>
 __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
   extern __shared__ __align__(1024) unsigned char smem[];
   const float* fv = reinterpret_cast<const float*>(smem + OFF_VEC);
@@ -176,7 +204,8 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
   const uint32_t bar_mma = smem_u32(&bars[0]), bar_q = smem_u32(&bars[1]), bar_g = smem_u32(&bars[2]);
 
   const int cta = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int B = p.n_seg, S = p.steps, u0 = cta * U;
+  const int B = p.n_seg, u0 = cta * U;
+  int S = p.steps;                                     // SES: open-ended until a version of the slot table sets the stop
   const int n_groups = (B + 7) / 8;                    // real 8-row groups of the A images
   const uint32_t img_bytes = (uint32_t)n_groups * SBO_H;
   const size_t xch_stride = (size_t)2 * img_bytes;     // per vector: two parities
@@ -271,10 +300,58 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
     float w2h_a[3 * UT], f1h1_a[UT];
 #pragma unroll
     for (int i = 0; i < 3 * UT; ++i) w2h_a[i] = 0.f;
+    // SES: this fold's slot as the table version in use has it (version -1 = buffer 1, written by the host), and CTA 0's
+    // decision state of it, held by the thread that stores the slot's samples.  The mailbox words are read one step
+    // before each boundary, so that their PCIe round trip overlaps the fc3 wait.
+    int sa = 0, se = 0;
+    unsigned long long sseed = 0;
+    const bool decider = SES && cta == 0 && owns_fold && slot == 0;
+    SesSlot ds{0u, 0, 0, 0ull, true};
+    unsigned long long m_req = 0, m_can = 0;
+    if constexpr (SES) {
+      if (owns_fold) { const SesEntry en = ld_ses_entry(p.ses_tab + MT + fold); sa = en.a; se = en.e; sseed = en.seed; }
+      if (decider) {
+        ds = SesSlot{(unsigned)(ld_volatile_u64(p.progress + fold) >> 32), sa, se, sseed, se <= 0};
+        m_req = ld_volatile_u64(&p.ses_mail[fold].req); m_can = ld_volatile_u64(&p.ses_mail[fold].cancel);
+      }
+    }
     read_phase_a(0);
 
     for (int t = 0; t < S; ++t) {
       const int par = t & 1;
+      if constexpr (SES) {
+        if ((t & (SES_PERIOD - 1)) == 0) {
+          // boundary: CTA 0 retires, cancels and admits, writes version t / SES_PERIOD of the table and decides whether
+          // the launch stops at the next boundary.  signal(0) below releases all of it with the h1' exchange.
+          bool busy = false;
+          if (decider) {
+            const unsigned long long rw = ses_retire_cancel(ds, t, (unsigned)m_can);
+            if (rw) st_release_sys_u64(p.progress + fold, rw);
+            if (ses_admits(ds, t, (unsigned)m_req)) {
+              asm volatile("fence.acq_rel.sys;" ::: "memory");      // the request's body after its tag
+              const unsigned long long seed = ld_volatile_u64(&p.ses_mail[fold].seed);
+              const long long steps = (long long)ld_volatile_u64(reinterpret_cast<const unsigned long long*>(&p.ses_mail[fold].steps));
+              st_release_sys_u64(p.progress + fold, ses_admit(ds, t, (unsigned)m_req, seed, steps));
+            }
+            busy = !ds.retired;
+            const SesEntry en{ds.a, ds.e, ds.seed};
+            p.ses_tab[((t / SES_PERIOD) & 1) * MT + fold] = en;
+          }
+          if (cta == 0) {
+            busy = named_bar_or(1, 128, busy);
+            if (tid == 0) p.ses_stop[(t / SES_PERIOD) & 1] = busy ? 0x7fffffff : t + SES_PERIOD;
+          }
+        }
+        if (t == sa) {                                    // admission: the utterance starts from zero state
+          x = 0.f;
+#pragma unroll
+          for (int i = 0; i < UT; ++i) { h1[i] = 0.f; h2[i] = 0.f; }
+        }
+      }
+      // the fold's own step (SES: local to its utterance) and whether it has one at this step
+      const int ts = SES ? t - sa : t;
+      const bool warm = SES ? ts > 0 : t > 0;
+      const bool on = !SES || (t >= sa && t < se);
       unsigned char* img_h1 = p.xch + 0 * xch_stride + (size_t)par * img_bytes;
       unsigned char* img_h2 = p.xch + 1 * xch_stride + (size_t)par * img_bytes;
       unsigned char* img_y1 = p.xch + 2 * xch_stride + (size_t)par * img_bytes;
@@ -295,8 +372,8 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
           for (int q = 0; q < 8 * UT; ++q) pre[q] = pre_a[q] + (qk_r[q] + x * vq_r[q]);
 #pragma unroll
           for (int i = 0; i < UT; ++i) {                  // gh_a: W1h h1 (step t-1, phase B)
-            const float ghr = (t > 0 ? gh_a[i] : 0.f) + b1h_r[i], ghz = (t > 0 ? gh_a[UT + i] : 0.f) + b1h_r[UT + i],
-                        ghn = (t > 0 ? gh_a[2 * UT + i] : 0.f) + b1h_r[2 * UT + i];
+            const float ghr = (warm ? gh_a[i] : 0.f) + b1h_r[i], ghz = (warm ? gh_a[UT + i] : 0.f) + b1h_r[UT + i],
+                        ghn = (warm ? gh_a[2 * UT + i] : 0.f) + b1h_r[2 * UT + i];
             h1[i] = gru_unit_fast(pre[i], pre[UT + i], pre[2 * UT + i], ghr, ghz, ghn, h1[i]);
           }
           publish(img_h1, h1);
@@ -318,8 +395,8 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
 #pragma unroll
                 for (int i = 0; i < UT; ++i) ex[i] = __ldg(p.expo + ((size_t)t * p.n_total + p.f0 + fold) * NCLS + u0 + j0 + i);
               } else {                                        // same keying as the SIMT engine: block 16 + class/4
-                const FoldPhilox k = fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
-                const Philox4 r = philox4x32_10((unsigned)t, k.fold, 16u + (unsigned)cta, (unsigned)p.offset, k.k0, k.k1);
+                const FoldPhilox k = SES ? FoldPhilox{0u, (unsigned)sseed, (unsigned)(sseed >> 32)} : fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
+                const Philox4 r = philox4x32_10((unsigned)ts, k.fold, 16u + (unsigned)cta, (unsigned)p.offset, k.k0, k.k1);
 #pragma unroll
                 for (int i = 0; i < UT; ++i) {
                   const int j = j0 + i;
@@ -349,10 +426,10 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
             }
           } else if (owns_fold) {
             {
-              const FoldPhilox k = fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
+              const FoldPhilox k = SES ? FoldPhilox{0u, (unsigned)sseed, (unsigned)(sseed >> 32)} : fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
               const unsigned g = k.fold, k0 = k.k0, k1 = k.k1, o0 = (unsigned)p.offset;
-              const Philox4 r0 = philox4x32_10((unsigned)t, g, 0u, o0, k0, k1), r1 = philox4x32_10((unsigned)t, g, 1u, o0, k0, k1),
-                            r2 = philox4x32_10((unsigned)t, g, 2u, o0, k0, k1);
+              const Philox4 r0 = philox4x32_10((unsigned)ts, g, 0u, o0, k0, k1), r1 = philox4x32_10((unsigned)ts, g, 1u, o0, k0, k1),
+                            r2 = philox4x32_10((unsigned)ts, g, 2u, o0, k0, k1);
               ur[0] = u_ref_range(r0.x); ur[1] = u_ref_range(r0.y); ur[2] = u_ref_range(r0.z); ur[3] = u_ref_range(r0.w);
               ur[4] = u_ref_range(r1.x); ur[5] = u_ref_range(r1.y); ur[6] = u_ref_range(r1.z); ur[7] = u_ref_range(r1.w);
               ur[8] = u_ref_range(r2.x); ur[9] = u_ref_range(r2.y); ur[10] = u_ref_range(r2.z);
@@ -380,8 +457,8 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
           for (int g = 0; g < 3; ++g) acc_rd(AC_S1, g, gi + g * UT);          // W2x h1'
 #pragma unroll
           for (int i = 0; i < UT; ++i) {                                     // w2h_a: W2h h2 (step t-1, phase C)
-            const float ghr = (t > 0 ? w2h_a[i] : 0.f) + b2h_r[i], ghz = (t > 0 ? w2h_a[UT + i] : 0.f) + b2h_r[UT + i],
-                        ghn = (t > 0 ? w2h_a[2 * UT + i] : 0.f) + b2h_r[2 * UT + i];
+            const float ghr = (warm ? w2h_a[i] : 0.f) + b2h_r[i], ghz = (warm ? w2h_a[UT + i] : 0.f) + b2h_r[UT + i],
+                        ghn = (warm ? w2h_a[2 * UT + i] : 0.f) + b2h_r[2 * UT + i];
             h2[i] = gru_unit_fast(gi[i] + pre[3 * UT + i], gi[UT + i] + pre[4 * UT + i], gi[2 * UT + i] + pre[5 * UT + i], ghr, ghz, ghn, h2[i]);
           }
           publish(img_h2, h2);
@@ -420,6 +497,18 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
           publish(img_y2, yv);
         }
         signal(3);
+        if constexpr (SES) {
+          if ((t & (SES_PERIOD - 1)) == SES_PERIOD - 1) {
+            // the version written at the previous boundary, in use from here: it agrees with the one in use so far on
+            // every step before the next boundary (DESIGN §3.7).  The acquire is satisfied: this CTA has gathered h1'
+            // of that boundary, released by CTA 0 after it wrote the version.
+            const int v = (t / SES_PERIOD) & 1;
+            counter_wait(p.counters + 0, (unsigned)P * (unsigned)(t + 2 - SES_PERIOD), p.abort_flag);
+            if (owns_fold) { const SesEntry en = ld_ses_entry(p.ses_tab + v * MT + fold); sa = en.a; se = en.e; sseed = en.seed; }
+            S = __ldcg(p.ses_stop + v);
+            if (decider) { m_req = ld_volatile_u64(&p.ses_mail[fold].req); m_can = ld_volatile_u64(&p.ses_mail[fold].cancel); }
+          }
+        }
         if (t + 1 < S) read_phase_a(t + 1);
       }
       if (profiling) { const long long c = clock64(); tprof[3] += c - tp0; tp0 = c; }
@@ -516,13 +605,14 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
           for (int k = 0; k < 10; ++k) lg[k] = lgc[k * ACP] + b3_r[k];
           const int k = mol_pick(lg, gn);
           x = mol_finish(lgc[(10 + k) * ACP] + b3[10 + k], lgc[(20 + k) * ACP] + b3[20 + k], lu);
-          if (owns_fold && slot == 0 && cta == 0) {
-            p.out[(size_t)(p.f0 + fold) * p.out_pitch + t] = x;
+          if (owns_fold && slot == 0 && cta == 0 && on) {
+            p.out[(size_t)(p.f0 + fold) * p.out_pitch + ts] = x;
             if (p.logits_out) {
 #pragma unroll
               for (int i = 0; i < 30; ++i) p.logits_out[((size_t)t * p.n_total + p.f0 + fold) * 30 + i] = lgc[i * ACP] + b3[i];
             }
-            if constexpr (LIVE) live_publish(p.progress + p.f0 + fold, t, S);
+            if constexpr (SES) ses_publish(p.progress + fold, ds.tag, ts, se - sa);
+            else if constexpr (LIVE) live_publish(p.progress + p.f0 + fold, t, S);
           }
         }
       } else {                                              // RAW: this CTA's 4 classes, then the candidate exchange
@@ -575,9 +665,10 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
           }
           combine_fold(best, bestk);
           x = 2.0f * (float)bestk / ((float)NCLS - 1.0f) - 1.0f;     // :235
-          if (owns_fold && slot == 0 && cta == 0) {
-            p.out[(size_t)(p.f0 + fold) * p.out_pitch + t] = x;
-            if constexpr (LIVE) live_publish(p.progress + p.f0 + fold, t, S);
+          if (owns_fold && slot == 0 && cta == 0 && on) {
+            p.out[(size_t)(p.f0 + fold) * p.out_pitch + ts] = x;
+            if constexpr (SES) ses_publish(p.progress + fold, ds.tag, ts, se - sa);
+            else if constexpr (LIVE) live_publish(p.progress + p.f0 + fold, t, S);
           }
         }
       }
@@ -721,6 +812,8 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
     float4 creg[COND_TASKS][2];
     // conditioning window of fold f of this tile: the strided fold, or the caller's tables (several utterances in one job)
     // strided windows: streams are indexed from the job's first fold, frame tensors from the stream's first sample
+    int2* ses_win = reinterpret_cast<int2*>(smem + OFF_SES);
+    const unsigned ses_frames = SES ? (unsigned)(p.seg_stride / p.hop) : 0u;   // frames of a slot's region
     auto row0_of = [&](int f) -> long long {
       return p.fold_row0 ? __ldg(p.fold_row0 + p.f0 + f) : (long long)(p.f0 + f + (FRAMES ? p.seg_first : 0)) * p.seg_stride - p.row_base;
     };
@@ -733,8 +826,15 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
     // from frame-rate tensors (UpsampleNetwork's stretch+conv cascade collapsed into 5 taps per output phase)
     auto cond_chunk = [&](int f, int c8, int n, float4& a, float4& b) {
       a = make_float4(0.f, 0.f, 0.f, 0.f); b = a;
-      const long long row = row0_of(f) + n;
-      if (row >= end_of(f)) return;
+      long long row;
+      if constexpr (SES) {                                 // slot f's window in the version the staging uses
+        const int2 w = ses_win[f];
+        if (n < w.x || n >= w.y) return;
+        row = (long long)f * p.seg_stride + (n - w.x);
+      } else {
+        row = row0_of(f) + n;
+        if (row >= end_of(f)) return;
+      }
       if constexpr (!FRAMES) { const float4* s = src_of(c8, row); a = __ldg(s); b = __ldg(s + 1); return; }
       const unsigned r = (unsigned)row, frame = r / (unsigned)p.hop, phase = r - frame * (unsigned)p.hop;
       if (c8 >= FEAT / 8) {
@@ -766,7 +866,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
     for (int j = 0; j < COND_TASKS; ++j) {
       const int task = st + j * 128;
       tk_c8[j] = -1; tk_left[j] = 0; tk_src[j] = nullptr; tk_frame[j] = 0; tk_phase[j] = 0;
-      if (deferred && task < n_tasks) {
+      if (deferred && !SES && task < n_tasks) {
         const int f = task / KQ, c8 = task % KQ;
         const long long r0 = row0_of(f);
         tk_c8[j] = c8; tk_left[j] = end_of(f) - r0;
@@ -776,6 +876,39 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
     }
     auto cond_fetch = [&](int n) {
       if (!deferred) return;
+      if constexpr (SES) {
+        // The window changes with admissions.  A slot's rows start on a frame boundary of its region, and every step's
+        // rows are fetched in order, so (frame, phase) restarts at the admission step and advances as above: no division.
+#pragma unroll
+        for (int j = 0; j < COND_TASKS; ++j) {
+          const int task = st + j * 128;
+          creg[j][0] = make_float4(0.f, 0.f, 0.f, 0.f); creg[j][1] = creg[j][0];
+          if (task < n_tasks) {
+            const int f = task / KQ, c8 = task - f * KQ;
+            const int2 w = ses_win[f];
+            if (n == w.x) { tk_frame[j] = (unsigned)f * ses_frames; tk_phase[j] = 0; }
+            if (n >= w.x && n < w.y) {
+              if (c8 >= FEAT / 8) {
+                const float4* s = reinterpret_cast<const float4*>(p.aux_frames + (size_t)tk_frame[j] * (4 * AUXD) + (c8 - FEAT / 8) * 8);
+                creg[j][0] = __ldg(s); creg[j][1] = __ldg(s + 1);
+              } else {
+                const float* k = p.up_taps + tk_phase[j] * 5;
+                const float* m = p.mel_frames + (size_t)tk_frame[j] * FEAT + c8 * 8;
+                float4 a = creg[j][0], b = creg[j][1];
+#pragma unroll
+                for (int d = 0; d < 5; ++d) {
+                  const float wgt = __ldg(k + d);
+                  const float4 x0 = __ldg(reinterpret_cast<const float4*>(m + d * FEAT)), x1 = __ldg(reinterpret_cast<const float4*>(m + d * FEAT) + 1);
+                  a.x = fmaf(wgt, x0.x, a.x); a.y = fmaf(wgt, x0.y, a.y); a.z = fmaf(wgt, x0.z, a.z); a.w = fmaf(wgt, x0.w, a.w);
+                  b.x = fmaf(wgt, x1.x, b.x); b.y = fmaf(wgt, x1.y, b.y); b.z = fmaf(wgt, x1.z, b.z); b.w = fmaf(wgt, x1.w, b.w);
+                }
+                creg[j][0] = a; creg[j][1] = b;
+              }
+            }
+            if (++tk_phase[j] == (unsigned)p.hop) { tk_phase[j] = 0; ++tk_frame[j]; }
+          }
+        }
+      } else {
 #pragma unroll
       for (int j = 0; j < COND_TASKS; ++j) {
         creg[j][0] = make_float4(0.f, 0.f, 0.f, 0.f); creg[j][1] = creg[j][0];
@@ -802,6 +935,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
           }
         }
         if constexpr (FRAMES) { if (++tk_phase[j] == (unsigned)p.hop) { tk_phase[j] = 0; ++tk_frame[j]; } }
+      }
       }
     };
     auto cond_store = [&](int n) {
@@ -836,6 +970,13 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
     // by a 13-instruction chain issued after the S2 chain of step n-1, so that between two exchanges the issuing warps
     // only ever do ONE of {store an image, issue the chain} and neither sits in front of a gather they could already
     // have launched.
+    // SES: the staging's windows of version `v` of the slot table (version -1 = buffer 1, before the loop), written
+    // between two barriers of the issuer warpgroup so that no staging thread reads a torn (a, e)
+    auto ses_windows = [&](int v) {
+      if (it < B) { const SesEntry en = ld_ses_entry(p.ses_tab + v * MT + it); ses_win[it] = make_int2(en.a, en.e); }
+      named_bar_sync(3, 128);
+    };
+    if constexpr (SES) ses_windows(1);
     cond_fetch(0);
     cond_store(0);
     named_bar_sync(2, 128);
@@ -864,6 +1005,16 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
       if (t + 2 < S) {
         // y2 of this step is still two epilogues away: free time for the staging threads
         mbar_wait(bar_q, (uint32_t)((t + 1) & 1), p.abort_flag);             // every warp's chain t+1 has consumed the image
+        if constexpr (SES) {
+          if ((t & (SES_PERIOD - 1)) == SES_PERIOD / 2) {
+            // the version written at this period's boundary, for rows from step t + 2 on (they agree with the last one
+            // before the next boundary; DESIGN §3.7).  Acquire: this CTA has gathered h1' of that boundary.
+            const int v = (t / SES_PERIOD) & 1;
+            counter_wait(p.counters + 0, (unsigned)P * (unsigned)(t + 1 - SES_PERIOD / 2), p.abort_flag);
+            S = __ldcg(p.ses_stop + v);
+            ses_windows(v);                                // (every staging thread passed barrier 2 after its last reads)
+          }
+        }
         cond_store(t + 2);
         if (t + 3 < S) cond_fetch(t + 3);
       }
@@ -894,9 +1045,9 @@ class TcEngine : public Engine {
   const char* name() const override { return cfg.precision == WRNN_PREC_BF16 ? "tcgen05-bf16" : "tcgen05-fp16"; }
   int grid_ctas() const override { return P; }
   // FRAMES = conditioning rows built in the kernel from frame-rate tensors (wrnn_job::mel_frames)
-  template <int FMT, bool FR, bool BIG, bool SC, bool LV = false>
+  template <int FMT, bool FR, bool BIG, bool SC, bool LV = false, bool SE = false>
   const void* kernel_of() const {
-    return cfg.mode == WRNN_MODE_RAW ? (const void*)wrnn_tc_kernel<FMT, FR, true, BIG, SC, LV> : (const void*)wrnn_tc_kernel<FMT, FR, false, BIG, SC, LV>;
+    return cfg.mode == WRNN_MODE_RAW ? (const void*)wrnn_tc_kernel<FMT, FR, true, BIG, SC, LV, SE> : (const void*)wrnn_tc_kernel<FMT, FR, false, BIG, SC, LV, SE>;
   }
   template <bool SC> const void* kernel_sc(bool frames, bool big) const {
     if (cfg.precision == WRNN_PREC_BF16)
@@ -911,6 +1062,11 @@ class TcEngine : public Engine {
     return cfg.precision == WRNN_PREC_BF16 ? kernel_of<1, true, BIG, false, true>() : kernel_of<0, true, BIG, false, true>();
   }
   const void* kernel_live(bool big) const { return big ? kernel_lv<true>() : kernel_lv<false>(); }
+  // the session form of the live kernel (wrnn_live_*)
+  template <bool BIG> const void* kernel_se() const {
+    return cfg.precision == WRNN_PREC_BF16 ? kernel_of<1, true, BIG, false, true, true>() : kernel_of<0, true, BIG, false, true, true>();
+  }
+  const void* kernel_session(bool big) const { return big ? kernel_se<true>() : kernel_se<false>(); }
   static constexpr int SMALL_TILE = 24;     // 24 folds x 26 chunks = 624 <= 5 tasks x 128 staging threads
 
   int init(const HostWeights& w) {
@@ -953,6 +1109,8 @@ class TcEngine : public Engine {
       WRNN_CUDA_OK(cudaFuncSetAttribute(kernel((v & 1) != 0, (v & 2) != 0, (v & 4) != 0), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     for (int v = 0; v < 2; ++v)
       WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_live(v != 0), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    for (int v = 0; v < 2; ++v)
+      WRNN_CUDA_OK(cudaFuncSetAttribute(kernel_session(v != 0), cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_SES));
     int n_sm = 0;
     WRNN_CUDA_OK(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
     if (n_sm < P) { set_error("tcgen05 engine needs >= 128 SMs for its co-resident weight shards"); return WRNN_E_NO_DEVICE; }
@@ -976,6 +1134,29 @@ class TcEngine : public Engine {
       return WRNN_E_INVALID;
     }
     return run(job, stream, keys, nullptr, progress);
+  }
+
+  int generate_session(const wrnn_job& job, cudaStream_t stream, const SesCtl& c) override {
+    WRNN_CUDA_OK(cudaSetDevice(device));
+    TcParams p{};
+    p.blob = static_cast<const unsigned char*>(d_blob_);
+    p.L = job.L; p.seg_stride = job.seg_stride;
+    p.n_seg = job.n_seg; p.n_total = job.n_seg; p.f0 = 0;
+    p.steps = 0x7fffffff; p.out_pitch = job.seg_len;   // open-ended: a version of the slot table sets the stop
+    p.out = job.out;
+    p.mel_frames = job.mel_frames; p.aux_frames = job.aux_frames; p.up_taps = job.up_taps; p.hop = job.hop;
+    p.xch = static_cast<unsigned char*>(d_scratch_);
+    p.xch5 = p.xch + xch5_off_;
+    p.counters = static_cast<unsigned*>(d_sync_);
+    p.abort_flag = reinterpret_cast<int*>(static_cast<unsigned*>(d_sync_) + 8);
+    p.prof = reinterpret_cast<long long*>(static_cast<unsigned char*>(d_sync_) + 64);
+    p.progress = c.progress; p.ses_tab = c.tab; p.ses_stop = c.stop; p.ses_mail = c.mail;
+    WRNN_CUDA_OK(cudaMemsetAsync(d_sync_, 0, 256, stream));
+    void* args[] = {&p};
+    WRNN_CUDA_OK(cudaLaunchCooperativeKernel(kernel_session(p.n_seg > SMALL_TILE), dim3(P), dim3(NT), args, SMEM_SES, stream));
+    ++launches;
+    last_steps_ = 0;
+    return WRNN_OK;
   }
 
   // nll != NULL: scoring (the loss of x_force[t] in the sampler's place; the draws are not read); progress != NULL: the
