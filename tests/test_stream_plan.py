@@ -215,6 +215,24 @@ def test_stream_plan_interpreted_on_the_cpu_equals_the_engine_contract(precision
 
 
 @pytest.mark.skipif(not cabi.is_built(), reason="library not built")
+@pytest.mark.parametrize("missing", ["I_weight", "fc3_bias"])
+def test_stream_plan_refuses_a_null_weight_pointer(missing):
+    """A null tensor in wrnn_weights is refused with wrnn_create's message, not dereferenced."""
+    lib = cabi.load()
+    lib.wrnn_debug_stream_plan.restype = C.c_int
+    lib.wrnn_debug_stream_plan.argtypes = [C.c_void_p] * 8 + [C.c_int32]
+    cfg = cabi.WrnnCfg(512, 512, 80, 32, 30, cabi.MODE_MOL, cabi.PREC_F16, 3)
+    sd = helpers.state_numpy(helpers.make_model(0, "MOL"))
+    w = cabi.WrnnWeights()
+    keep = [np.ascontiguousarray(sd[key], dtype=np.float32) for key in cabi.WEIGHT_KEYS]
+    for field, a in zip(cabi.WEIGHT_FIELDS, keep):
+        setattr(w, field, None if field == missing else a.ctypes.data)
+    nb, nc = C.c_uint64(0), C.c_uint64(0)
+    assert lib.wrnn_debug_stream_plan(C.byref(cfg), C.byref(w), None, C.byref(nb), None, C.byref(nc), None, None, -1) == -1
+    assert lib.wrnn_last_error().decode() == f"null weight pointer: {missing}"
+
+
+@pytest.mark.skipif(not cabi.is_built(), reason="library not built")
 def test_stream_plan_on_the_trained_checkpoint_teacher_forced():
     """Shipped checkpoint, real Tacotron mel, inputs forced to the reference's own samples: the interpreted plan's
     logits stay within the fp16 tolerances stated for the GPU engines (tests/test_gpu_trained.py)."""

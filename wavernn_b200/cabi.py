@@ -334,13 +334,8 @@ class Engine:
                     philox_seed: int = 0):
         """wrnn_vocode_host: mel (80, T) numpy -> float64 waveform of (T-1)*hop samples, what generate(mel[None], None,
         batched, target, overlap, mu_law) returns with gen_rng='philox' -- without torch."""
-        import numpy as np
-        mel = np.ascontiguousarray(mel, dtype=np.float32)
-        if mel.ndim == 3 and mel.shape[0] == 1:
-            mel = mel[0]
-        T = mel.shape[-1]
-        wav = np.empty(max(T - 1, 0) * getattr(self, "hop_length", 275), dtype=np.float64)
-        job = WrnnVocodeJob(mel.ctypes.data, int(T), int(bool(batched)), int(target), int(overlap), int(bool(mu_law)),
+        mel, wav = self._mel_and_wav(mel)
+        job = WrnnVocodeJob(mel.ctypes.data, mel.shape[-1], int(bool(batched)), int(target), int(overlap), int(bool(mu_law)),
                             int(philox_seed), wav.ctypes.data)
         _check(self.lib, self.lib.wrnn_vocode_host(self._h, C.byref(job)))
         return wav
@@ -358,12 +353,10 @@ class Engine:
                          mu_law: bool = False):
         """wrnn_vocode_many_host: a list of numpy mels (80, T_i) and one Philox seed per mel -> the list of float64
         waveforms, each bit-identical to vocode_host(mel_i, philox_seed=seeds[i]) on a handle with a fixed engine."""
-        import numpy as np
-        mels = [np.ascontiguousarray(m[0] if m.ndim == 3 and m.shape[0] == 1 else m, dtype=np.float32) for m in mels]
+        pairs = [self._mel_and_wav(m) for m in mels]
+        mels, wavs = [m for m, _ in pairs], [w for _, w in pairs]
         if len(seeds) != len(mels):
             raise ValueError("one seed per mel")
-        hop = getattr(self, "hop_length", 275)
-        wavs = [np.empty(max(m.shape[-1] - 1, 0) * hop, dtype=np.float64) for m in mels]
         b, keep = vocode_batch([(m.ctypes.data, m.shape[-1], s, w.ctypes.data) for m, s, w in zip(mels, seeds, wavs)],
                                batched=batched, target=target, overlap=overlap, mu_law=mu_law)
         _check(self.lib, self.lib.wrnn_vocode_many_host(self._h, C.byref(b)))
@@ -375,11 +368,8 @@ class Engine:
         batched=False, mu_law=mu_law, philox_seed=philox_seed), yielding each newly final slice while the kernel is still
         generating (views of one array; their concatenation is bit-identical to vocode_host's).  Each poll waits up to
         wait_us.  Closing the generator early still waits for the job, which cannot be cancelled."""
-        import numpy as np
-        mel = np.ascontiguousarray(mel[0] if mel.ndim == 3 and mel.shape[0] == 1 else mel, dtype=np.float32)
-        T = mel.shape[-1]
-        wav = np.empty(max(T - 1, 0) * getattr(self, "hop_length", 275), dtype=np.float64)
-        job = WrnnVocodeJob(mel.ctypes.data, int(T), 0, 0, 0, int(bool(mu_law)), int(philox_seed), wav.ctypes.data)
+        mel, wav = self._mel_and_wav(mel)
+        job = WrnnVocodeJob(mel.ctypes.data, mel.shape[-1], 0, 0, 0, int(bool(mu_law)), int(philox_seed), wav.ctypes.data)
         _check(self.lib, self.lib.wrnn_vocode_live_start(self._h, C.byref(job), None))
         n, prev, rc = C.c_int64(0), 0, 1
         try:
@@ -401,11 +391,10 @@ class Engine:
         of utterance i's slices is bit-identical to vocode_many_host's waveform i).  Each poll waits up to wait_us.
         Closing the generator early still waits for the job, which cannot be cancelled."""
         import numpy as np
-        mels = [np.ascontiguousarray(m[0] if m.ndim == 3 and m.shape[0] == 1 else m, dtype=np.float32) for m in mels]
+        pairs = [self._mel_and_wav(m) for m in mels]
+        mels, wavs = [m for m, _ in pairs], [w for _, w in pairs]
         if len(seeds) != len(mels):
             raise ValueError("one seed per mel")
-        hop = getattr(self, "hop_length", 275)
-        wavs = [np.empty(max(m.shape[-1] - 1, 0) * hop, dtype=np.float64) for m in mels]
         b, keep = vocode_batch([(m.ctypes.data, m.shape[-1], s, w.ctypes.data) for m, s, w in zip(mels, seeds, wavs)],
                                batched=False, mu_law=mu_law)
         _check(self.lib, self.lib.wrnn_vocode_many_live_start(self._h, C.byref(b), None))
@@ -423,6 +412,15 @@ class Engine:
         finally:
             while rc == 1:                               # closed early: the job runs to its end, into `wavs`
                 rc = self.lib.wrnn_vocode_many_live_poll(self._h, 100000, n.ctypes.data)
+
+    def _mel_and_wav(self, mel):
+        """mel (80, T) or (1, 80, T) as a contiguous float32 (80, T) array, and a zeroed float64 waveform of its
+        (T - 1) * hop samples."""
+        import numpy as np
+        mel = np.ascontiguousarray(mel, dtype=np.float32)
+        if mel.ndim == 3 and mel.shape[0] == 1:
+            mel = mel[0]
+        return mel, np.zeros(max(mel.shape[-1] - 1, 0) * getattr(self, "hop_length", 275), dtype=np.float64)
 
     def live_session(self, capacity: int, max_T: int, mu_law: bool = False):
         """wrnn_live_open: a LiveSession of `capacity` slots (1 to 64) for mels of up to max_T frames, into whose running
@@ -451,7 +449,7 @@ class Engine:
         """wrnn_score_many_host: a list of numpy mels (80, T_i) and the waveforms xs[i] (n_i samples, n_i <= T_i * hop)
         -> the list of per-sample losses (nats, float32), without torch."""
         import numpy as np
-        mels = [np.ascontiguousarray(m[0] if m.ndim == 3 and m.shape[0] == 1 else m, dtype=np.float32) for m in mels]
+        mels = [self._mel_and_wav(m)[0] for m in mels]
         xs = [np.ascontiguousarray(x, dtype=np.float32).reshape(-1) for x in xs]
         if len(xs) != len(mels):
             raise ValueError("one waveform per mel")
@@ -484,7 +482,6 @@ class LiveSession:
 
     def __init__(self, engine: Engine, capacity: int, max_T: int, mu_law: bool = False):
         self.engine, self.lib, self.capacity = engine, engine.lib, int(capacity)
-        self.hop = getattr(engine, "hop_length", 275)
         _check(self.lib, self.lib.wrnn_live_open(engine._h, self.capacity, int(max_T), int(bool(mu_law)), None))
         self.open = True
         self.waves, self.states, self._mels, self._prev = {}, {}, {}, {}
@@ -492,11 +489,8 @@ class LiveSession:
 
     def submit(self, mel, *, philox_seed: int) -> int:
         """Submits mel (80, T) numpy; returns its ticket.  Raises EngineError(WRNN_E_BUSY) when every slot is held."""
-        import numpy as np
-        mel = np.ascontiguousarray(mel[0] if mel.ndim == 3 and mel.shape[0] == 1 else mel, dtype=np.float32)
-        T = mel.shape[-1]
-        wav = np.zeros(max(T - 1, 0) * self.hop, dtype=np.float64)
-        u = WrnnUtterance(mel.ctypes.data, int(T), int(philox_seed), wav.ctypes.data)
+        mel, wav = self.engine._mel_and_wav(mel)
+        u = WrnnUtterance(mel.ctypes.data, mel.shape[-1], int(philox_seed), wav.ctypes.data)
         tk = C.c_int64(0)
         _check(self.lib, self.lib.wrnn_live_submit(self.engine._h, C.byref(u), C.byref(tk)))
         t = int(tk.value)

@@ -6,6 +6,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <new>
+#include <optional>
 #include <string>
 #include <thread>
 #include <vector>
@@ -18,13 +19,109 @@ namespace wrnn {
 static thread_local std::string g_last_error;
 void set_error(const std::string& msg) { g_last_error = msg; }
 
-static int fetch(std::vector<float>& dst, const float* src, size_t n, const char* what) {
-  if (!src) { set_error(std::string("null weight pointer: ") + what); return WRNN_E_INVALID; }
-  dst.resize(n);
-  // cudaMemcpyDefault resolves host or device pointers through UVA
-  cudaError_t e = cudaMemcpy(dst.data(), src, n * sizeof(float), cudaMemcpyDefault);
-  if (e != cudaSuccess) { set_error(std::string("copying ") + what + ": " + cudaGetErrorString(e)); return WRNN_E_CUDA; }
+int check_frames(const std::string& name, long long T) {
+  if (T >= 21) return WRNN_OK;
+  set_error(name + " must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples");
+  return WRNN_E_INVALID;
+}
+
+int check_utterance(const std::string& at, const void* mel, const void* wav, long long T) {
+  if (!mel || !wav) { set_error(at + "mel and wav are required"); return WRNN_E_INVALID; }
+  return check_frames(at + "T", T);
+}
+
+// The 16 tensors of `w` into hw, in the style of cond::build_host_upsampler: host_only reads host memory with no CUDA
+// call, otherwise cudaMemcpyDefault resolves host or device pointers through UVA.
+static int read_weights(const wrnn_cfg& cfg, const wrnn_weights& w, bool host_only, HostWeights& hw) {
+  const size_t W2W = H + AUXD, NC = (size_t)cfg.n_classes;
+#define WT(dst, src, n) {&hw.dst, w.src, (n), #src}
+  const struct { std::vector<float>* dst; const float* src; size_t n; const char* name; } list[] = {
+      WT(I_w, I_weight, (size_t)H * (1 + F1IN)), WT(I_b, I_bias, H),
+      WT(w1i, rnn1_weight_ih, (size_t)G3 * H), WT(w1h, rnn1_weight_hh, (size_t)G3 * H),
+      WT(b1i, rnn1_bias_ih, G3), WT(b1h, rnn1_bias_hh, G3),
+      WT(w2i, rnn2_weight_ih, (size_t)G3 * W2W), WT(w2h, rnn2_weight_hh, (size_t)G3 * H),
+      WT(b2i, rnn2_bias_ih, G3), WT(b2h, rnn2_bias_hh, G3),
+      WT(f1w, fc1_weight, (size_t)H * W2W), WT(f1b, fc1_bias, H),
+      WT(f2w, fc2_weight, (size_t)H * W2W), WT(f2b, fc2_bias, H),
+      WT(f3w, fc3_weight, NC * H), WT(f3b, fc3_bias, NC)};
+#undef WT
+  hw.n_classes = cfg.n_classes;
+  for (const auto& t : list) {
+    if (!t.src) { set_error(std::string("null weight pointer: ") + t.name); return WRNN_E_INVALID; }
+    t.dst->resize(t.n);
+    if (host_only) { std::memcpy(t.dst->data(), t.src, t.n * sizeof(float)); continue; }
+    const cudaError_t e = cudaMemcpy(t.dst->data(), t.src, t.n * sizeof(float), cudaMemcpyDefault);
+    if (e != cudaSuccess) { set_error(std::string("copying ") + t.name + ": " + cudaGetErrorString(e)); return WRNN_E_CUDA; }
+  }
   return WRNN_OK;
+}
+
+static int grow(void** buf, size_t* bytes, size_t want) {
+  if (want <= *bytes) return WRNN_OK;
+  if (*buf) cudaFree(*buf);
+  *buf = nullptr; *bytes = 0;
+  WRNN_CUDA_OK(cudaMalloc(buf, want));
+  *bytes = want;
+  return WRNN_OK;
+}
+
+// grow for a pinned host buffer mapped into the device's address space; *dev is its device alias.
+static int grow_mapped(void** host, void** dev, size_t* bytes, size_t want) {
+  if (want <= *bytes) return WRNN_OK;
+  if (*host) cudaFreeHost(*host);
+  *host = *dev = nullptr; *bytes = 0;
+  WRNN_CUDA_OK(cudaHostAlloc(host, want, cudaHostAllocMapped));
+  WRNN_CUDA_OK(cudaHostGetDevicePointer(dev, *host, 0));
+  *bytes = want;
+  return WRNN_OK;
+}
+
+// Staging of the host-memory entry points.  stage places each item at a 256-B-aligned offset of the handle's one device
+// staging buffer and copies it there on st (cudaMemcpyDefault: src may be host or device memory; src NULL: a region the
+// job writes); dev[k] is item k's device address, NULL for an empty item.  unstage, their common end, copies the results
+// back, synchronises and returns the engine's check().
+struct Staged { const void* src; size_t bytes; };
+struct Unstaged { void* dst; const void* src; size_t bytes; };
+static size_t align256(size_t bytes) { return (bytes + 255) & ~size_t(255); }
+
+static int stage(wrnn_t* h, const std::vector<Staged>& items, cudaStream_t st, std::vector<void*>& dev) {
+  size_t total = 0;
+  for (const Staged& it : items) total += align256(it.bytes);
+  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
+  const int rc = grow(&h->d_stage, &h->stage_bytes, total);
+  if (rc != WRNN_OK) return rc;
+  char* d = static_cast<char*>(h->d_stage);
+  dev.assign(items.size(), nullptr);
+  for (size_t k = 0; k < items.size(); ++k) {
+    if (!items[k].bytes) continue;
+    dev[k] = d;
+    if (items[k].src) WRNN_CUDA_OK(cudaMemcpyAsync(d, items[k].src, items[k].bytes, cudaMemcpyDefault, st));
+    d += align256(items[k].bytes);
+  }
+  return WRNN_OK;
+}
+
+static int unstage(wrnn_t* h, const std::vector<Unstaged>& items) {
+  for (const Unstaged& it : items)
+    if (it.bytes) WRNN_CUDA_OK(cudaMemcpyAsync(it.dst, it.src, it.bytes, cudaMemcpyDeviceToHost, 0));
+  WRNN_CUDA_OK(cudaStreamSynchronize(0));
+  return h->last->check();
+}
+
+// The host epilogue's tables (wrnn_vocode's unbatched geometry): mu is empty unless mu-law applies, which it does on a
+// RAW head only.
+struct LiveTables {
+  std::vector<double> mu, tail;
+  long long tail_len = 0;
+  int n_classes = 0;
+};
+static LiveTables live_tables(int mode, bool mu_law, int n_classes, int hop) {
+  LiveTables t;
+  std::vector<double> fade_in, fade_out;
+  cond::epilogue_tables(0, mu_law && mode == WRNN_MODE_RAW, n_classes, hop, fade_in, fade_out, t.mu, t.tail);
+  t.tail_len = 20ll * hop;
+  t.n_classes = n_classes;
+  return t;
 }
 
 // A live job: wrnn_vocode_live_start's one utterance or wrnn_vocode_many_live_start's n, utterance i being fold i.  The
@@ -34,17 +131,16 @@ static int fetch(std::vector<float>& dst, const float* src, size_t n, const char
 struct LiveJob {
   static constexpr int MAX_UTTS = 64;   // one persistent tile
   static constexpr size_t SAMPLES_OFF = MAX_UTTS * sizeof(unsigned long long);
-  void* host = nullptr;                 // cudaHostAlloc(..., cudaHostAllocMapped), grown on demand
+  void* host = nullptr;                 // pinned and mapped (grow_mapped)
   void* dev = nullptr;                  // its device alias
   size_t bytes = 0;
   cudaEvent_t done = nullptr;           // recorded after the kernel
   Engine* e = nullptr;
   bool many = false;                    // started by wrnn_vocode_many_live_start (served by its poll only)
-  long long steps = 0, tail_len = 0;    // samples per fold (the row pitch of the sample block), fade-out length
-  int n_classes = 0;
+  long long steps = 0;                  // samples per fold (the row pitch of the sample block)
+  LiveTables tabs;
   std::vector<double*> wav;             // per utterance: the caller's [wave_len[i]]
   std::vector<long long> wave_len, delivered;
-  std::vector<double> mu, tail;         // the epilogue tables (mu empty without mu_law)
   int n() const { return (int)wav.size(); }
   unsigned long long progress(int i) const {
     return __atomic_load_n(static_cast<const unsigned long long*>(host) + i, __ATOMIC_ACQUIRE);
@@ -100,19 +196,8 @@ int wrnn_create(wrnn_t** out, const wrnn_cfg* cfg, const wrnn_weights* w, int de
     return WRNN_E_NO_DEVICE;
   }
   HostWeights hw;
-  hw.n_classes = cfg->n_classes;
-  const size_t W2W = H + AUXD;
-  int rc;
-#define FETCH(field, src, n) if ((rc = fetch(hw.field, w->src, (n), #src)) != WRNN_OK) return rc
-  FETCH(I_w, I_weight, (size_t)H * (1 + F1IN)); FETCH(I_b, I_bias, H);
-  FETCH(w1i, rnn1_weight_ih, (size_t)G3 * H); FETCH(w1h, rnn1_weight_hh, (size_t)G3 * H);
-  FETCH(b1i, rnn1_bias_ih, G3); FETCH(b1h, rnn1_bias_hh, G3);
-  FETCH(w2i, rnn2_weight_ih, (size_t)G3 * W2W); FETCH(w2h, rnn2_weight_hh, (size_t)G3 * H);
-  FETCH(b2i, rnn2_bias_ih, G3); FETCH(b2h, rnn2_bias_hh, G3);
-  FETCH(f1w, fc1_weight, (size_t)H * W2W); FETCH(f1b, fc1_bias, H);
-  FETCH(f2w, fc2_weight, (size_t)H * W2W); FETCH(f2b, fc2_bias, H);
-  FETCH(f3w, fc3_weight, (size_t)cfg->n_classes * H); FETCH(f3b, fc3_bias, cfg->n_classes);
-#undef FETCH
+  int rc = read_weights(*cfg, *w, false, hw);
+  if (rc != WRNN_OK) return rc;
   Engine* eng = nullptr;
   int engine = cfg->engine;
   if (cfg->precision == WRNN_PREC_FP32) {
@@ -256,45 +341,23 @@ int wrnn_generate_host(wrnn_t* h, const wrnn_job* job) {
   Engine* e = nullptr;
   if ((rc = pick_engine(h, job, &e)) != WRNN_OK) return rc;
   h->last = e;
-  WRNN_CUDA_OK(cudaSetDevice(e->device));
   const size_t S = job->steps > 0 ? job->steps : job->seg_len;
-  const size_t B = job->n_seg, NC = e->cfg.n_classes;
-  const size_t n_mel = (size_t)job->L * FEAT, n_aux = (size_t)job->L * 4 * AUXD;
-  const size_t n_uni = job->uniforms ? S * 11 * B : 0, n_exp = job->expo ? S * B * NC : 0;
-  const size_t n_xf = job->x_force ? S * B : 0, n_out = B * S, n_log = job->logits_out ? S * B * NC : 0;
-  const size_t n_tab = job->fold_row0 ? 4 * B : 0;   // two int64 tables, counted in floats
-  const size_t total = (n_mel + n_aux + n_uni + n_exp + n_xf + n_out + n_log + n_tab + 2) * sizeof(float);
-  if (total > h->stage_bytes) {
-    if (h->d_stage) cudaFree(h->d_stage);
-    h->d_stage = nullptr; h->stage_bytes = 0;
-    WRNN_CUDA_OK(cudaMalloc(&h->d_stage, total));
-    h->stage_bytes = total;
-  }
-  float* d = static_cast<float*>(h->d_stage);
-  wrnn_job dj = *job;
-  auto up = [&](const float* src, size_t n) -> float* {
-    if (!n) return nullptr;
-    float* p = d; d += n;
-    cudaMemcpyAsync(p, src, n * sizeof(float), cudaMemcpyHostToDevice, 0);
-    return p;
-  };
-  dj.mels_up = up(job->mels_up, n_mel); dj.aux = up(job->aux, n_aux);
-  dj.uniforms = up(job->uniforms, n_uni); dj.expo = up(job->expo, n_exp); dj.x_force = up(job->x_force, n_xf);
-  dj.out = d; d += n_out;
-  dj.logits_out = n_log ? d : nullptr; d += n_log;
-  if (n_tab) {
-    d = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(d) + 7) & ~uintptr_t(7));
-    int64_t* t0 = reinterpret_cast<int64_t*>(d);
-    cudaMemcpyAsync(t0, job->fold_row0, B * 8, cudaMemcpyHostToDevice, 0);
-    cudaMemcpyAsync(t0 + B, job->fold_row_end, B * 8, cudaMemcpyHostToDevice, 0);
-    dj.fold_row0 = t0; dj.fold_row_end = t0 + B;
-  }
-  rc = e->generate(dj, 0, nullptr);
+  const size_t B = job->n_seg, NC = e->cfg.n_classes, F = sizeof(float);
+  const size_t b_tab = job->fold_row0 ? B * sizeof(int64_t) : 0, b_out = B * S * F, b_log = job->logits_out ? S * B * NC * F : 0;
+  std::vector<void*> d;
+  rc = stage(h, {{job->mels_up, (size_t)job->L * FEAT * F}, {job->aux, (size_t)job->L * 4 * AUXD * F},
+                 {job->uniforms, job->uniforms ? S * 11 * B * F : 0}, {job->expo, job->expo ? S * B * NC * F : 0},
+                 {job->x_force, job->x_force ? S * B * F : 0}, {job->fold_row0, b_tab}, {job->fold_row_end, b_tab},
+                 {nullptr, b_out}, {nullptr, b_log}},
+             0, d);
   if (rc != WRNN_OK) return rc;
-  WRNN_CUDA_OK(cudaMemcpyAsync(job->out, dj.out, n_out * sizeof(float), cudaMemcpyDeviceToHost, 0));
-  if (n_log) WRNN_CUDA_OK(cudaMemcpyAsync(job->logits_out, dj.logits_out, n_log * sizeof(float), cudaMemcpyDeviceToHost, 0));
-  WRNN_CUDA_OK(cudaStreamSynchronize(0));
-  return e->check();
+  wrnn_job dj = *job;
+  dj.mels_up = static_cast<float*>(d[0]); dj.aux = static_cast<float*>(d[1]);
+  dj.uniforms = static_cast<float*>(d[2]); dj.expo = static_cast<float*>(d[3]); dj.x_force = static_cast<float*>(d[4]);
+  dj.fold_row0 = static_cast<int64_t*>(d[5]); dj.fold_row_end = static_cast<int64_t*>(d[6]);
+  dj.out = static_cast<float*>(d[7]); dj.logits_out = static_cast<float*>(d[8]);
+  if ((rc = e->generate(dj, 0, nullptr)) != WRNN_OK) return rc;
+  return unstage(h, {{job->out, dj.out, b_out}, {job->logits_out, dj.logits_out, b_log}});
 }
 
 const char* wrnn_engine_name(const wrnn_t* h) { return (h && h->last) ? h->last->name() : ""; }
@@ -319,20 +382,11 @@ int wrnn_expand_conditioning(const float* mel_frames, const float* aux_frames, c
 // wrnn_vocode: generate(gen_rng='philox') restated -- the frame-rate branch of WaveRNN._run_segments and the device branch
 // of WaveRNN._finish, with the conditioning network of wrnn_cond.cu in place of torch's.
 // ---------------------------------------------------------------------------------------------------------------------
-static int grow(void** buf, size_t* bytes, size_t want) {
-  if (want <= *bytes) return WRNN_OK;
-  if (*buf) cudaFree(*buf);
-  *buf = nullptr; *bytes = 0;
-  WRNN_CUDA_OK(cudaMalloc(buf, want));
-  *bytes = want;
-  return WRNN_OK;
-}
-
 static int validate_vocode(const wrnn_t* h, const wrnn_vocode_job* job) {
   if (!h || !h->engine || !job) { set_error("null handle or job"); return WRNN_E_INVALID; }
   if (!h->upsampler) { set_error("no upsampler attached (wrnn_attach_upsampler)"); return WRNN_E_INVALID; }
-  if (!job->mel || !job->wav) { set_error("mel and wav are required"); return WRNN_E_INVALID; }
-  if (job->T < 21) { set_error("T must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples"); return WRNN_E_INVALID; }
+  const int rc = check_utterance("", job->mel, job->wav, job->T);
+  if (rc != WRNN_OK) return rc;
   if (job->T * h->upsampler->hop >= (1ll << 31)) { set_error("stream longer than 2^31 samples"); return WRNN_E_INVALID; }
   if (job->batched && (job->target <= 0 || job->overlap <= 0)) {
     set_error("a batched job needs target > 0 and overlap > 0"); return WRNN_E_INVALID;
@@ -354,12 +408,28 @@ static int pick_vocode_engine(wrnn_t* h, wrnn_job& j, Engine** e, bool* expanded
   return pick_engine(h, &j, e);
 }
 
+// Scratch floats of the expanded rows of a stream of L rows.
+static size_t rows_floats(long long L) { return align_floats((size_t)L * FEAT) + align_floats((size_t)L * 4 * AUXD); }
+
+// The conditioning of job j: the frames, or on an engine that takes per-sample rows (expanded), rows [0, n_rows) of the
+// stream of L rows expanded into `rows` (rows_floats(L) of scratch), enqueued on st.
+static int frames_or_rows(const Upsampler& u, float* mel_frames, float* aux_frames, bool expanded, long long L,
+                          long long n_rows, float* rows, cudaStream_t st, wrnn_job& j) {
+  if (!expanded) {
+    j.mel_frames = mel_frames; j.aux_frames = aux_frames; j.up_taps = u.d_taps;
+    return WRNN_OK;
+  }
+  j.mels_up = rows; j.aux = rows + align_floats((size_t)L * FEAT);
+  return expand_conditioning(mel_frames, aux_frames, u.d_taps, u.hop, 0, n_rows, rows, rows + align_floats((size_t)L * FEAT), st);
+}
+
 // fade_in / fade_out / mu / tail of the epilogue on the device, rebuilt and uploaded only when (overlap, mu_law,
-// n_classes) changes.
+// n_classes) changes.  mu-law applies to a RAW head only.
 struct EpTables { const double *fade_in, *fade_out, *mu, *tail; };
-static int epilogue_tables(wrnn_t* h, int ov, bool mu_law, cudaStream_t st, EpTables* t) {
+static int epilogue_tables(wrnn_t* h, int ov, int mu_law_flag, cudaStream_t st, EpTables* t) {
   Upsampler& u = *h->upsampler;
   const int nc = h->engine->cfg.n_classes;
+  const bool mu_law = mu_law_flag && h->engine->cfg.mode == WRNN_MODE_RAW;
   if (u.tabs_key[0] != ov || u.tabs_key[1] != (mu_law ? 1 : 0) || u.tabs_key[2] != nc) {
     u.tabs_key[0] = u.tabs_key[1] = u.tabs_key[2] = -1;
     std::vector<double> fi, fo, mu, tail;
@@ -417,25 +487,15 @@ static int vocode_job(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st, Vo
 
   const size_t n_mf = align_floats((size_t)(T + 4) * FEAT), n_af = align_floats((size_t)T * cond::CD);
   const size_t n_smp = align_floats((size_t)g.n_seg * g.seg_len);
-  const size_t n_rows = expanded ? align_floats((size_t)L * FEAT) + align_floats((size_t)L * 4 * AUXD) : 0;
-  rc = grow(&u.d_scratch, &u.scratch_bytes, (n_mf + n_af + n_smp + n_rows) * sizeof(float));
+  rc = grow(&u.d_scratch, &u.scratch_bytes, (n_mf + n_af + n_smp + (expanded ? rows_floats(L) : 0)) * sizeof(float));
   if (rc != WRNN_OK) return rc;
   float* mel_frames = static_cast<float*>(u.d_scratch);
   float* aux_frames = mel_frames + n_mf;
   float* samples = aux_frames + n_af;
 
-  const bool mu_law = job->mu_law && h->engine->cfg.mode == WRNN_MODE_RAW;
-  if ((rc = epilogue_tables(h, (int)g.overlap, mu_law, st, &v->tabs)) != WRNN_OK) return rc;
-
+  if ((rc = epilogue_tables(h, (int)g.overlap, job->mu_law, st, &v->tabs)) != WRNN_OK) return rc;
   if ((rc = conditioning_frames(u, job->mel, T, mel_frames, aux_frames, nullptr, st)) != WRNN_OK) return rc;
-  if (expanded) {
-    float* mels_up = samples + n_smp;
-    float* aux = mels_up + align_floats((size_t)L * FEAT);
-    if ((rc = expand_conditioning(mel_frames, aux_frames, u.d_taps, hop, 0, L, mels_up, aux, st)) != WRNN_OK) return rc;
-    j.mels_up = mels_up; j.aux = aux;
-  } else {
-    j.mel_frames = mel_frames; j.aux_frames = aux_frames; j.up_taps = u.d_taps;
-  }
+  if ((rc = frames_or_rows(u, mel_frames, aux_frames, expanded, L, L, samples + n_smp, st, j)) != WRNN_OK) return rc;
   j.out = samples;
   v->g = g;
   v->e = e;
@@ -454,81 +514,97 @@ static int vocode(wrnn_t* h, const wrnn_vocode_job* job, cudaStream_t st) {
                        h->engine->cfg.n_classes, v.tabs.tail, 20ll * hop, (job->T - 1) * hop, job->wav, st);
 }
 
-// wrnn_vocode_many: the batch as one job (layout: cond::batch_plan).  `b` holds DEVICE mel pointers (and DEVICE wav
-// pointers unless live).
-static int vocode_many_job(wrnn_t* h, const wrnn_vocode_batch* b, const cond::BatchPlan& pl, cudaStream_t st, bool live,
-                           VocodeJob* v) {
+// The job of a batch laid out by cond::batch_plan or cond::score_plan (mels[i]: utterance i's DEVICE mel), up to what
+// its caller adds: the fold tables, the engine, scratch and the conditioning frames (or the expanded rows of a SIMT
+// engine), enqueued on st.  Scratch: [row0 | row_end | CondUtt table | the caller's table (tab_bytes) | mel_frames |
+// aux_frames | the caller's regions (n_floats) | expanded rows].  The frame regions span every utterance's T + 4 frames
+// (aux_frames included, so that no row of the laid-out stream maps outside them).  Once the engine e is picked,
+// fill(e, tab) refuses it (returning its code, message set) or writes the caller's table into the host image at tab;
+// the tables then go up in one copy.
+struct BatchJob {
+  wrnn_job j;                          // fold tables and conditioning set; out and x_force are the caller's
+  Engine* e = nullptr;
+  const unsigned char* tab = nullptr;  // the caller's table (device)
+  float* regions = nullptr;            // the caller's regions (device)
+};
+
+template <class Fill>
+static int batch_job(wrnn_t* h, const cond::BatchPlan& pl, const float* const* mels, size_t tab_bytes, size_t n_floats,
+                     cudaStream_t st, BatchJob* bj, Fill fill) {
   Upsampler& u = *h->upsampler;
-  const int hop = u.hop, n = b->n_utts;
+  const int n = (int)pl.frame0.size() - 1;
   const size_t nf = (size_t)pl.g.n_seg;
   WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
 
-  wrnn_job& j = v->j;
+  wrnn_job& j = bj->j;
   std::memset(&j, 0, sizeof(j));
   j.L = pl.L; j.seg_stride = pl.g.seg_stride; j.n_seg = (int32_t)nf; j.seg_len = (int32_t)pl.g.seg_len;
-  j.hop = hop; j.cond_mode = WRNN_COND_AUTO;
+  j.hop = u.hop; j.cond_mode = WRNN_COND_AUTO;
   const void* tag = h->upsampler;                      // placeholders: only tested against NULL
   j.fold_row0 = j.fold_row_end = static_cast<const int64_t*>(tag);
-  Engine* e = nullptr;
   bool expanded = false;
-  int rc = pick_vocode_engine(h, j, &e, &expanded);
+  int rc = pick_vocode_engine(h, j, &bj->e, &expanded);
   if (rc != WRNN_OK) return rc;
-  if (live && e->live_refusal()) { set_error(e->live_refusal()); return WRNN_E_INVALID; }
 
-  // scratch: [row0 | row_end | keys | CondUtt table | EpUtt table | mel_frames | aux_frames | samples | expanded rows]
-  // The frame regions span every utterance's T + 4 frames (aux_frames included, so that no row of the laid-out stream
-  // maps outside them); the tables go up in one copy.
+  const size_t b_row = align256(nf * sizeof(int64_t)), b_cu = align256(n * sizeof(CondUtt));
+  const size_t o_tab = 2 * b_row + b_cu, b_tab = o_tab + align256(tab_bytes);
+  u.host_plan.assign(b_tab, 0);
+  unsigned char* hp = u.host_plan.data();
+  if ((rc = fill(*bj->e, hp + o_tab)) != WRNN_OK) return rc;
+  std::memcpy(hp, pl.row0.data(), nf * sizeof(int64_t));
+  std::memcpy(hp + b_row, pl.row_end.data(), nf * sizeof(int64_t));
+  CondUtt* cu = reinterpret_cast<CondUtt*>(hp + 2 * b_row);
+  for (int i = 0; i < n; ++i) cu[i] = CondUtt{mels[i], pl.frame0[i + 1] - pl.frame0[i] - 4, pl.frame0[i]};
+
   const size_t n_frames = (size_t)pl.frame0.back();
-  const size_t b_row = align_floats(2 * nf) * 4, b_key = align_floats(4 * nf) * 4;
-  const size_t b_cu = align_floats(n * sizeof(CondUtt) / 4 + 1) * 4, b_eu = align_floats(n * sizeof(EpUtt) / 4 + 1) * 4;
-  const size_t b_tab = 2 * b_row + b_key + b_cu + b_eu;
-  const size_t n_mf = align_floats(n_frames * FEAT), n_af = align_floats(n_frames * cond::CD), n_smp = align_floats(nf * pl.g.seg_len);
-  const size_t n_rows = expanded ? align_floats((size_t)pl.L * FEAT) + align_floats((size_t)pl.L * 4 * AUXD) : 0;
-  rc = grow(&u.d_scratch, &u.scratch_bytes, b_tab + (n_mf + n_af + n_smp + n_rows) * sizeof(float));
+  const size_t n_mf = align_floats(n_frames * FEAT), n_af = align_floats(n_frames * cond::CD);
+  rc = grow(&u.d_scratch, &u.scratch_bytes, b_tab + (n_mf + n_af + n_floats + (expanded ? rows_floats(pl.L) : 0)) * sizeof(float));
   if (rc != WRNN_OK) return rc;
   unsigned char* d = static_cast<unsigned char*>(u.d_scratch);
   float* mel_frames = reinterpret_cast<float*>(d + b_tab);
   float* aux_frames = mel_frames + n_mf;
-  float* samples = aux_frames + n_af;
-
-  u.host_plan.assign(b_tab, 0);
-  unsigned char* hp = u.host_plan.data();
-  std::memcpy(hp, pl.row0.data(), nf * 8);
-  std::memcpy(hp + b_row, pl.row_end.data(), nf * 8);
-  std::memcpy(hp + 2 * b_row, pl.keys.data(), nf * sizeof(FoldKey));
-  CondUtt* cu = reinterpret_cast<CondUtt*>(hp + 2 * b_row + b_key);
-  EpUtt* eu = reinterpret_cast<EpUtt*>(hp + 2 * b_row + b_key + b_cu);
-  for (int i = 0; i < n; ++i) {
-    cu[i] = CondUtt{b->utts[i].mel, b->utts[i].T, pl.frame0[i]};
-    eu[i] = EpUtt{pl.fold0[i], (int)(pl.fold0[i + 1] - pl.fold0[i]), (b->utts[i].T - 1) * hop, b->utts[i].wav};
-  }
+  bj->regions = aux_frames + n_af;
   WRNN_CUDA_OK(cudaMemcpyAsync(d, hp, b_tab, cudaMemcpyHostToDevice, st));
   j.fold_row0 = reinterpret_cast<const int64_t*>(d);
   j.fold_row_end = reinterpret_cast<const int64_t*>(d + b_row);
-  const FoldKey* keys = reinterpret_cast<const FoldKey*>(d + 2 * b_row);
-  const CondUtt* d_cu = reinterpret_cast<const CondUtt*>(d + 2 * b_row + b_key);
-  const EpUtt* d_eu = reinterpret_cast<const EpUtt*>(d + 2 * b_row + b_key + b_cu);
+  bj->tab = d + o_tab;
 
-  const bool mu_law = b->mu_law && h->engine->cfg.mode == WRNN_MODE_RAW;
-  if (!live && (rc = epilogue_tables(h, (int)pl.g.overlap, mu_law, st, &v->tabs)) != WRNN_OK) return rc;
-
+  const CondUtt* d_cu = reinterpret_cast<const CondUtt*>(d + 2 * b_row);
   if ((rc = conditioning_frames_batch(u, d_cu, n, pl.max_T, mel_frames, aux_frames, st)) != WRNN_OK) return rc;
-  if (expanded) {
-    // rows [0, L - 4*hop): the last utterance's 4*hop gap rows would read frames past the end and no fold reads them
-    float* mels_up = samples + n_smp;
-    float* aux = mels_up + align_floats((size_t)pl.L * FEAT);
-    if ((rc = expand_conditioning(mel_frames, aux_frames, u.d_taps, hop, 0, pl.L - 4ll * hop, mels_up, aux, st)) != WRNN_OK) return rc;
-    j.mels_up = mels_up; j.aux = aux;
-  } else {
-    j.mel_frames = mel_frames; j.aux_frames = aux_frames; j.up_taps = u.d_taps;
-  }
-  j.out = samples;
-  v->g = pl.g;
-  v->e = e;
-  v->keys = keys;
-  v->eu = d_eu;
-  h->last = e;
+  // rows [0, L - 4*hop): the last utterance's 4*hop gap rows would read frames past the end and no fold reads them
+  rc = frames_or_rows(u, mel_frames, aux_frames, expanded, pl.L, pl.L - 4ll * u.hop, bj->regions + n_floats, st, j);
+  if (rc != WRNN_OK) return rc;
+  h->last = bj->e;
   return WRNN_OK;
+}
+
+// wrnn_vocode_many's job (layout: cond::batch_plan): batch_job with the per-fold Philox keys and the epilogue's
+// utterance table as its table and the sample block as its region.  A live job refuses an engine without live
+// vocoding and has no device epilogue.  `b` holds DEVICE mel pointers (and DEVICE wav pointers unless live).
+static int vocode_many_job(wrnn_t* h, const wrnn_vocode_batch* b, const cond::BatchPlan& pl, cudaStream_t st, bool live,
+                           VocodeJob* v) {
+  const int hop = h->upsampler->hop, n = b->n_utts;
+  const size_t nf = (size_t)pl.g.n_seg, b_key = align256(nf * sizeof(FoldKey));
+  std::vector<const float*> mels(n);
+  for (int i = 0; i < n; ++i) mels[i] = b->utts[i].mel;
+  BatchJob bj;
+  int rc = batch_job(h, pl, mels.data(), b_key + n * sizeof(EpUtt), align_floats(nf * pl.g.seg_len), st, &bj,
+                     [&](const Engine& e, unsigned char* tab) -> int {
+                       if (live && e.live_refusal()) { set_error(e.live_refusal()); return WRNN_E_INVALID; }
+                       std::memcpy(tab, pl.keys.data(), nf * sizeof(FoldKey));
+                       EpUtt* eu = reinterpret_cast<EpUtt*>(tab + b_key);
+                       for (int i = 0; i < n; ++i)
+                         eu[i] = EpUtt{pl.fold0[i], (int)(pl.fold0[i + 1] - pl.fold0[i]), (b->utts[i].T - 1) * hop, b->utts[i].wav};
+                       return WRNN_OK;
+                     });
+  if (rc != WRNN_OK) return rc;
+  v->j = bj.j;
+  v->j.out = bj.regions;
+  v->g = pl.g;
+  v->e = bj.e;
+  v->keys = reinterpret_cast<const FoldKey*>(bj.tab);
+  v->eu = reinterpret_cast<const EpUtt*>(bj.tab + b_key);
+  return live ? WRNN_OK : epilogue_tables(h, (int)pl.g.overlap, b->mu_law, st, &v->tabs);
 }
 
 static int vocode_many(wrnn_t* h, const wrnn_vocode_batch* b, const cond::BatchPlan& pl, cudaStream_t st) {
@@ -567,71 +643,28 @@ __global__ void score_scatter_kernel(const ScoreUtt* __restrict__ u, int n_utts,
 }
 
 static int score_many(wrnn_t* h, const wrnn_score_utt* utts, int n, const cond::BatchPlan& pl, cudaStream_t st) {
-  Upsampler& u = *h->upsampler;
-  const int hop = u.hop;
-  const size_t steps = (size_t)pl.g.seg_len;
-  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
-
-  wrnn_job j;
-  std::memset(&j, 0, sizeof(j));
-  j.L = pl.L; j.seg_stride = pl.g.seg_stride; j.n_seg = n; j.seg_len = (int32_t)steps;
-  j.hop = hop; j.cond_mode = WRNN_COND_AUTO;
-  const void* tag = h->upsampler;                      // placeholders: only tested against NULL
-  j.fold_row0 = j.fold_row_end = static_cast<const int64_t*>(tag);
-  Engine* e = nullptr;
-  bool expanded = false;
-  int rc = pick_vocode_engine(h, j, &e, &expanded);
+  const long long steps = pl.g.seg_len;
+  const size_t n_xf = align_floats((size_t)steps * n);
+  std::vector<const float*> mels(n);
+  for (int i = 0; i < n; ++i) mels[i] = utts[i].mel;
+  BatchJob bj;
+  int rc = batch_job(h, pl, mels.data(), n * sizeof(ScoreUtt), 2 * n_xf, st, &bj, [&](const Engine& e, unsigned char* tab) -> int {
+    if (!e.scores()) { set_error(kNoRawStreamScore); return WRNN_E_INVALID; }
+    ScoreUtt* su = reinterpret_cast<ScoreUtt*>(tab);
+    for (int i = 0; i < n; ++i) su[i] = ScoreUtt{utts[i].x, utts[i].nll, utts[i].n};
+    return WRNN_OK;
+  });
   if (rc != WRNN_OK) return rc;
-  if (!e->scores()) { set_error(kNoRawStreamScore); return WRNN_E_INVALID; }
-
-  // scratch: [row0 | row_end | CondUtt table | ScoreUtt table | mel_frames | aux_frames | x_force | nll | expanded rows]
-  const size_t n_frames = (size_t)pl.frame0.back();
-  const size_t b_row = align_floats(2 * (size_t)n) * 4;
-  const size_t b_cu = align_floats(n * sizeof(CondUtt) / 4 + 1) * 4, b_su = align_floats(n * sizeof(ScoreUtt) / 4 + 1) * 4;
-  const size_t b_tab = 2 * b_row + b_cu + b_su;
-  const size_t n_mf = align_floats(n_frames * FEAT), n_af = align_floats(n_frames * cond::CD), n_xf = align_floats(steps * n);
-  const size_t n_rows = expanded ? align_floats((size_t)pl.L * FEAT) + align_floats((size_t)pl.L * 4 * AUXD) : 0;
-  rc = grow(&u.d_scratch, &u.scratch_bytes, b_tab + (n_mf + n_af + 2 * n_xf + n_rows) * sizeof(float));
-  if (rc != WRNN_OK) return rc;
-  unsigned char* d = static_cast<unsigned char*>(u.d_scratch);
-  float* mel_frames = reinterpret_cast<float*>(d + b_tab);
-  float* aux_frames = mel_frames + n_mf;
-  float* xf = aux_frames + n_af;
+  // regions: [x_force | nll]
+  const ScoreUtt* d_su = reinterpret_cast<const ScoreUtt*>(bj.tab);
+  float* xf = bj.regions;
   float* nl = xf + n_xf;
-
-  u.host_plan.assign(b_tab, 0);
-  unsigned char* hp = u.host_plan.data();
-  std::memcpy(hp, pl.row0.data(), n * 8);
-  std::memcpy(hp + b_row, pl.row_end.data(), n * 8);
-  CondUtt* cu = reinterpret_cast<CondUtt*>(hp + 2 * b_row);
-  ScoreUtt* su = reinterpret_cast<ScoreUtt*>(hp + 2 * b_row + b_cu);
-  for (int i = 0; i < n; ++i) {
-    cu[i] = CondUtt{utts[i].mel, utts[i].T, pl.frame0[i]};
-    su[i] = ScoreUtt{utts[i].x, utts[i].nll, utts[i].n};
-  }
-  WRNN_CUDA_OK(cudaMemcpyAsync(d, hp, b_tab, cudaMemcpyHostToDevice, st));
-  j.fold_row0 = reinterpret_cast<const int64_t*>(d);
-  j.fold_row_end = reinterpret_cast<const int64_t*>(d + b_row);
-  const CondUtt* d_cu = reinterpret_cast<const CondUtt*>(d + 2 * b_row);
-  const ScoreUtt* d_su = reinterpret_cast<const ScoreUtt*>(d + 2 * b_row + b_cu);
-
-  if ((rc = conditioning_frames_batch(u, d_cu, n, pl.max_T, mel_frames, aux_frames, st)) != WRNN_OK) return rc;
-  if (expanded) {
-    // rows [0, L - 4*hop): the last utterance's 4*hop gap rows would read frames past the end and no fold reads them
-    float* mels_up = nl + n_xf;
-    float* aux = mels_up + align_floats((size_t)pl.L * FEAT);
-    if ((rc = expand_conditioning(mel_frames, aux_frames, u.d_taps, hop, 0, pl.L - 4ll * hop, mels_up, aux, st)) != WRNN_OK) return rc;
-    j.mels_up = mels_up; j.aux = aux;
-  } else {
-    j.mel_frames = mel_frames; j.aux_frames = aux_frames; j.up_taps = u.d_taps;
-  }
-  const int grid = grid_stride_blocks(((long long)steps * n + 255) / 256);
-  score_gather_kernel<<<grid, 256, 0, st>>>(d_su, n, (long long)steps, xf);
+  const int grid = grid_stride_blocks((steps * n + 255) / 256);
+  score_gather_kernel<<<grid, 256, 0, st>>>(d_su, n, steps, xf);
   WRNN_CUDA_OK(cudaGetLastError());
-  j.x_force = xf;
-  h->last = e;
-  if ((rc = e->score(j, nl, st, nullptr)) != WRNN_OK) return rc;
-  score_scatter_kernel<<<grid, 256, 0, st>>>(d_su, n, (long long)steps, nl);
+  bj.j.x_force = xf;
+  if ((rc = bj.e->score(bj.j, nl, st, nullptr)) != WRNN_OK) return rc;
+  score_scatter_kernel<<<grid, 256, 0, st>>>(d_su, n, steps, nl);
   WRNN_CUDA_OK(cudaGetLastError());
   return WRNN_OK;
 }
@@ -664,19 +697,13 @@ int wrnn_vocode_host(wrnn_t* h, const wrnn_vocode_job* job) {
   if (rc != WRNN_OK) return rc;
   rc = validate_vocode(h, job);
   if (rc != WRNN_OK) return rc;
-  Upsampler& u = *h->upsampler;
-  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
-  const size_t n_mel = align_floats((size_t)job->T * FEAT), n_wav = (size_t)(job->T - 1) * u.hop;
-  if ((rc = grow(&u.d_stage, &u.stage_bytes, n_mel * sizeof(float) + n_wav * sizeof(double))) != WRNN_OK) return rc;
-  float* d_mel = static_cast<float*>(u.d_stage);
-  double* d_wav = reinterpret_cast<double*>(d_mel + n_mel);
-  WRNN_CUDA_OK(cudaMemcpyAsync(d_mel, job->mel, (size_t)job->T * FEAT * sizeof(float), cudaMemcpyHostToDevice, 0));
+  const size_t b_wav = (size_t)(job->T - 1) * h->upsampler->hop * sizeof(double);
+  std::vector<void*> d;
+  if ((rc = stage(h, {{job->mel, (size_t)job->T * FEAT * sizeof(float)}, {nullptr, b_wav}}, 0, d)) != WRNN_OK) return rc;
   wrnn_vocode_job dj = *job;
-  dj.mel = d_mel; dj.wav = d_wav;
+  dj.mel = static_cast<float*>(d[0]); dj.wav = static_cast<double*>(d[1]);
   if ((rc = vocode(h, &dj, 0)) != WRNN_OK) return rc;
-  WRNN_CUDA_OK(cudaMemcpyAsync(job->wav, d_wav, n_wav * sizeof(double), cudaMemcpyDeviceToHost, 0));
-  WRNN_CUDA_OK(cudaStreamSynchronize(0));
-  return h->last->check();
+  return unstage(h, {{job->wav, dj.wav, b_wav}});
 }
 
 int wrnn_vocode_many(wrnn_t* h, const wrnn_vocode_batch* b, void* stream) {
@@ -694,29 +721,25 @@ int wrnn_vocode_many_host(wrnn_t* h, const wrnn_vocode_batch* b) {
   if (rc != WRNN_OK) return rc;
   rc = validate_many(h, b, pl);
   if (rc != WRNN_OK) return rc;
-  Upsampler& u = *h->upsampler;
-  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
   const int n = b->n_utts;
-  std::vector<size_t> mel_off(n + 1, 0);
-  for (int i = 0; i < n; ++i) mel_off[i + 1] = mel_off[i] + align_floats((size_t)b->utts[i].T * FEAT);
-  const size_t n_wav = (size_t)pl.wav0.back();
-  if ((rc = grow(&u.d_stage, &u.stage_bytes, mel_off[n] * sizeof(float) + n_wav * sizeof(double))) != WRNN_OK) return rc;
-  float* d_mel = static_cast<float*>(u.d_stage);
-  double* d_wav = reinterpret_cast<double*>(d_mel + mel_off[n]);
-  std::vector<wrnn_utterance> du(b->utts, b->utts + n);
+  std::vector<Staged> in(2 * n);                       // [mels | waveforms]
   for (int i = 0; i < n; ++i) {
-    WRNN_CUDA_OK(cudaMemcpyAsync(d_mel + mel_off[i], b->utts[i].mel, (size_t)b->utts[i].T * FEAT * sizeof(float), cudaMemcpyHostToDevice, 0));
-    du[i].mel = d_mel + mel_off[i];
-    du[i].wav = d_wav + pl.wav0[i];
+    in[i] = {b->utts[i].mel, (size_t)b->utts[i].T * FEAT * sizeof(float)};
+    in[n + i] = {nullptr, (size_t)(pl.wav0[i + 1] - pl.wav0[i]) * sizeof(double)};
+  }
+  std::vector<void*> d;
+  if ((rc = stage(h, in, 0, d)) != WRNN_OK) return rc;
+  std::vector<wrnn_utterance> du(b->utts, b->utts + n);
+  std::vector<Unstaged> out(n);
+  for (int i = 0; i < n; ++i) {
+    du[i].mel = static_cast<float*>(d[i]);
+    du[i].wav = static_cast<double*>(d[n + i]);
+    out[i] = {b->utts[i].wav, d[n + i], in[n + i].bytes};
   }
   wrnn_vocode_batch db = *b;
   db.utts = du.data();
   if ((rc = vocode_many(h, &db, pl, 0)) != WRNN_OK) return rc;
-  for (int i = 0; i < n; ++i)
-    WRNN_CUDA_OK(cudaMemcpyAsync(b->utts[i].wav, d_wav + pl.wav0[i], (size_t)(pl.wav0[i + 1] - pl.wav0[i]) * sizeof(double),
-                                 cudaMemcpyDeviceToHost, 0));
-  WRNN_CUDA_OK(cudaStreamSynchronize(0));
-  return h->last->check();
+  return unstage(h, out);
 }
 
 int wrnn_score_many(wrnn_t* h, const wrnn_score_utt* utts, int32_t n_utts, void* stream) {
@@ -734,29 +757,23 @@ int wrnn_score_many_host(wrnn_t* h, const wrnn_score_utt* utts, int32_t n_utts) 
   if (rc != WRNN_OK) return rc;
   rc = validate_score_many(h, utts, n_utts, pl);
   if (rc != WRNN_OK) return rc;
-  Upsampler& u = *h->upsampler;
-  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
   const int n = n_utts;
-  std::vector<size_t> mel_off(n + 1, 0), x_off(n + 1, 0);
+  std::vector<Staged> in(3 * n);                       // [mels | waveforms | losses]
   for (int i = 0; i < n; ++i) {
-    mel_off[i + 1] = mel_off[i] + align_floats((size_t)utts[i].T * FEAT);
-    x_off[i + 1] = x_off[i] + align_floats((size_t)utts[i].n);
+    in[i] = {utts[i].mel, (size_t)utts[i].T * FEAT * sizeof(float)};
+    in[n + i] = {utts[i].x, (size_t)utts[i].n * sizeof(float)};
+    in[2 * n + i] = {nullptr, (size_t)utts[i].n * sizeof(float)};
   }
-  if ((rc = grow(&u.d_stage, &u.stage_bytes, (mel_off[n] + 2 * x_off[n]) * sizeof(float))) != WRNN_OK) return rc;
-  float* d_mel = static_cast<float*>(u.d_stage);
-  float* d_x = d_mel + mel_off[n];
-  float* d_nll = d_x + x_off[n];
+  std::vector<void*> d;
+  if ((rc = stage(h, in, 0, d)) != WRNN_OK) return rc;
   std::vector<wrnn_score_utt> du(utts, utts + n);
+  std::vector<Unstaged> out(n);
   for (int i = 0; i < n; ++i) {
-    WRNN_CUDA_OK(cudaMemcpyAsync(d_mel + mel_off[i], utts[i].mel, (size_t)utts[i].T * FEAT * sizeof(float), cudaMemcpyHostToDevice, 0));
-    WRNN_CUDA_OK(cudaMemcpyAsync(d_x + x_off[i], utts[i].x, (size_t)utts[i].n * sizeof(float), cudaMemcpyHostToDevice, 0));
-    du[i].mel = d_mel + mel_off[i]; du[i].x = d_x + x_off[i]; du[i].nll = d_nll + x_off[i];
+    du[i].mel = static_cast<float*>(d[i]); du[i].x = static_cast<float*>(d[n + i]); du[i].nll = static_cast<float*>(d[2 * n + i]);
+    out[i] = {utts[i].nll, du[i].nll, in[2 * n + i].bytes};
   }
   if ((rc = score_many(h, du.data(), n, pl, 0)) != WRNN_OK) return rc;
-  for (int i = 0; i < n; ++i)
-    WRNN_CUDA_OK(cudaMemcpyAsync(utts[i].nll, d_nll + x_off[i], (size_t)utts[i].n * sizeof(float), cudaMemcpyDeviceToHost, 0));
-  WRNN_CUDA_OK(cudaStreamSynchronize(0));
-  return h->last->check();
+  return unstage(h, out);
 }
 
 }  // extern "C"
@@ -770,44 +787,52 @@ int wrnn_score_many_host(wrnn_t* h, const wrnn_score_utt* utts, int32_t n_utts) 
 // wrnn_epilogue_kernel in the unbatched geometry, on the host: samples [n0, n1) of x -> wav.  The same operations in the
 // same order: the mu-law label recovered in fp32 and rounded half to even (saturating, NaN -> 0, then clamped), 0.0 + y
 // (a -0.0 sample becomes +0.0), then the fade-out over the last tail_len samples.
-static void live_epilogue(const float* x, long long n0, long long n1, long long wave_len, long long tail_len, const double* mu,
-                          int nc, const double* tail, double* wav) {
+static void live_epilogue(const LiveTables& t, const float* x, long long n0, long long n1, long long wave_len, double* wav) {
+  const int nc = t.n_classes;
   for (long long n = n0; n < n1; ++n) {
     const float xf = x[n];
     double y = (double)xf;
-    if (mu) {
+    if (!t.mu.empty()) {
       const float r = std::nearbyint((xf + 1.0f) * (0.5f * (float)(nc - 1)));
-      y = mu[!(r > 0.f) ? 0 : (r >= (float)(nc - 1) ? nc - 1 : (int)r)];
+      y = t.mu[!(r > 0.f) ? 0 : (r >= (float)(nc - 1) ? nc - 1 : (int)r)];
     }
     double v = 0.0 + y;
-    if (n >= wave_len - tail_len) v *= tail[n - (wave_len - tail_len)];
+    if (n >= wave_len - t.tail_len) v *= t.tail[n - (wave_len - t.tail_len)];
     wav[n] = v;
   }
 }
 
-static int live_grow(LiveJob& lj, size_t want) {
-  if (want <= lj.bytes) return WRNN_OK;
-  if (lj.host) cudaFreeHost(lj.host);
-  lj.host = lj.dev = nullptr; lj.bytes = 0;
-  WRNN_CUDA_OK(cudaHostAlloc(&lj.host, want, cudaHostAllocMapped));
-  WRNN_CUDA_OK(cudaHostGetDevicePointer(&lj.dev, lj.host, 0));
-  lj.bytes = want;
-  return WRNN_OK;
+// One utterance's delivery, for both kinds of live job: its samples [delivered, min(count, wave_len)) of x, count being
+// what its fold has published, through live_epilogue into wav.  Returns whether any were delivered.
+static bool live_deliver_one(const LiveTables& t, const float* x, long long count, long long wave_len, long long& delivered,
+                             double* wav) {
+  const long long ready = count < wave_len ? count : wave_len;
+  if (ready <= delivered) return false;
+  live_epilogue(t, x, delivered, ready, wave_len, wav);
+  delivered = ready;
+  return true;
+}
+
+// Calls f until it returns a value, sleeping in short intervals in between (a few hundred steps of the kernel each), for
+// at most wait_us in all (no limit when wait_us < 0).  Returns f's value, or nothing at the deadline.
+template <class F>
+static std::optional<int> wait_for(long long wait_us, F f) {
+  const auto end = std::chrono::steady_clock::now() + std::chrono::microseconds(wait_us);
+  const std::chrono::steady_clock::duration interval = std::chrono::microseconds(100);
+  for (;;) {
+    if (const std::optional<int> r = f()) return r;
+    const auto left = wait_us < 0 ? interval : end - std::chrono::steady_clock::now();
+    if (left <= left.zero()) return std::nullopt;
+    std::this_thread::sleep_for(std::min(left, interval));
+  }
 }
 
 // Delivers, per utterance, the samples its fold has published so far (at most its wave_len) into the caller's wav.
 // Returns whether any utterance received samples.
 static bool live_deliver(LiveJob& lj) {
   bool more = false;
-  for (int i = 0; i < lj.n(); ++i) {
-    const unsigned long long p = lj.progress(i);
-    const long long ready = (long long)p < lj.wave_len[i] ? (long long)p : lj.wave_len[i];
-    if (ready <= lj.delivered[i]) continue;
-    live_epilogue(lj.samples(i), lj.delivered[i], ready, lj.wave_len[i], lj.tail_len, lj.mu.empty() ? nullptr : lj.mu.data(),
-                  lj.n_classes, lj.tail.data(), lj.wav[i]);
-    lj.delivered[i] = ready;
-    more = true;
-  }
+  for (int i = 0; i < lj.n(); ++i)
+    more = live_deliver_one(lj.tabs, lj.samples(i), (long long)lj.progress(i), lj.wave_len[i], lj.delivered[i], lj.wav[i]) || more;
   return more;
 }
 
@@ -819,7 +844,7 @@ static int live_launch(wrnn_t* h, VocodeJob& v, bool many, bool mu_law, const st
   LiveJob& lj = *h->live;
   const int n = (int)wav.size(), hop = h->upsampler->hop;
   const long long steps = v.j.seg_len;
-  int rc = live_grow(lj, LiveJob::SAMPLES_OFF + (size_t)n * steps * sizeof(float));
+  int rc = grow_mapped(&lj.host, &lj.dev, &lj.bytes, LiveJob::SAMPLES_OFF + (size_t)n * steps * sizeof(float));
   if (rc != WRNN_OK) return rc;
   for (int i = 0; i < n; ++i)                                   // no kernel of this handle runs
     __atomic_store_n(static_cast<unsigned long long*>(lj.host) + i, 0ull, __ATOMIC_RELEASE);
@@ -828,13 +853,10 @@ static int live_launch(wrnn_t* h, VocodeJob& v, bool many, bool mu_law, const st
   if ((rc = v.e->generate_live(v.j, st, v.keys, static_cast<unsigned long long*>(lj.dev))) != WRNN_OK) return rc;
   WRNN_CUDA_OK(cudaEventRecord(lj.done, st));
 
-  std::vector<double> fi, fo;
-  cond::epilogue_tables(0, mu_law, h->engine->cfg.n_classes, hop, fi, fo, lj.mu, lj.tail);
+  lj.tabs = live_tables(h->engine->cfg.mode, mu_law, h->engine->cfg.n_classes, hop);
   lj.e = v.e;
   lj.many = many;
   lj.steps = steps;
-  lj.tail_len = 20ll * hop;
-  lj.n_classes = h->engine->cfg.n_classes;
   lj.wav = wav;
   lj.wave_len.resize(n);
   for (int i = 0; i < n; ++i) lj.wave_len[i] = (T[i] - 1) * hop;
@@ -858,10 +880,7 @@ static int live_poll(wrnn_t* h, int32_t wait_us, bool many, int64_t* n_ready) {
                    : "the live job in flight was started by wrnn_vocode_many_live_start: poll it with wrnn_vocode_many_live_poll");
     return WRNN_E_INVALID;
   }
-  auto report = [&] { for (int i = 0; i < lj.n(); ++i) n_ready[i] = lj.delivered[i]; };
-  const auto t0 = std::chrono::steady_clock::now();
-  const auto wait = std::chrono::microseconds(wait_us > 0 ? wait_us : 0);
-  for (;;) {
+  const std::optional<int> rc = wait_for(wait_us > 0 ? wait_us : 0, [&]() -> std::optional<int> {
     const cudaError_t q = cudaEventQuery(lj.done);
     if (q == cudaSuccess) {                            // the kernel has finished: every sample is published
       h->live_busy = false;
@@ -875,24 +894,17 @@ static int live_poll(wrnn_t* h, int32_t wait_us, bool many, int64_t* n_ready) {
             rc = WRNN_E_CUDA;
           }
       }
-      report();
       return rc;
     }
     if (q != cudaErrorNotReady) {
       h->live_busy = false;
-      report();
       set_error(std::string("live job: ") + cudaGetErrorString(q));
       return WRNN_E_CUDA;
     }
-    const bool more = live_deliver(lj);
-    const auto left = wait - (std::chrono::steady_clock::now() - t0);
-    if (more || left <= std::chrono::microseconds(0)) {
-      report();
-      return 1;
-    }
-    // sleep in short intervals: a few hundred steps of the kernel each
-    std::this_thread::sleep_for(std::min<std::chrono::steady_clock::duration>(left, std::chrono::microseconds(100)));
-  }
+    return live_deliver(lj) ? std::optional<int>(1) : std::nullopt;
+  });
+  for (int i = 0; i < lj.n(); ++i) n_ready[i] = lj.delivered[i];
+  return rc ? *rc : 1;
 }
 
 // Both live starts, after their own refusals (b is unbatched, of 1 to 64 utterances with mel, wav and T >= 21): the
@@ -902,21 +914,18 @@ static int live_start(wrnn_t* h, const wrnn_vocode_batch* b, bool many, cudaStre
   if (rc != WRNN_OK) return rc;
   cond::BatchPlan pl;
   if ((rc = validate_many(h, b, pl)) != WRNN_OK) return rc;
-  Upsampler& u = *h->upsampler;
-  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
 
   // the mels (host or device) into staging, so that the conditioning network reads device memory
   const int n = b->n_utts;
-  std::vector<size_t> mel_off(n + 1, 0);
-  for (int i = 0; i < n; ++i) mel_off[i + 1] = mel_off[i] + align_floats((size_t)b->utts[i].T * FEAT);
-  if ((rc = grow(&u.d_stage, &u.stage_bytes, mel_off[n] * sizeof(float))) != WRNN_OK) return rc;
-  float* d_mel = static_cast<float*>(u.d_stage);
+  std::vector<Staged> in(n);
+  for (int i = 0; i < n; ++i) in[i] = {b->utts[i].mel, (size_t)b->utts[i].T * FEAT * sizeof(float)};
+  std::vector<void*> d;
+  if ((rc = stage(h, in, st, d)) != WRNN_OK) return rc;
   std::vector<wrnn_utterance> du(b->utts, b->utts + n);
   std::vector<double*> wav(n);
   std::vector<long long> T(n);
   for (int i = 0; i < n; ++i) {
-    WRNN_CUDA_OK(cudaMemcpyAsync(d_mel + mel_off[i], b->utts[i].mel, (size_t)b->utts[i].T * FEAT * sizeof(float), cudaMemcpyDefault, st));
-    du[i].mel = d_mel + mel_off[i];
+    du[i].mel = static_cast<float*>(d[i]);
     wav[i] = b->utts[i].wav;
     T[i] = b->utts[i].T;
   }
@@ -924,7 +933,7 @@ static int live_start(wrnn_t* h, const wrnn_vocode_batch* b, bool many, cudaStre
   db.utts = du.data();
   VocodeJob v;
   if ((rc = vocode_many_job(h, &db, pl, st, true, &v)) != WRNN_OK) return rc;
-  return live_launch(h, v, many, b->mu_law && h->engine->cfg.mode == WRNN_MODE_RAW, wav, T, st);
+  return live_launch(h, v, many, b->mu_law, wav, T, st);
 }
 
 extern "C" {
@@ -936,8 +945,8 @@ int wrnn_vocode_live_start(wrnn_t* h, const wrnn_vocode_job* job, void* stream) 
               "sample is final before the whole job is");
     return WRNN_E_INVALID;
   }
-  if (!job->mel || !job->wav) { set_error("mel and wav are required"); return WRNN_E_INVALID; }
-  if (job->T < 21) { set_error("T must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples"); return WRNN_E_INVALID; }
+  const int rc = check_utterance("", job->mel, job->wav, job->T);
+  if (rc != WRNN_OK) return rc;
   // the batch of one utterance: the same fold, keyed (philox_seed, 0), as wrnn_vocode's unbatched job
   const wrnn_utterance u{job->mel, job->T, job->philox_seed, job->wav};
   const wrnn_vocode_batch b{&u, 1, 0, 0, 0, job->mu_law};
@@ -960,12 +969,9 @@ int wrnn_vocode_many_live_start(wrnn_t* h, const wrnn_vocode_batch* b, void* str
   }
   if (!b->utts) { set_error("utts is required"); return WRNN_E_INVALID; }
   for (int i = 0; i < b->n_utts; ++i) {
-    const std::string at = "utterance " + std::to_string(i) + ": ";
-    if (!b->utts[i].mel || !b->utts[i].wav) { set_error(at + "mel and wav are required"); return WRNN_E_INVALID; }
-    if (b->utts[i].T < 21) {
-      set_error(at + "T must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples");
-      return WRNN_E_INVALID;
-    }
+    const wrnn_utterance& u = b->utts[i];
+    const int rc = check_utterance("utterance " + std::to_string(i) + ": ", u.mel, u.wav, u.T);
+    if (rc != WRNN_OK) return rc;
   }
   return live_start(h, b, true, static_cast<cudaStream_t>(stream));
 }
@@ -973,15 +979,14 @@ int wrnn_vocode_many_live_start(wrnn_t* h, const wrnn_vocode_batch* b, void* str
 int wrnn_vocode_many_live_poll(wrnn_t* h, int32_t wait_us, int64_t* n_ready) { return live_poll(h, wait_us, true, n_ready); }
 
 // Test hook (CPU-only, no device needed): wrnn_vocode_live_poll's epilogue over samples x [n] (n <= wave_len) of an
-// unbatched job of wave_len samples at this hop, with the tables wrnn_vocode builds.  Checked in tests/test_live_abi.py.
+// unbatched job of wave_len samples at this hop, with the tables wrnn_vocode builds (mu_law: a RAW head's).  Checked in
+// tests/test_live_abi.py.
 int wrnn_debug_live_epilogue(const float* x, int64_t n, int64_t wave_len, int32_t hop, int32_t mu_law, int32_t n_classes,
                              double* wav) {
   if (!x || !wav || hop <= 0 || n < 0 || n > wave_len || wave_len < 20ll * hop || (mu_law && n_classes < 2)) {
     set_error("bad argument"); return WRNN_E_INVALID;
   }
-  std::vector<double> fi, fo, mu, tail;
-  cond::epilogue_tables(0, mu_law != 0, n_classes, hop, fi, fo, mu, tail);
-  live_epilogue(x, 0, n, wave_len, 20ll * hop, mu_law ? mu.data() : nullptr, n_classes, tail.data(), wav);
+  live_epilogue(live_tables(WRNN_MODE_RAW, mu_law != 0, n_classes, hop), x, 0, n, wave_len, wav);
   return WRNN_OK;
 }
 
@@ -1003,10 +1008,7 @@ int wrnn_debug_live_many_deliver(const float* x, int64_t steps, const uint64_t* 
   LiveJob lj;
   lj.host = buf.data();
   lj.steps = steps;
-  lj.tail_len = 20ll * hop;
-  lj.n_classes = n_classes;
-  std::vector<double> fi, fo;
-  cond::epilogue_tables(0, mu_law != 0, n_classes, hop, fi, fo, lj.mu, lj.tail);
+  lj.tabs = live_tables(WRNN_MODE_RAW, mu_law != 0, n_classes, hop);
   double* w = wav;
   for (int i = 0; i < n_utts; ++i) {
     lj.wav.push_back(w);
@@ -1039,17 +1041,8 @@ int wrnn_debug_stream_plan(const wrnn_cfg* cfg, const wrnn_weights* w, uint8_t* 
     return WRNN_E_INVALID;
   }
   HostWeights hw;
-  hw.n_classes = cfg->n_classes;
-  const size_t W2W = H + AUXD;
-  auto take = [&](std::vector<float>& dst, const float* src, size_t n) { dst.assign(src, src + n); };
-  take(hw.I_w, w->I_weight, (size_t)H * (1 + F1IN)); take(hw.I_b, w->I_bias, H);
-  take(hw.w1i, w->rnn1_weight_ih, (size_t)G3 * H); take(hw.w1h, w->rnn1_weight_hh, (size_t)G3 * H);
-  take(hw.b1i, w->rnn1_bias_ih, G3); take(hw.b1h, w->rnn1_bias_hh, G3);
-  take(hw.w2i, w->rnn2_weight_ih, (size_t)G3 * W2W); take(hw.w2h, w->rnn2_weight_hh, (size_t)G3 * H);
-  take(hw.b2i, w->rnn2_bias_ih, G3); take(hw.b2h, w->rnn2_bias_hh, G3);
-  take(hw.f1w, w->fc1_weight, (size_t)H * W2W); take(hw.f1b, w->fc1_bias, H);
-  take(hw.f2w, w->fc2_weight, (size_t)H * W2W); take(hw.f2b, w->fc2_bias, H);
-  take(hw.f3w, w->fc3_weight, (size_t)cfg->n_classes * H); take(hw.f3b, w->fc3_bias, cfg->n_classes);
+  const int rc = read_weights(*cfg, *w, true, hw);
+  if (rc != WRNN_OK) return rc;
   stream::Plan plan;
   stream::build_plan(hw, cfg->precision == WRNN_PREC_BF16, plan, only_block);
   if (blob) {
@@ -1097,9 +1090,9 @@ struct LiveSession {
     bool cancelled = false;
     cudaEvent_t ready = nullptr;     // the slot's conditioning frames are complete
   };
-  int C = 0, hop = 0, n_classes = 0;
-  long long max_T = 0, max_steps = 0, tail_len = 0;
-  std::vector<double> mu, tail;      // the epilogue tables (mu empty without mu_law)
+  int C = 0, hop = 0;
+  long long max_T = 0, max_steps = 0;
+  LiveTables tabs;
   Engine* e = nullptr;
   cudaStream_t st = nullptr, side = nullptr;
   void* host = nullptr; void* dev = nullptr;         // pinned, mapped
@@ -1138,13 +1131,7 @@ static bool session_deliver(LiveSession& ss) {
     const unsigned long long w = __atomic_load_n(ss.progress() + s, __ATOMIC_ACQUIRE);
     if ((unsigned)(w >> 32) != sl.tag) continue;
     const long long count = (long long)(w & (SES_RETIRED - 1u));
-    const long long ready = count < sl.wave_len ? count : sl.wave_len;
-    if (ready > sl.delivered && !sl.cancelled) {
-      live_epilogue(ss.samples(s), sl.delivered, ready, sl.wave_len, ss.tail_len, ss.mu.empty() ? nullptr : ss.mu.data(),
-                    ss.n_classes, ss.tail.data(), sl.wav);
-      sl.delivered = ready;
-      more = true;
-    }
+    if (!sl.cancelled && live_deliver_one(ss.tabs, ss.samples(s), count, sl.wave_len, sl.delivered, sl.wav)) more = true;
     if (w & SES_RETIRED) { ss.release(sl); more = true; }
   }
   return more;
@@ -1237,9 +1224,10 @@ int wrnn_live_open(wrnn_t* h, int32_t capacity, int64_t max_T, int32_t mu_law, v
   if (capacity < 1 || capacity > LiveSession::MAX_SLOTS) {
     set_error("a live session holds 1 to 64 slots: one persistent tile holds 64 folds"); return WRNN_E_INVALID;
   }
-  if (max_T < 21) { set_error("max_T must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples"); return WRNN_E_INVALID; }
+  int rc = check_frames("max_T", max_T);
+  if (rc != WRNN_OK) return rc;
   if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
-  int rc = idle_or_busy(h);
+  rc = idle_or_busy(h);
   if (rc != WRNN_OK) return rc;
   if (!h->upsampler) { set_error("no upsampler attached (wrnn_attach_upsampler)"); return WRNN_E_INVALID; }
   if (h->engine->live_refusal()) { set_error(h->engine->live_refusal()); return WRNN_E_INVALID; }
@@ -1250,18 +1238,16 @@ int wrnn_live_open(wrnn_t* h, int32_t capacity, int64_t max_T, int32_t mu_law, v
   LiveSession* ss = new (std::nothrow) LiveSession();
   if (!ss) { set_error("out of host memory"); return WRNN_E_INVALID; }
   ss->C = capacity; ss->hop = hop; ss->max_T = max_T; ss->max_steps = (max_T - 1) * hop;
-  ss->n_classes = h->engine->cfg.n_classes; ss->tail_len = 20ll * hop;
+  ss->tabs = live_tables(h->engine->cfg.mode, mu_law != 0, h->engine->cfg.n_classes, hop);
   ss->e = h->engine; ss->st = static_cast<cudaStream_t>(stream); ss->taps = h->upsampler->d_taps;
   ss->slots.resize(capacity);
   ss->tab.assign(2 * LiveSession::MAX_SLOTS, SesEntry{0, 0, 0ull});
-  std::vector<double> fi, fo;
-  cond::epilogue_tables(0, mu_law && h->engine->cfg.mode == WRNN_MODE_RAW, ss->n_classes, hop, fi, fo, ss->mu, ss->tail);
   auto fail = [&](int code) { session_free(ss); return code; };
 #define SES_OK(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { set_error(std::string(#expr) + " failed: " + cudaGetErrorString(_e)); return fail(WRNN_E_CUDA); } } while (0)
   SES_OK(cudaSetDevice(h->engine->device));
-  const size_t host_bytes = LiveSession::SAMPLES_OFF + (size_t)capacity * ss->max_steps * sizeof(float);
-  SES_OK(cudaHostAlloc(&ss->host, host_bytes, cudaHostAllocMapped));
-  SES_OK(cudaHostGetDevicePointer(&ss->dev, ss->host, 0));
+  size_t host_bytes = 0;
+  rc = grow_mapped(&ss->host, &ss->dev, &host_bytes, LiveSession::SAMPLES_OFF + (size_t)capacity * ss->max_steps * sizeof(float));
+  if (rc != WRNN_OK) return fail(rc);
   std::memset(ss->host, 0, LiveSession::SAMPLES_OFF);
   SES_OK(cudaMalloc(&ss->d_ctl, 2 * LiveSession::MAX_SLOTS * sizeof(SesEntry) + 64));
   const size_t rf = (size_t)(max_T + 4) * capacity;
@@ -1281,13 +1267,13 @@ int wrnn_live_open(wrnn_t* h, int32_t capacity, int64_t max_T, int32_t mu_law, v
 
 int wrnn_live_submit(wrnn_t* h, const wrnn_utterance* u, int64_t* ticket) {
   if (!u || !ticket) { set_error("null utterance or ticket"); return WRNN_E_INVALID; }
-  if (!u->mel || !u->wav) { set_error("mel and wav are required"); return WRNN_E_INVALID; }
-  if (u->T < 21) { set_error("T must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples"); return WRNN_E_INVALID; }
+  int rc = check_utterance("", u->mel, u->wav, u->T);
+  if (rc != WRNN_OK) return rc;
   if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
   if (!h->session) { set_error("no live session is open on this handle (wrnn_live_open)"); return WRNN_E_INVALID; }
   LiveSession& ss = *h->session;
   if (u->T > ss.max_T) { set_error("T exceeds the session's max_T (" + std::to_string(ss.max_T) + ")"); return WRNN_E_INVALID; }
-  int rc = session_pump(ss);                           // releases what has finished, so that its slot can be reused
+  rc = session_pump(ss);                               // releases what has finished, so that its slot can be reused
   if (rc != WRNN_OK) return rc;
   session_deliver(ss);
   int s = 0;
@@ -1341,16 +1327,12 @@ int wrnn_live_poll(wrnn_t* h, int32_t wait_us, wrnn_live_ticket* out, int32_t ma
   LiveSession& ss = *h->session;
   if (max_out < 2 * ss.C) { set_error("max_out must be at least twice the session's capacity"); return WRNN_E_INVALID; }
   *n_out = 0;
-  const auto t0 = std::chrono::steady_clock::now();
-  const auto wait = std::chrono::microseconds(wait_us > 0 ? wait_us : 0);
-  for (;;) {
-    int rc = session_pump(ss);
-    if (rc != WRNN_OK) return rc;
-    bool more = session_deliver(ss) || !ss.released.empty();
-    const auto left = wait - (std::chrono::steady_clock::now() - t0);
-    if (more || left <= std::chrono::microseconds(0)) break;
-    std::this_thread::sleep_for(std::min<std::chrono::steady_clock::duration>(left, std::chrono::microseconds(100)));
-  }
+  const std::optional<int> rc = wait_for(wait_us > 0 ? wait_us : 0, [&]() -> std::optional<int> {
+    const int rc = session_pump(ss);
+    if (rc != WRNN_OK || session_deliver(ss) || !ss.released.empty()) return rc;
+    return std::nullopt;
+  });
+  if (rc && *rc != WRNN_OK) return *rc;
   // released tickets first, then every ticket still held (at most C)
   int n = 0, held = 0;
   size_t k = 0;
@@ -1373,18 +1355,17 @@ int wrnn_live_close(wrnn_t* h) {
     LiveSession::Slot& sl = ss->slots[s];
     if (sl.state != LiveSession::FREE && !sl.cancelled) wrnn_live_cancel(h, sl.ticket);
   }
-  int rc = WRNN_OK;
-  for (;;) {                                           // the launch stops once every cancelled slot is retired
-    if ((rc = session_pump(*ss)) != WRNN_OK) break;
+  const std::optional<int> rc = wait_for(-1, [&]() -> std::optional<int> {   // the launch stops once every cancelled slot is retired
+    const int rc = session_pump(*ss);
+    if (rc != WRNN_OK) return rc;
     session_deliver(*ss);
     bool held = false;
     for (const auto& sl : ss->slots) held = held || sl.state != LiveSession::FREE;
-    if (!held && !ss->running) break;
-    std::this_thread::sleep_for(std::chrono::microseconds(100));
-  }
+    return (!held && !ss->running) ? std::optional<int>(WRNN_OK) : std::nullopt;
+  });
   h->session = nullptr;
   session_free(ss);
-  return rc;
+  return *rc;
 }
 
 // Test hook (CPU-only, no device needed): one delivery of wrnn_live_poll on a host buffer laid out as the session's
@@ -1407,9 +1388,8 @@ int wrnn_debug_live_session_deliver(const float* x, int64_t max_steps, const uin
   std::memcpy(buf.data() + LiveSession::SAMPLES_OFF, x, (size_t)C * max_steps * sizeof(float));
   LiveSession ss;
   ss.host = buf.data();
-  ss.C = C; ss.hop = hop; ss.max_steps = max_steps; ss.tail_len = 20ll * hop; ss.n_classes = n_classes;
-  std::vector<double> fi, fo;
-  cond::epilogue_tables(0, mu_law != 0, n_classes, hop, fi, fo, ss.mu, ss.tail);
+  ss.C = C; ss.hop = hop; ss.max_steps = max_steps;
+  ss.tabs = live_tables(WRNN_MODE_RAW, mu_law != 0, n_classes, hop);
   ss.slots.resize(C);
   double* w = wav;
   for (int s = 0; s < C; ++s) {

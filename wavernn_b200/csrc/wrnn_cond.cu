@@ -347,8 +347,8 @@ int batch_plan(int hop, const wrnn_vocode_batch& b, BatchPlan& out) {
   for (int i = 0; i < b.n_utts; ++i) {
     const wrnn_utterance& u = b.utts[i];
     const std::string at = "utterance " + std::to_string(i) + ": ";
-    if (!u.mel || !u.wav) { set_error(at + "mel and wav are required"); return WRNN_E_INVALID; }
-    if (u.T < 21) { set_error(at + "T must be >= 21 mel frames: the fade-out spans the last 20 hops of the (T-1)*hop samples"); return WRNN_E_INVALID; }
+    const int rc = check_utterance(at, u.mel, u.wav, u.T);
+    if (rc != WRNN_OK) return rc;
     if (u.T >= (1ll << 31) / hop) { set_error(at + "stream longer than 2^31 samples"); return WRNN_E_INVALID; }
     out.frame0.push_back(frames); out.wav0.push_back(waves);
     frames += u.T + 4; waves += (u.T - 1) * hop;
@@ -447,7 +447,6 @@ Upsampler::~Upsampler() {
   if (d_taps) cudaFree(d_taps);
   if (d_scratch) cudaFree(d_scratch);
   if (d_tabs) cudaFree(d_tabs);
-  if (d_stage) cudaFree(d_stage);
   cudaSetDevice(prev);
 }
 

@@ -76,13 +76,10 @@ struct Upsampler {
   void* d_scratch = nullptr;
   size_t scratch_bytes = 0;
   std::vector<double> host_tabs;        // [fade_in | fade_out | mu | tail], kept alive for the asynchronous upload
-  std::vector<unsigned char> host_plan; // wrnn_vocode_many: fold tables, keys and utterance tables, uploaded in one copy
+  std::vector<unsigned char> host_plan; // a batch job's fold tables and utterance tables, uploaded in one copy
   double* d_tabs = nullptr;
   size_t tabs_len = 0;
   long long tabs_key[3] = {-1, -1, -1}; // overlap, mu_law, n_classes of the tables in d_tabs
-  // wrnn_vocode_host staging
-  void* d_stage = nullptr;
-  size_t stage_bytes = 0;
   ~Upsampler();
 };
 

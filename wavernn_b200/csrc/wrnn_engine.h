@@ -155,7 +155,7 @@ struct wrnn_handle {
   wrnn::HostWeights* host_weights = nullptr;
   bool auto_engine = false;
   bool stream_failed = false;
-  // staging for wrnn_generate_host
+  // staging of the host-memory entry points (wrnn_generate_host, wrnn_vocode_host, ..., and a live start's mels)
   void* d_stage = nullptr;
   size_t stage_bytes = 0;
   // wrnn_attach_upsampler: folded MelResNet, tap table and the scratch of wrnn_vocode
@@ -171,4 +171,8 @@ struct wrnn_handle {
 namespace wrnn {
 // WRNN_E_BUSY with its message while a live job is in flight on h, else WRNN_OK (every entry point but the live poll)
 int idle_or_busy(const wrnn_handle* h);
+// The rule of every vocoded utterance: T >= 21 mel frames, the fade-out spanning the last 20 hops.  `name` is what the
+// message calls T.  check_utterance also requires mel and wav; `at` prefixes its messages ("utterance i: " or "").
+int check_frames(const std::string& name, long long T);
+int check_utterance(const std::string& at, const void* mel, const void* wav, long long T);
 }  // namespace wrnn
