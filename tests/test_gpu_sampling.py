@@ -32,16 +32,27 @@ FORMS = {
     "tc-small": ("tcgen05", "fp16", 5, None, None),       # one tile of <= 24 folds
     "tc-big": ("tcgen05", "fp16", 40, None, None),        # one BIG tile (25 .. 64 folds)
     "tc-tiles": ("tcgen05", "fp16", 70, None, None),      # tiles of 64 + 6 folds
+    "tc-small-bf16": ("tcgen05", "bf16", 5, None, None),
+    "tc-big-bf16": ("tcgen05", "bf16", 40, None, None),
+    "tc-tiles-bf16": ("tcgen05", "bf16", 70, None, None),
     "stream-16x1": ("stream", "fp16", 40, "16", "1"),
     "stream-16x4": ("stream", "fp16", 40, "16", "4"),
     "stream-32x1": ("stream", "fp16", 40, "32", "1"),
     "stream-32x4": ("stream", "fp16", 40, "32", "4"),
+    "stream-32x4-bf16": ("stream", "bf16", 40, "32", "4"),
     "simt-fp16": ("simt", "fp16", 40, None, None),
     "simt-fp32": ("simt", "fp32", 40, None, None),
     "simt-bf16": ("simt", "bf16", 40, None, None),
 }
 MOL_FORMS = list(FORMS)
 RAW_FORMS = [f for f in FORMS if not f.startswith("stream")]     # the stream engine has no RAW head
+
+
+def engine_name(form):
+    """The name the engine of `form` reports."""
+    engine, precision, _, _, cl = FORMS[form]
+    return {"tcgen05": f"tcgen05-{precision}", "simt": f"simt-{precision}",
+            "stream": f"tcgen05-stream-x4-{precision}" if cl == "4" else f"tcgen05-stream-{precision}"}[engine]
 
 
 class Runner:
@@ -79,11 +90,7 @@ class Runner:
                           stream=torch.cuda.current_stream(dev).cuda_stream)
         torch.cuda.synchronize(dev)
         self.eng.check()
-        name = self.eng.name
-        engine, precision, _, _, cl = FORMS[self.form]
-        want = {"tcgen05": f"tcgen05-{precision}", "simt": f"simt-{precision}",
-                "stream": f"tcgen05-stream-x4-{precision}" if cl == "4" else f"tcgen05-stream-{precision}"}[engine]
-        assert name == want, (self.form, name)
+        assert self.eng.name == engine_name(self.form), (self.form, self.eng.name)
         res, lgs = out.cpu().numpy(), lg.cpu().numpy()
         assert not np.isnan(res).any() and not np.isnan(lgs).any(), "outputs left unwritten"
         return res, lgs

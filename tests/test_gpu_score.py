@@ -3,13 +3,15 @@
   1. The same chains as generation: wrnn_score's logits_out is bit-identical to wrnn_generate's with the same x_force,
      on every scoring instantiation (persistent fp16 | bf16 x MoL | RAW x rows | FRAMES x small | BIG tile; stream fp16 |
      bf16 x rows | FRAMES x 16 | 32 folds x 1 | 4 CTAs, MoL; SIMT fp32 | fp16 | bf16 x MoL | RAW), on the jobs of
-     tests/kernel_jobs.py; rows of nll at and past `steps` stay untouched.
+     tests/kernel_jobs.py (persistent also at 73 folds over two launches, SIMT at 73 folds in three tiles); rows of nll
+     at and past `steps` stay untouched.
   2. The loss arithmetic: nll against tests/score_oracle.py evaluated on that run's own logits, within its tolerance.
   3. Against the reference: the SIMT fp32 engine against tests/golden/score_pins.npz (b) and (c), within bounds derived
      on the CPU (tests/test_score_abi.py).
   4. Mel level: wrnn_score_many equals, bit for bit, each utterance alone, wrnn_score fed wrnn_conditioning_frames'
-     tensors, the host entry and the permuted batch, on fixed-engine handles; an AUTO handle sends 257 utterances to the
-     stream engine.
+     tensors, the host entry and the permuted batch, on fixed-engine handles; 70 recordings on a persistent handle (two
+     launches) equal the host entry and, at both ends of each launch, themselves alone; an AUTO handle sends 257
+     utterances to the stream engine.
   5. Quality on the H100: the shipped checkpoint on the Tacotron fixture at fp16 / bf16 on both tensor-core engines
      against SIMT fp32 (median, mean, share of samples moved by > 1 nat), pinned against the same statistics of the
      CPU emulation's logits at each precision.
@@ -30,9 +32,11 @@ from wavernn_b200 import cabi
 pytestmark = pytest.mark.gpu
 
 PRECISIONS, HEADS = ("fp16", "bf16"), ("MOL", "RAW")
-PERSISTENT = [(p, h, fr, big) for p in PRECISIONS for h in HEADS for fr in (False, True) for big in (False, True)]
+# tile sizes: the last small tile, the first BIG tile, a 64-fold BIG tile then a 9-fold small one over two launches
+TILES = {"small": K.SMALL_TILE, "big": K.SMALL_TILE + 1, "tiles": 73}
+PERSISTENT = [(p, h, fr, size) for p in PRECISIONS for h in HEADS for fr in (False, True) for size in TILES]
 STREAM = [(p, fr, nf, cl) for p in PRECISIONS for fr in (False, True) for nf in (16, 32) for cl in (1, 4)]
-SIMT = [(p, h) for p in ("fp32", "fp16", "bf16") for h in HEADS]
+SIMT = [(p, h, n) for n in (K.SMALL_TILE, 73) for p in ("fp32", "fp16", "bf16") for h in HEADS]   # 73: three tiles
 # SIMT fp32 against the reference's own loss (score_pins.npz (b), (c)): tests/test_score_abi.py asserts each is at least
 # 4 x the largest gap between the fp32 CPU emulation + score_oracle and the fixture.
 from test_score_abi import RAND_TOL, TRAINED_TOL  # noqa: E402
@@ -142,13 +146,15 @@ def check_scoring(eng, job, frames, form=None, what=""):
     assert (d <= tol).all(), (what, float((d / tol).max()), "worst sample", i, float(y[i]), float(nll.reshape(-1)[i]), float(want[i]))
 
 
-@pytest.mark.parametrize("precision,head,frames,big", PERSISTENT,
-                         ids=[f"tc-{p}-{h}-{'frames' if fr else 'rows'}-{'big' if big else 'small'}" for p, h, fr, big in PERSISTENT])
-def test_persistent_scoring(st, precision, head, frames, big):
+@pytest.mark.parametrize("precision,head,frames,size", PERSISTENT,
+                         ids=[f"tc-{p}-{h}-{'frames' if fr else 'rows'}-{size}" for p, h, fr, size in PERSISTENT])
+def test_persistent_scoring(st, precision, head, frames, size):
     eng = st.engine("tcgen05", precision, head)
-    job = st.job(K.SMALL_TILE + (1 if big else 0), head, frames)
-    check_scoring(eng, job, frames, what=f"tc-{precision}-{head}-{'frames' if frames else 'rows'}-{'big' if big else 'small'}")
+    job = st.job(TILES[size], head, frames)
+    n0 = eng.launch_count
+    check_scoring(eng, job, frames, what=f"tc-{precision}-{head}-{'frames' if frames else 'rows'}-{size}")
     assert eng.name.startswith("tcgen05-")
+    assert eng.launch_count - n0 == 2 * -(-TILES[size] // 64)          # generation and scoring, 64 folds per launch
 
 
 @pytest.mark.parametrize("precision,frames,nf,cl", STREAM,
@@ -160,10 +166,10 @@ def test_stream_scoring(st, precision, frames, nf, cl):
     assert ("-x4-" in eng.name) == (cl == 4)
 
 
-@pytest.mark.parametrize("precision,head", SIMT, ids=[f"simt-{p}-{h}" for p, h in SIMT])
-def test_simt_scoring(st, precision, head):
+@pytest.mark.parametrize("precision,head,n", SIMT, ids=[f"simt-{p}-{h}" + ("-tiles" if n == 73 else "") for p, h, n in SIMT])
+def test_simt_scoring(st, precision, head, n):
     eng = st.engine("simt", precision, head)
-    check_scoring(eng, st.job(K.SMALL_TILE, head, False), False, what=f"simt-{precision}-{head}")
+    check_scoring(eng, st.job(n, head, False), False, what=f"simt-{precision}-{head}" + ("-tiles" if n == 73 else ""))
 
 
 def test_stream_refuses_raw_scoring(st):
@@ -338,6 +344,35 @@ def test_score_many(st, head, engine, precision):
         assert all(np.array_equal(pb[k], batch[i]) for k, i in enumerate(perm)), (name, "permuted")
         print(f"score_many {head} [{name}]: {len(mels)} utterances bit-identical alone / frames / host / permuted; "
               f"mean nll {[float(b.mean()) for b in batch]}")
+    finally:
+        eng.close()
+
+
+MANY = [("MOL", "fp16"), ("RAW", "bf16")]
+
+
+@pytest.mark.parametrize("head,precision", MANY, ids=[f"{h}-{p}" for h, p in MANY])
+def test_score_many_70_recordings_on_the_persistent_engine(st, head, precision):
+    """70 recordings on a fixed persistent handle: a 64-fold launch, then 6 folds.  The batch equals the host entry, and
+    the recordings at both ends of each launch equal themselves scored alone."""
+    m = st.model(head)[0]
+    eng = cabi.Engine(m.hot_state(), n_classes=m.n_classes, mode=head, precision=precision, engine="tcgen05")
+    try:
+        eng.attach_upsampler(m.state_dict())
+        Ts = [2 + i % 4 for i in range(70)]
+        mels, xs = utterances(head, Ts, [T * 275 - 13 * (i % 7) for i, T in enumerate(Ts)], seed=3)
+        n0 = eng.launch_count
+        batch = score_many_device(eng, mels, xs)
+        launches = eng.launch_count - n0
+        assert eng.name == f"tcgen05-{precision}" and launches == 2, (eng.name, launches)
+        assert all(np.isfinite(b).all() for b in batch)
+        host = eng.score_many_host(mels, xs)
+        assert all(np.array_equal(a, b) for a, b in zip(host, batch)), (eng.name, "host")
+        for i in (0, 63, 64, 69):
+            alone = score_many_device(eng, [mels[i]], [xs[i]])[0]
+            assert np.array_equal(alone, batch[i]), (eng.name, i, "alone")
+        print(f"score_many {head} [{eng.name}]: 70 recordings in {launches} launches, bit-identical to the host entry and "
+              f"recordings 0, 63, 64, 69 alone")
     finally:
         eng.close()
 
