@@ -456,6 +456,69 @@ int wrnn_score_many(wrnn_t *h, const wrnn_score_utt *utts, int32_t n_utts, void 
 /* The same with HOST mel / x / nll: copies in, runs, copies out, synchronises and returns wrnn_check's verdict. */
 int wrnn_score_many_host(wrnn_t *h, const wrnn_score_utt *utts, int32_t n_utts);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * Mel analysis: the reference's melspectrogram(y) (utils/dsp.py:72-81: librosa 0.6.3 STFT -> Slaney mel filterbank ->
+ * amp_to_db -> normalize) on the device, so that a recording can be analysed, vocoded again or scored without librosa.
+ * An analysis object needs no weights.  Per frame: the reflect-padded samples (np.pad(y, n_fft / 2, 'reflect')) times
+ * the periodic Hann window of win_length centred in n_fft, a float64 real FFT, each bin rounded to complex64 as
+ * librosa's stft(dtype=np.complex64) stores it, its magnitude, the band sums with the float64 filterbank, then
+ * clip((20 log10(max(1e-5, M)) - min_level_db) / -min_level_db, 0, 1) stored as float32 (DESIGN.md §3.8).
+ * --------------------------------------------------------------------------------------------------------------- */
+typedef struct {
+  int32_t sample_rate;   /* 22050; > 0                                             */
+  int32_t n_fft;         /* 2048; a power of two, 256..4096                        */
+  int32_t hop_length;    /* 275; >= 1                                              */
+  int32_t win_length;    /* 1100; 1..n_fft                                         */
+  int32_t n_mels;        /* 80; 1..128                                             */
+  float fmin;            /* 40; 0 <= fmin < sample_rate / 2                        */
+  float min_level_db;    /* -100; < 0                                              */
+} wrnn_mel_cfg;          /* the hparams fields utils/dsp.py reads; fmax is sample_rate / 2 as in linear_to_mel */
+
+typedef struct wrnn_mel_plan wrnn_mel_t;
+
+/* Builds the tables once, in float64 on the host (window, twiddles, Slaney filterbank with Slaney norm and each band's
+ * nonzero bin range: librosa 0.6.3 filters.mel(sr, n_fft, n_mels, fmin), htk=False, norm=1) and uploads them to
+ * `device`.  A configuration outside the ranges above is refused (WRNN_E_INVALID, with a message) before the device is
+ * looked at.  An analysis object has no busy state: any number of calls may use it at once, on any streams. */
+int wrnn_mel_create(wrnn_mel_t **out, const wrnn_mel_cfg *cfg, int device);
+void wrnn_mel_destroy(wrnn_mel_t *m);
+
+typedef struct {
+  const float *y;        /* [n] waveform, float32 as librosa.load returns it                             */
+  int64_t n;             /* > n_fft / 2 (one reflection of the centre padding)                           */
+  float *mel;            /* [n_mels, 1 + n / hop_length], the layout of the reference's mel .npy          */
+} wrnn_mel_utt;
+
+/* Every frame of every utterance in one kernel launch.  Each utterance's mel is bit-identical to its own call.
+ * Refused (WRNN_E_INVALID): a null m or u, n_utts < 1, a null y or mel, n_i <= n_fft / 2 (the message names i), a
+ * batch of 2^31 frames or more.  DEVICE pointers; asynchronous on `stream`. */
+int wrnn_melspectrogram_many(const wrnn_mel_t *m, const wrnn_mel_utt *u, int32_t n_utts, void *stream);
+/* The same with HOST y / mel: copies in, runs, copies out and synchronises. */
+int wrnn_melspectrogram_many_host(const wrnn_mel_t *m, const wrnn_mel_utt *u, int32_t n_utts);
+
+/* Scoring a recording from its audio alone: what preprocess.py:36-47 and utils/dataset.py:86-91 do, on the device.
+ *   1. y /= max|y| (float32) when peak_norm is set or the peak exceeds 1;
+ *   2. mel = the analysis of that y by `m` (T = 1 + n / hop frames, so T * hop >= n);
+ *   3. the stored labels, evaluated in float32: MoL trunc(clip((y + 1) * 65535 / 2, 0, 65535)); RAW with mu_law
+ *      encode_mu_law(y, n_classes); RAW without it trunc(float_2_label(y, bits)); mapped back with label_2_float;
+ *   4. wrnn_score_many's job on {mel, those targets}.
+ * Contract: nll is bit-identical to wrnn_score_many on the same handle given the mel wrnn_melspectrogram_many makes of
+ * the normalised y and those targets.  mu_law is wrnn_vocode_job::mu_law, a property of the training data that the
+ * handle does not know; the MoL head ignores it.
+ * Refused (WRNN_E_INVALID, the handle stays usable): those of wrnn_score_many; a null m; m->n_mels != feat_dims, or
+ * m->hop_length other than the attached upsampler's hop_length, or m on another device (the message names both);
+ * any n_i <= n_fft / 2 (the message names i).  Busy rules are the handle's.  DEVICE y / nll; asynchronous. */
+typedef struct {
+  const float *y;        /* [n] the recording, float32                                        */
+  int64_t n;             /* samples, > n_fft / 2                                               */
+  float *nll;            /* [n] per-sample loss in nats                                        */
+} wrnn_score_wav_utt;
+int wrnn_score_wav_many(wrnn_t *h, const wrnn_mel_t *m, const wrnn_score_wav_utt *u, int32_t n_utts, int32_t peak_norm,
+                        int32_t mu_law, void *stream);
+/* The same with HOST y / nll: copies in, runs, copies out, synchronises and returns wrnn_check's verdict. */
+int wrnn_score_wav_many_host(wrnn_t *h, const wrnn_mel_t *m, const wrnn_score_wav_utt *u, int32_t n_utts,
+                             int32_t peak_norm, int32_t mu_law);
+
 /* Host helper for parity mode: replays torch's default CPU generator (MT19937) natively, so the
  * draws the reference makes before / inside its loop cost a few ms instead of ~30.
  *   state : the generator's 624 words and its position `pos` in [0, 624] (624 = block exhausted)

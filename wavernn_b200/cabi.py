@@ -26,7 +26,8 @@ EXPORTS = ("wrnn_abi_version", "wrnn_last_error", "wrnn_create", "wrnn_destroy",
            "wrnn_vocode_many", "wrnn_vocode_many_host", "wrnn_score", "wrnn_score_many", "wrnn_score_many_host",
            "wrnn_vocode_live_start", "wrnn_vocode_live_poll", "wrnn_vocode_many_live_start",
            "wrnn_vocode_many_live_poll", "wrnn_live_open", "wrnn_live_submit", "wrnn_live_cancel", "wrnn_live_poll",
-           "wrnn_live_close")
+           "wrnn_live_close", "wrnn_mel_create", "wrnn_mel_destroy", "wrnn_melspectrogram_many",
+           "wrnn_melspectrogram_many_host", "wrnn_score_wav_many", "wrnn_score_wav_many_host")
 LIVE_RUNNING, LIVE_DONE, LIVE_CANCELLED = 0, 1, 2
 
 _fp = C.POINTER(C.c_float)
@@ -92,6 +93,33 @@ class WrnnLiveTicket(C.Structure):
 
 class WrnnScoreUtt(C.Structure):
     _fields_ = [("mel", C.c_void_p), ("T", C.c_int64), ("x", C.c_void_p), ("n", C.c_int64), ("nll", C.c_void_p)]
+
+
+class WrnnMelCfg(C.Structure):
+    _fields_ = [("sample_rate", C.c_int32), ("n_fft", C.c_int32), ("hop_length", C.c_int32), ("win_length", C.c_int32),
+                ("n_mels", C.c_int32), ("fmin", C.c_float), ("min_level_db", C.c_float)]
+
+
+class WrnnMelUtt(C.Structure):
+    _fields_ = [("y", C.c_void_p), ("n", C.c_int64), ("mel", C.c_void_p)]
+
+
+class WrnnScoreWavUtt(C.Structure):
+    _fields_ = [("y", C.c_void_p), ("n", C.c_int64), ("nll", C.c_void_p)]
+
+
+def mel_cfg(*, sample_rate=22050, n_fft=2048, hop_length=275, win_length=1100, n_mels=80, fmin=40.0,
+            min_level_db=-100.0) -> WrnnMelCfg:
+    """A wrnn_mel_cfg; the defaults are the reference's hparams."""
+    return WrnnMelCfg(int(sample_rate), int(n_fft), int(hop_length), int(win_length), int(n_mels), float(fmin),
+                      float(min_level_db))
+
+
+def ptr_n_ptr_array(struct, items):
+    """A wrnn_mel_utt or wrnn_score_wav_utt array over `items`, a list of (address, n, address) (0 = NULL).  Returns
+    the array and its length (an empty list gives a NULL array)."""
+    arr = (struct * max(len(items), 1))(*[struct(a or None, int(n), b or None) for a, n, b in items])
+    return (arr if items else None), len(items)
 
 
 def score_utts(utts):
@@ -193,7 +221,35 @@ def load() -> C.CDLL:
     lib.wrnn_live_poll.argtypes = [C.c_void_p, C.c_int32, C.POINTER(WrnnLiveTicket), C.c_int32, C.POINTER(C.c_int32)]
     lib.wrnn_live_close.restype = C.c_int
     lib.wrnn_live_close.argtypes = [C.c_void_p]
+    lib.wrnn_mel_create.restype = C.c_int
+    lib.wrnn_mel_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(WrnnMelCfg), C.c_int]
+    lib.wrnn_mel_destroy.restype = None
+    lib.wrnn_mel_destroy.argtypes = [C.c_void_p]
+    lib.wrnn_melspectrogram_many.restype = C.c_int
+    lib.wrnn_melspectrogram_many.argtypes = [C.c_void_p, C.POINTER(WrnnMelUtt), C.c_int32, C.c_void_p]
+    lib.wrnn_melspectrogram_many_host.restype = C.c_int
+    lib.wrnn_melspectrogram_many_host.argtypes = [C.c_void_p, C.POINTER(WrnnMelUtt), C.c_int32]
+    lib.wrnn_score_wav_many.restype = C.c_int
+    lib.wrnn_score_wav_many.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(WrnnScoreWavUtt), C.c_int32, C.c_int32, C.c_int32,
+                                        C.c_void_p]
+    lib.wrnn_score_wav_many_host.restype = C.c_int
+    lib.wrnn_score_wav_many_host.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(WrnnScoreWavUtt), C.c_int32, C.c_int32,
+                                             C.c_int32]
     # test hooks (not declared in the header)
+    lib.wrnn_debug_mel_tables.restype = C.c_int
+    lib.wrnn_debug_mel_tables.argtypes = [C.POINTER(WrnnMelCfg), C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.wrnn_debug_mel_plan.restype = C.c_int
+    lib.wrnn_debug_mel_plan.argtypes = [C.POINTER(WrnnMelCfg), C.POINTER(WrnnMelUtt), C.c_int32, C.c_void_p]
+    lib.wrnn_debug_mel_frames.restype = C.c_int
+    lib.wrnn_debug_mel_frames.argtypes = [C.POINTER(WrnnMelCfg), C.c_void_p, C.c_int64, C.c_void_p]
+    lib.wrnn_debug_score_wav_plan.restype = C.c_int
+    lib.wrnn_debug_score_wav_plan.argtypes = [C.c_int32, C.c_int32, C.POINTER(WrnnMelCfg), C.POINTER(WrnnScoreWavUtt),
+                                              C.c_int32, C.c_void_p]
+    lib.wrnn_debug_wav_targets.restype = C.c_int
+    lib.wrnn_debug_wav_targets.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
+    lib.wrnn_debug_score_wav_targets.restype = C.c_int
+    lib.wrnn_debug_score_wav_targets.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.wrnn_debug_live_session_deliver.restype = C.c_int
     lib.wrnn_debug_live_session_deliver.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                                     C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -459,6 +515,25 @@ class Engine:
         _check(self.lib, self.lib.wrnn_score_many_host(self._h, arr, n))
         return nlls
 
+    def score_wav_many(self, analysis: "MelAnalysis", *, ys, ns, nlls, peak_norm: bool = False, mu_law: bool = False,
+                       stream: int = 0):
+        """wrnn_score_wav_many with raw device addresses: recording i is ys[i] [ns[i]] fp32 -> nlls[i] [ns[i]], its mel
+        made by `analysis` and its targets quantised as preprocess.py stores them.  Asynchronous."""
+        arr, n = ptr_n_ptr_array(WrnnScoreWavUtt, list(zip(ys, ns, nlls)))
+        _check(self.lib, self.lib.wrnn_score_wav_many(self._h, analysis._m, arr, n, int(bool(peak_norm)), int(bool(mu_law)),
+                                                      C.c_void_p(stream or None)))
+
+    def score_wav_many_host(self, analysis: "MelAnalysis", ys, *, peak_norm: bool = False, mu_law: bool = False):
+        """wrnn_score_wav_many_host: a list of numpy recordings (float32) -> the list of per-sample losses (nats,
+        float32): the loss train_wavernn.py would report on each recording, from its audio alone."""
+        import numpy as np
+        ys = [np.ascontiguousarray(y, dtype=np.float32).reshape(-1) for y in ys]
+        nlls = [np.empty(y.size, dtype=np.float32) for y in ys]
+        arr, n = ptr_n_ptr_array(WrnnScoreWavUtt, [(y.ctypes.data, y.size, o.ctypes.data) for y, o in zip(ys, nlls)])
+        _check(self.lib, self.lib.wrnn_score_wav_many_host(self._h, analysis._m, arr, n, int(bool(peak_norm)),
+                                                           int(bool(mu_law))))
+        return nlls
+
     def check(self):
         _check(self.lib, self.lib.wrnn_check(self._h))
 
@@ -466,6 +541,47 @@ class Engine:
         if self._h:
             self.lib.wrnn_destroy(self._h)
             self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class MelAnalysis:
+    """Owns one `wrnn_mel_t*`: the reference's melspectrogram(y) on the device, for the wrnn_mel_cfg built from the
+    keyword arguments (cabi.mel_cfg; defaults are the reference's hparams)."""
+
+    def __init__(self, *, device: int = 0, **cfg):
+        self._m = C.c_void_p()
+        self.lib = load()
+        self.cfg = mel_cfg(**cfg)
+        _check(self.lib, self.lib.wrnn_mel_create(C.byref(self._m), C.byref(self.cfg), int(device)))
+
+    def frames(self, n: int) -> int:
+        """Frames of the mel of n samples: 1 + n // hop_length."""
+        return 1 + int(n) // self.cfg.hop_length
+
+    def melspectrogram_many(self, *, ys, ns, mels, stream: int = 0):
+        """wrnn_melspectrogram_many with raw device addresses: ys[i] [ns[i]] fp32 -> mels[i] [n_mels, frames(ns[i])].
+        Asynchronous."""
+        arr, n = ptr_n_ptr_array(WrnnMelUtt, list(zip(ys, ns, mels)))
+        _check(self.lib, self.lib.wrnn_melspectrogram_many(self._m, arr, n, C.c_void_p(stream or None)))
+
+    def melspectrogram_many_host(self, ys):
+        """wrnn_melspectrogram_many_host: a list of numpy waveforms -> the list of float32 mels [n_mels, T_i]."""
+        import numpy as np
+        ys = [np.ascontiguousarray(y, dtype=np.float32).reshape(-1) for y in ys]
+        mels = [np.empty((self.cfg.n_mels, self.frames(y.size)), dtype=np.float32) for y in ys]
+        arr, n = ptr_n_ptr_array(WrnnMelUtt, [(y.ctypes.data, y.size, m.ctypes.data) for y, m in zip(ys, mels)])
+        _check(self.lib, self.lib.wrnn_melspectrogram_many_host(self._m, arr, n))
+        return mels
+
+    def close(self):
+        if self._m:
+            self.lib.wrnn_mel_destroy(self._m)
+            self._m = C.c_void_p()
 
     def __del__(self):
         try:

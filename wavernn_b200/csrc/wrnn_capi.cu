@@ -13,6 +13,7 @@
 
 #include "wrnn_cond.h"
 #include "wrnn_engine.h"
+#include "wrnn_mel.h"
 #include "wrnn_stream_plan.h"
 
 namespace wrnn {
@@ -273,6 +274,7 @@ void wrnn_destroy(wrnn_t* h) {
     delete h->live;
   }
   if (h->d_stage) cudaFree(h->d_stage);
+  if (h->d_audio) cudaFree(h->d_audio);
   delete h->engine;
   delete h->fallback;
   delete h->stream;
@@ -774,6 +776,236 @@ int wrnn_score_many_host(wrnn_t* h, const wrnn_score_utt* utts, int32_t n_utts) 
   }
   if ((rc = score_many(h, du.data(), n, pl, 0)) != WRNN_OK) return rc;
   return unstage(h, out);
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------------------------------
+// wrnn_score_wav_many: preprocess.py:36-47 and utils/dataset.py:86-91 on the device, then wrnn_score_many's job.
+// ---------------------------------------------------------------------------------------------------------------------
+// A float32 product that is never contracted into an FMA with the addition after it (numpy rounds both).
+__host__ __device__ inline float mul_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+// The stored label of sample y (float32, as numpy 1.22 evaluates preprocess.py) mapped back to the float target with
+// label_2_float (float32, as torch evaluates dataset.py).  Logarithms are the correctly rounded float of the double
+// logarithm, so the host and the device agree.
+__host__ __device__ inline float wav_target(float y, int mode, int n_classes, bool mu_law) {
+  const int bits = mode == WRNN_MODE_MOL ? 16 : (int)log2((double)n_classes);
+  const float top = (float)((1 << bits) - 1);
+  float label;
+  if (mode == WRNN_MODE_RAW && mu_law) {                 // encode_mu_law(y, 2^bits)
+    const float mu = top;
+    const float s = y > 0.f ? 1.f : (y < 0.f ? -1.f : 0.f);
+    const float fx = s * (float)log((double)(1.f + mul_rn(mu, fabsf(y)))) / (float)log((double)(1 << bits));
+    label = floorf(mul_rn((fx + 1.f) / 2.f, mu) + 0.5f);
+  } else {                                               // trunc(float_2_label(y, bits))
+    const float v = (y + 1.f) * top / 2.f;
+    label = truncf(v < 0.f ? 0.f : (v > top ? top : v));
+  }
+  return 2.f * label / top - 1.f;
+}
+
+struct WavUtt {
+  const float* y;
+  long long n;
+  float* yn;      // the normalised recording
+  float* x;       // its targets
+};
+
+// One block per recording: max |y|.
+__global__ void wav_peak_kernel(const WavUtt* __restrict__ u, float* __restrict__ peak) {
+  __shared__ float red[256];
+  const WavUtt w = u[blockIdx.x];
+  float p = 0.f;
+  for (long long i = threadIdx.x; i < w.n; i += blockDim.x) p = fmaxf(p, fabsf(__ldg(w.y + i)));
+  red[threadIdx.x] = p;
+  __syncthreads();
+  for (int s = blockDim.x / 2; s > 0; s >>= 1) {
+    if ((int)threadIdx.x < s) red[threadIdx.x] = fmaxf(red[threadIdx.x], red[threadIdx.x + s]);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) peak[blockIdx.x] = red[0];
+}
+
+// Recording blockIdx.y: y / peak when peak_norm is set or the peak exceeds 1, and the targets of that y.
+__global__ void wav_targets_kernel(const WavUtt* __restrict__ u, const float* __restrict__ peak, int peak_norm, int mode,
+                                   int n_classes, int mu_law) {
+  const WavUtt w = u[blockIdx.y];
+  const float p = peak[blockIdx.y];
+  const bool norm = peak_norm || p > 1.f;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < w.n; i += (long long)gridDim.x * blockDim.x) {
+    float y = __ldg(w.y + i);
+    if (norm) y = y / p;
+    w.yn[i] = y;
+    w.x[i] = wav_target(y, mode, n_classes, mu_law != 0);
+  }
+}
+
+// Enqueues the peak, normalisation and target kernels over the DEVICE table `d_u` of n recordings.
+static int wav_targets(const WavUtt* d_u, int n, long long max_n, float* peak, int peak_norm, int mode, int n_classes,
+                       int mu_law, cudaStream_t st) {
+  wav_peak_kernel<<<n, 256, 0, st>>>(d_u, peak);
+  WRNN_CUDA_OK(cudaGetLastError());
+  const dim3 grid((unsigned)std::min<long long>((max_n + 255) / 256, 64), (unsigned)n);
+  wav_targets_kernel<<<grid, 256, 0, st>>>(d_u, peak, peak_norm, mode, n_classes, mu_law);
+  WRNN_CUDA_OK(cudaGetLastError());
+  return WRNN_OK;
+}
+
+// The batch's checks, on the host: the analysis against the model, each recording, then wrnn_score_many's plan of the
+// job it becomes (T_i = 1 + n_i / hop frames) and the analysis's frame table.
+static int score_wav_plan(int feat, int hop, const wrnn_mel_t* m, const wrnn_score_wav_utt* u, int n, cond::BatchPlan& pl,
+                          std::vector<int64_t>& frame0) {
+  if (!m) { set_error("null analysis object"); return WRNN_E_INVALID; }
+  if (m->cfg.n_mels != feat) {
+    set_error("the analysis makes n_mels = " + std::to_string(m->cfg.n_mels) + " bands, the model takes feat_dims = " + std::to_string(feat));
+    return WRNN_E_INVALID;
+  }
+  if (m->cfg.hop_length != hop) {
+    set_error("the analysis has hop_length " + std::to_string(m->cfg.hop_length) + ", the attached upsampler hop_length " + std::to_string(hop));
+    return WRNN_E_INVALID;
+  }
+  if (!u || n < 1 || n > 65535) return cond::score_plan(hop, nullptr, 0, pl);
+  const void* tag = m;                                 // placeholders: the plans only test these against NULL
+  std::vector<wrnn_mel_utt> mu(n);
+  std::vector<wrnn_score_utt> su(n);
+  for (int i = 0; i < n; ++i) {
+    if (!u[i].y || !u[i].nll) { set_error("utterance " + std::to_string(i) + ": y and nll are required"); return WRNN_E_INVALID; }
+    mu[i] = wrnn_mel_utt{u[i].y, u[i].n, static_cast<float*>(const_cast<void*>(tag))};
+  }
+  int rc = mel::plan(m->cfg, mu.data(), n, frame0);
+  if (rc != WRNN_OK) return rc;
+  for (int i = 0; i < n; ++i)
+    su[i] = wrnn_score_utt{static_cast<const float*>(tag), frame0[i + 1] - frame0[i], u[i].y, u[i].n, u[i].nll};
+  return cond::score_plan(hop, su.data(), n, pl);
+}
+
+static int validate_score_wav(const wrnn_t* h, const wrnn_mel_t* m, const wrnn_score_wav_utt* u, int n, cond::BatchPlan& pl,
+                              std::vector<int64_t>& frame0) {
+  if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
+  if (!h->upsampler) { set_error("no upsampler attached (wrnn_attach_upsampler)"); return WRNN_E_INVALID; }
+  if (!h->engine->scores()) { set_error(kNoRawStreamScore); return WRNN_E_INVALID; }
+  int rc = score_wav_plan(h->engine->cfg.feat_dims, h->upsampler->hop, m, u, n, pl, frame0);
+  if (rc != WRNN_OK) return rc;
+  if (m->device != h->engine->device) {
+    set_error("the analysis object is on device " + std::to_string(m->device) + ", the handle on device " + std::to_string(h->engine->device));
+    return WRNN_E_INVALID;
+  }
+  return WRNN_OK;
+}
+
+// Handle scratch d_audio: [WavUtt table | peaks | normalised recordings | mels | targets], each region 256-B aligned.
+static int score_wav_many(wrnn_t* h, const wrnn_mel_t* m, const wrnn_score_wav_utt* u, int n, int peak_norm, int mu_law,
+                          const cond::BatchPlan& pl, const std::vector<int64_t>& frame0, cudaStream_t st) {
+  const int nm = m->cfg.n_mels;
+  std::vector<size_t> off(3 * n + 3, 0);
+  off[1] = align256(n * sizeof(WavUtt));
+  off[2] = off[1] + align256(n * sizeof(float));
+  long long max_n = 0;
+  for (int k = 0; k < 3 * n; ++k) {
+    const int i = k % n;
+    const size_t floats = k / n == 1 ? (size_t)nm * (frame0[i + 1] - frame0[i]) : (size_t)u[i].n;
+    off[k + 3] = off[k + 2] + align256(floats * sizeof(float));
+    max_n = std::max<long long>(max_n, u[i].n);
+  }
+  WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
+  int rc = grow(&h->d_audio, &h->audio_bytes, off[3 * n + 2]);
+  if (rc != WRNN_OK) return rc;
+  char* d = static_cast<char*>(h->d_audio);
+  auto region = [&](int kind, int i) { return reinterpret_cast<float*>(d + off[2 + kind * n + i]); };
+  std::vector<WavUtt> wu(n);
+  std::vector<wrnn_mel_utt> mu(n);
+  std::vector<wrnn_score_utt> su(n);
+  for (int i = 0; i < n; ++i) {
+    wu[i] = WavUtt{u[i].y, u[i].n, region(0, i), region(2, i)};
+    mu[i] = wrnn_mel_utt{region(0, i), u[i].n, region(1, i)};
+    su[i] = wrnn_score_utt{region(1, i), frame0[i + 1] - frame0[i], region(2, i), u[i].n, u[i].nll};
+  }
+  WRNN_CUDA_OK(cudaMemcpyAsync(d, wu.data(), n * sizeof(WavUtt), cudaMemcpyHostToDevice, st));
+  const wrnn_cfg& c = h->engine->cfg;
+  if ((rc = wav_targets(reinterpret_cast<const WavUtt*>(d), n, max_n, reinterpret_cast<float*>(d + off[1]), peak_norm, c.mode,
+                        c.n_classes, mu_law, st)) != WRNN_OK)
+    return rc;
+  if ((rc = wrnn_melspectrogram_many(m, mu.data(), n, st)) != WRNN_OK) return rc;
+  return score_many(h, su.data(), n, pl, st);
+}
+
+extern "C" {
+
+int wrnn_score_wav_many(wrnn_t* h, const wrnn_mel_t* m, const wrnn_score_wav_utt* u, int32_t n_utts, int32_t peak_norm,
+                        int32_t mu_law, void* stream) {
+  cond::BatchPlan pl;
+  std::vector<int64_t> frame0;
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  if ((rc = validate_score_wav(h, m, u, n_utts, pl, frame0)) != WRNN_OK) return rc;
+  return score_wav_many(h, m, u, n_utts, peak_norm, mu_law, pl, frame0, static_cast<cudaStream_t>(stream));
+}
+
+int wrnn_score_wav_many_host(wrnn_t* h, const wrnn_mel_t* m, const wrnn_score_wav_utt* u, int32_t n_utts, int32_t peak_norm,
+                             int32_t mu_law) {
+  cond::BatchPlan pl;
+  std::vector<int64_t> frame0;
+  int rc = idle_or_busy(h);
+  if (rc != WRNN_OK) return rc;
+  if ((rc = validate_score_wav(h, m, u, n_utts, pl, frame0)) != WRNN_OK) return rc;
+  const int n = n_utts;
+  std::vector<Staged> in(2 * n);                       // [recordings | losses]
+  for (int i = 0; i < n; ++i) {
+    in[i] = {u[i].y, (size_t)u[i].n * sizeof(float)};
+    in[n + i] = {nullptr, (size_t)u[i].n * sizeof(float)};
+  }
+  std::vector<void*> d;
+  if ((rc = stage(h, in, 0, d)) != WRNN_OK) return rc;
+  std::vector<wrnn_score_wav_utt> du(u, u + n);
+  std::vector<Unstaged> out(n);
+  for (int i = 0; i < n; ++i) {
+    du[i].y = static_cast<float*>(d[i]); du[i].nll = static_cast<float*>(d[n + i]);
+    out[i] = {u[i].nll, du[i].nll, in[n + i].bytes};
+  }
+  if ((rc = score_wav_many(h, m, du.data(), n, peak_norm, mu_law, pl, frame0, 0)) != WRNN_OK) return rc;
+  return unstage(h, out);
+}
+
+// ---- test hooks (not declared in the header) ------------------------------------------------------------------------
+// wrnn_score_wav_many's plan without a handle: its refusals, and T_i (T [n_utts]) of the job it becomes.
+int wrnn_debug_score_wav_plan(int32_t feat_dims, int32_t hop, const wrnn_mel_cfg* cfg, const wrnn_score_wav_utt* u,
+                              int32_t n_utts, int64_t* T) {
+  int rc = mel::check_cfg(cfg);
+  if (rc != WRNN_OK) return rc;
+  wrnn_mel_plan m;
+  m.cfg = *cfg;
+  cond::BatchPlan pl;
+  std::vector<int64_t> frame0;
+  if ((rc = score_wav_plan(feat_dims, hop, &m, u, n_utts, pl, frame0)) != WRNN_OK) return rc;
+  for (int i = 0; T && i < n_utts; ++i) T[i] = frame0[i + 1] - frame0[i];
+  return WRNN_OK;
+}
+
+// The targets of each sample of y [n] (HOST), without normalisation: wav_target on the host.
+int wrnn_debug_wav_targets(const float* y, int64_t n, int32_t mode, int32_t n_classes, int32_t mu_law, float* x) {
+  for (int64_t i = 0; i < n; ++i) x[i] = wav_target(y[i], mode, n_classes, mu_law != 0);
+  return WRNN_OK;
+}
+
+// What wrnn_score_wav_many runs before the analysis, for one recording (DEVICE pointers, asynchronous on `stream`):
+// the normalised recording yn [n] and its targets x [n].  peak: one float of device scratch.
+int wrnn_debug_score_wav_targets(const float* y, int64_t n, int32_t mode, int32_t n_classes, int32_t peak_norm,
+                                 int32_t mu_law, float* yn, float* x, float* peak, void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const WavUtt w{y, n, yn, x};
+  void* d = nullptr;
+  WRNN_CUDA_OK(cudaMallocAsync(&d, sizeof(WavUtt), st));
+  WRNN_CUDA_OK(cudaMemcpyAsync(d, &w, sizeof(WavUtt), cudaMemcpyHostToDevice, st));
+  const int rc = wav_targets(static_cast<const WavUtt*>(d), 1, n, peak, peak_norm, mode, n_classes, mu_law, st);
+  if (rc != WRNN_OK) return rc;
+  WRNN_CUDA_OK(cudaFreeAsync(d, st));
+  return WRNN_OK;
 }
 
 }  // extern "C"

@@ -158,6 +158,9 @@ struct wrnn_handle {
   // staging of the host-memory entry points (wrnn_generate_host, wrnn_vocode_host, ..., and a live start's mels)
   void* d_stage = nullptr;
   size_t stage_bytes = 0;
+  // wrnn_score_wav_many: the normalised recordings, their mels and their targets
+  void* d_audio = nullptr;
+  size_t audio_bytes = 0;
   // wrnn_attach_upsampler: folded MelResNet, tap table and the scratch of wrnn_vocode
   wrnn::Upsampler* upsampler = nullptr;
   // wrnn_vocode_live_start / wrnn_vocode_many_live_start: the live job (in flight while live_busy) and its pinned, mapped

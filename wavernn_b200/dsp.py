@@ -31,6 +31,22 @@ def decode_mu_law(y, mu, from_labels=True):
     return np.sign(y) / mu * ((1 + mu) ** np.abs(y) - 1)
 
 
+_analyses = {}
+
+
+def melspectrogram(y):
+    """utils/dsp.py:melspectrogram(y) with hp's sample_rate, n_fft, hop_length, win_length, num_mels, fmin and
+    min_level_db, computed on the device (wrnn_melspectrogram_many_host; there is no CPU path): float32 [num_mels,
+    1 + len(y) // hop_length]."""
+    from . import cabi
+    key = (hp.sample_rate, hp.n_fft, hp.hop_length, hp.win_length, hp.num_mels, hp.fmin, hp.min_level_db)
+    if key not in _analyses:
+        _analyses[key] = cabi.MelAnalysis(sample_rate=hp.sample_rate, n_fft=hp.n_fft, hop_length=hp.hop_length,
+                                          win_length=hp.win_length, n_mels=hp.num_mels, fmin=hp.fmin,
+                                          min_level_db=hp.min_level_db)
+    return _analyses[key].melspectrogram_many_host([y])[0]
+
+
 def save_wav(x, path, sample_rate=None):
     """float32 wav at hp.sample_rate (utils/dsp.py:22-23 wrote through
     librosa.output.write_wav, removed in librosa>=0.8)."""
