@@ -1,6 +1,6 @@
 """wrnn_melspectrogram_many and wrnn_score_wav_many on the GPU.
 
-  1. The kernel against tests/mel_oracle.py, one absolute tolerance (test_mel_abi.MEL_TOL, at least 4 x the largest gap)
+  1. The kernel against tests/mel_oracle.py, one absolute tolerance (test_mel_abi.MEL_TOL, 2^-23: one output step)
      for every signal -- the checkpoint's vocoded speech, a 440 Hz tone, a chirp, full-scale and 1e-4 noise, digital
      silence with one click (silent frames exactly 0), the minimum length, ten minutes -- and every configuration.
   2. A batch of mixed lengths is bit-identical to each waveform analysed alone, and to the host entry.
@@ -61,7 +61,7 @@ def test_kernel_against_oracle(name):
                 silent = ref.max(axis=0) == 0
                 assert silent.sum() > 10 and (g[:, silent] == 0).all()
         print(f"{name}: max |kernel - oracle| " + ", ".join(f"{k} {v:.2e}" for k, v in worst.items()))
-        assert 4 * max(worst.values()) <= MEL_TOL, worst
+        assert max(worst.values()) <= MEL_TOL, worst
     finally:
         an.close()
 

@@ -13,9 +13,12 @@ import mel_oracle as MO
 from wavernn_b200 import cabi
 
 ROOT = helpers.GOLDEN.parent.parent
-# The kernel's tolerance against the oracle, in normalized units, for every signal and configuration: at least 4 x the
-# largest gap measured (tests/test_gpu_mel.py asserts it on the H100) and no looser than 1e-5.
-MEL_TOL = 1e-5
+# The kernel's tolerance against the oracle, in normalized units, for every signal and configuration.  Each output is
+# the float32 rounding of a float64 quantity that the kernel and the oracle both compute to about 1e-12 (rounding each
+# bin to complex64, the one rounding inside, moves a band's dB value by far less).  Outputs lie in [0, 1], where a
+# float32 step is at most 2^-24, so two such roundings differ by at most one step plus the float64 gap: 2^-23 leaves a
+# margin of one step.  tests/test_mel_edges.py holds it on every configuration of its grid; log10 in float32 misses it.
+MEL_TOL = 2.0 ** -23
 FAKE = 0x1000                      # the plan hooks only test pointers against NULL
 CONFIGS = {"default": {}, "1024-1024-256": dict(n_fft=1024, win_length=1024, hop_length=256), "n_fft4096": dict(n_fft=4096),
            "n_mels128": dict(n_mels=128), "fmin0": dict(fmin=0.0)}
@@ -92,7 +95,7 @@ def test_kernel_code_on_the_host(lib, name):
         if k == "silence_click":
             assert (got[:, ref.max(axis=0) == 0] == 0).all()
     print(f"{name}: host run of the kernel code vs oracle {worst:.3e}")
-    assert 4 * worst <= MEL_TOL
+    assert worst <= MEL_TOL
 
 
 def test_struct_layouts_match_header(tmp_path):

@@ -61,10 +61,11 @@ static std::vector<double> linspace(double start, double stop, int num) {
 
 static void build_tables(const wrnn_mel_cfg& c, HostTabs& t) {
   const int N = c.n_fft, nb = N / 2 + 1, W = c.win_length, M = c.n_mels;
-  // scipy.signal.get_window('hann', W, fftbins=True): 0.5 + 0.5 cos(linspace(-pi, pi, W + 1)[n]), centred as pad_center
+  // scipy.signal.get_window('hann', W, fftbins=True): 0.5 + 0.5 cos(linspace(-pi, pi, W + 1)[n]), centred as pad_center;
+  // a one-sample window is [1] (scipy's length guard, as torch.hann_window(1)), not the formula's 0
   t.window.assign(N, 0.0);
   const double step = 2 * M_PI / W;
-  for (int n = 0; n < W; ++n) t.window[(N - W) / 2 + n] = 0.5 + 0.5 * std::cos(n * step + -M_PI);
+  for (int n = 0; n < W; ++n) t.window[(N - W) / 2 + n] = W == 1 ? 1.0 : 0.5 + 0.5 * std::cos(n * step + -M_PI);
   t.tw.resize(N);
   for (int m = 0; m < N / 2; ++m) {
     t.tw[2 * m] = std::cos(2 * M_PI * m / N);
@@ -138,12 +139,14 @@ __host__ __device__ inline float bin_magnitude(const Tabs& tb, int k, const doub
   return (float)sqrt((double)xr * xr + (double)xi * xi);
 }
 // Band m: its float64 sum, amp_to_db and normalize, stored as float32.  20 log10(1e-5) is -100 exactly (as numpy
-// evaluates it), so a frame of digital silence is exactly 0.
+// evaluates it), so a frame of digital silence is exactly 0 at min_level_db = -100.  A NaN sum (a frame that read a
+// NaN sample) stays NaN through the floor and the clamp, as np.maximum and np.clip keep it; a band with no filter
+// weight sums nothing and keeps its silent value, where numpy's 0 x NaN would make it NaN.
 __host__ __device__ inline float band_value(const Tabs& tb, int m, const float* mag) {
   const int lo = tb.bands[3 * m], cnt = tb.bands[3 * m + 1], off = tb.bands[3 * m + 2];
   double acc = 0.0;
   for (int i = 0; i < cnt; ++i) acc += tb.basis[off + i] * (double)mag[lo + i];
-  const double S = acc > 1e-5 ? 20.0 * log10(acc) : -100.0;
+  const double S = !(acc <= 1e-5) ? 20.0 * log10(acc) : -100.0;
   const double v = (S - tb.min_level_db) / -tb.min_level_db;
   return (float)(v < 0.0 ? 0.0 : (v > 1.0 ? 1.0 : v));
 }
