@@ -117,6 +117,27 @@ __device__ __forceinline__ FoldPhilox fold_philox(const FoldKey* keys, int f, in
   }
   return FoldPhilox{(unsigned)(seg_first + f), (unsigned)seed, (unsigned)(seed >> 32)};
 }
+// the key of a live-session slot: its occupant's seed, counter fold 0
+__device__ __forceinline__ FoldPhilox slot_philox(unsigned long long seed) {
+  return FoldPhilox{0u, (unsigned)seed, (unsigned)(seed >> 32)};
+}
+// The in-kernel draws of one step of a fold, the same on every tensor-core engine.  MoL: words 0-9 (mixture) and 10
+// (logistic) of Philox blocks 0-2 at counter (step, fold, block, offset), each mapped by u_ref_range.
+__device__ __forceinline__ void mol_uniforms(const FoldPhilox& k, unsigned step, unsigned offset, float (&ur)[11]) {
+  const unsigned g = k.fold, k0 = k.k0, k1 = k.k1, o0 = offset;
+  const Philox4 r0 = philox4x32_10(step, g, 0u, o0, k0, k1), r1 = philox4x32_10(step, g, 1u, o0, k0, k1),
+                r2 = philox4x32_10(step, g, 2u, o0, k0, k1);
+  ur[0] = u_ref_range(r0.x); ur[1] = u_ref_range(r0.y); ur[2] = u_ref_range(r0.z); ur[3] = u_ref_range(r0.w);
+  ur[4] = u_ref_range(r1.x); ur[5] = u_ref_range(r1.y); ur[6] = u_ref_range(r1.z); ur[7] = u_ref_range(r1.w);
+  ur[8] = u_ref_range(r2.x); ur[9] = u_ref_range(r2.y); ur[10] = u_ref_range(r2.z);
+}
+// RAW: class c draws Exp(1) from word c % 4 of block 16 + c / 4.
+__device__ __forceinline__ Philox4 raw_block(const FoldPhilox& k, unsigned step, unsigned cls_block, unsigned offset) {
+  return philox4x32_10(step, k.fold, 16u + cls_block, offset, k.k0, k.k1);
+}
+__device__ __forceinline__ float raw_exp(const Philox4& r, unsigned word) {
+  return -logf(u01_open(word == 0 ? r.x : word == 1 ? r.y : word == 2 ? r.z : r.w));
+}
 
 // -------------------------------------------------------------------------------------
 // samplers

@@ -342,13 +342,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
           for (int i = 0; i < 10; ++i) ur[i] = __ldca(u + gf * 10 + i);
           ur[10] = __ldca(u + 10 * p.n_total + gf);
         } else {
-          const FoldPhilox k = fold_philox(p.keys, gf, p.seg_first, p.seed);
-          const unsigned gg = k.fold, k0 = k.k0, k1 = k.k1, o0 = (unsigned)p.offset;
-          const Philox4 r0 = philox4x32_10((unsigned)t, gg, 0u, o0, k0, k1), r1 = philox4x32_10((unsigned)t, gg, 1u, o0, k0, k1),
-                        r2 = philox4x32_10((unsigned)t, gg, 2u, o0, k0, k1);
-          ur[0] = u_ref_range(r0.x); ur[1] = u_ref_range(r0.y); ur[2] = u_ref_range(r0.z); ur[3] = u_ref_range(r0.w);
-          ur[4] = u_ref_range(r1.x); ur[5] = u_ref_range(r1.y); ur[6] = u_ref_range(r1.z); ur[7] = u_ref_range(r1.w);
-          ur[8] = u_ref_range(r2.x); ur[9] = u_ref_range(r2.y); ur[10] = u_ref_range(r2.z);
+          mol_uniforms(fold_philox(p.keys, gf, p.seg_first, p.seed), (unsigned)t, (unsigned)p.offset, ur);
         }
       }
 
@@ -411,7 +405,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
           publish_ready(phase == 2 ? W_Y1 : W_Y2, blk, phase == 2 ? off_y1 : off_y2);
         } else if constexpr (RAW) {
           // P5, RAW head, classes [128 blk, 128 blk + 128): logit = F3 y2 + b3, score = logit - log e with e the class's
-          // Exp(1) draw (Philox keyed as wrnn_tc.cu / wrnn_simt.cu: block 16 + class / 4, word class % 4; or `expo`);
+          // Exp(1) draw (raw_block / raw_exp: block 16 + class / 4, word class % 4; or `expo`);
           // the pick is the best score, ties to the lowest class.  This thread holds rows rw, rw + 8 of folds 8j + fc (+1):
           // two words of two different Philox blocks per fold, each block computed for the one word it gives.
           uint2* cw = reinterpret_cast<uint2*>(smem + SM::OFF_LOG) + (blk & 1) * 8 * NF;      // [warp][fold] best of the warp's 16 rows
@@ -435,9 +429,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_stream_kernel(const StreamParams p
                   if (p.expo) {
                     ex = __ldg(p.expo + row_out + k);
                   } else {
-                    const Philox4 r = philox4x32_10((unsigned)t, key.fold, 16u + (unsigned)(k >> 2), o0, key.k0, key.k1);
-                    const unsigned w = (k & 3) == 0 ? r.x : (k & 3) == 1 ? r.y : (k & 3) == 2 ? r.z : r.w;
-                    ex = -logf(u01_open(w));
+                    ex = raw_exp(raw_block(key, (unsigned)t, (unsigned)(k >> 2), o0), (unsigned)(k & 3));
                   }
                   if (p.logits_out) p.logits_out[row_out + k] = lg;
                 }

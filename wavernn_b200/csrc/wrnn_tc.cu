@@ -394,14 +394,11 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
               if (p.expo) {
 #pragma unroll
                 for (int i = 0; i < UT; ++i) ex[i] = __ldg(p.expo + ((size_t)t * p.n_total + p.f0 + fold) * NCLS + u0 + j0 + i);
-              } else {                                        // same keying as the SIMT engine: block 16 + class/4
-                const FoldPhilox k = SES ? FoldPhilox{0u, (unsigned)sseed, (unsigned)(sseed >> 32)} : fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
-                const Philox4 r = philox4x32_10((unsigned)ts, k.fold, 16u + (unsigned)cta, (unsigned)p.offset, k.k0, k.k1);
+              } else {                                        // this thread's classes share one block: 16 + cta
+                const FoldPhilox k = SES ? slot_philox(sseed) : fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
+                const Philox4 r = raw_block(k, (unsigned)ts, (unsigned)cta, (unsigned)p.offset);
 #pragma unroll
-                for (int i = 0; i < UT; ++i) {
-                  const int j = j0 + i;
-                  ex[i] = -logf(u01_open(j == 0 ? r.x : j == 1 ? r.y : j == 2 ? r.z : r.w));
-                }
+                for (int i = 0; i < UT; ++i) ex[i] = raw_exp(r, (unsigned)(j0 + i));
               }
             }
           } else if (p.uniforms) {
@@ -425,15 +422,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
               ur[10] = __ldg(u + 10 * p.n_total + p.f0 + fold);
             }
           } else if (owns_fold) {
-            {
-              const FoldPhilox k = SES ? FoldPhilox{0u, (unsigned)sseed, (unsigned)(sseed >> 32)} : fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
-              const unsigned g = k.fold, k0 = k.k0, k1 = k.k1, o0 = (unsigned)p.offset;
-              const Philox4 r0 = philox4x32_10((unsigned)ts, g, 0u, o0, k0, k1), r1 = philox4x32_10((unsigned)ts, g, 1u, o0, k0, k1),
-                            r2 = philox4x32_10((unsigned)ts, g, 2u, o0, k0, k1);
-              ur[0] = u_ref_range(r0.x); ur[1] = u_ref_range(r0.y); ur[2] = u_ref_range(r0.z); ur[3] = u_ref_range(r0.w);
-              ur[4] = u_ref_range(r1.x); ur[5] = u_ref_range(r1.y); ur[6] = u_ref_range(r1.z); ur[7] = u_ref_range(r1.w);
-              ur[8] = u_ref_range(r2.x); ur[9] = u_ref_range(r2.y); ur[10] = u_ref_range(r2.z);
-            }
+            mol_uniforms(SES ? slot_philox(sseed) : fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed), (unsigned)ts, (unsigned)p.offset, ur);
           }
           if constexpr (RAW) {
 #pragma unroll
