@@ -496,6 +496,32 @@ int wrnn_melspectrogram_many(const wrnn_mel_t *m, const wrnn_mel_utt *u, int32_t
 /* The same with HOST y / mel: copies in, runs, copies out and synchronises. */
 int wrnn_melspectrogram_many_host(const wrnn_mel_t *m, const wrnn_mel_utt *u, int32_t n_utts);
 
+/* Griffin-Lim: the reference's reconstruct_waveform(mel, n_iter) (utils/dsp.py:105-116, librosa 0.7 mel_to_stft and
+ * griffinlim), the inverse of the analysis above with the same configuration and tables.  Per utterance:
+ *   1. S = the non-negative least-squares inversion of db_to_amp(denormalize(mel)) (float32) through the float32
+ *      filterbank, per frame in float64: the clipped minimum-norm least-squares start, then a fixed number of
+ *      accelerated projected-gradient steps (DESIGN.md §3.9);
+ *   2. angles = exp(2 pi i u), u a Philox4x32-10 draw keyed by (phase_seed, frame, bin);
+ *   3. n_iter times: inverse = istft(S angles) (float64 inverse FFT times the window, overlap-added into float32 in
+ *      frame order, divided by the float32 window sum-square, centre-trimmed), rebuilt = stft(inverse) (complex64),
+ *      angles = rebuilt - (0.99 / 1.99) tprev, angles /= |angles| + 1e-16;
+ *   4. wav = istft(S angles).
+ * Contract: each utterance's wav is bit-identical to its own call; the same phase_seed gives the same bits. */
+typedef struct {
+  const float *mel;      /* [n_mels, T] normalized mel, the layout of the reference's mel .npy          */
+  int64_t T;             /* frames; hop_length * (T - 1) > n_fft / 2                                   */
+  uint64_t phase_seed;   /* key of the initial phases                                                  */
+  float *wav;            /* [hop_length * (T - 1)] float32, as reconstruct_waveform returns it          */
+} wrnn_gl_utt;
+/* Every frame of every utterance in each launch: one launch for the solve, then two per iteration and two more.
+ * n_iter >= 0 (0 is the istft of the initial phases).  Refused (WRNN_E_INVALID): a null m or u, n_utts < 1, a null
+ * mel or wav, hop_length * (T_i - 1) <= n_fft / 2 (the message names i), a batch of 2^31 frames or more, n_iter < 0.
+ * Scratch (about 29 KB per frame at n_fft = 2048) is allocated stream-ordered inside the call, in batches of at most
+ * 1 GiB; a failed allocation is WRNN_E_CUDA.  DEVICE mel / wav; asynchronous on `stream`. */
+int wrnn_griffinlim_many(const wrnn_mel_t *m, const wrnn_gl_utt *u, int32_t n_utts, int32_t n_iter, void *stream);
+/* The same with HOST mel / wav: copies in, runs, copies out and synchronises. */
+int wrnn_griffinlim_many_host(const wrnn_mel_t *m, const wrnn_gl_utt *u, int32_t n_utts, int32_t n_iter);
+
 /* Scoring a recording from its audio alone: what preprocess.py:36-47 and utils/dataset.py:86-91 do, on the device.
  *   1. y /= max|y| (float32) when peak_norm is set or the peak exceeds 1;
  *   2. mel = the analysis of that y by `m` (T = 1 + n / hop frames, so T * hop >= n);

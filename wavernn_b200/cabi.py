@@ -27,7 +27,8 @@ EXPORTS = ("wrnn_abi_version", "wrnn_last_error", "wrnn_create", "wrnn_destroy",
            "wrnn_vocode_live_start", "wrnn_vocode_live_poll", "wrnn_vocode_many_live_start",
            "wrnn_vocode_many_live_poll", "wrnn_live_open", "wrnn_live_submit", "wrnn_live_cancel", "wrnn_live_poll",
            "wrnn_live_close", "wrnn_mel_create", "wrnn_mel_destroy", "wrnn_melspectrogram_many",
-           "wrnn_melspectrogram_many_host", "wrnn_score_wav_many", "wrnn_score_wav_many_host")
+           "wrnn_melspectrogram_many_host", "wrnn_score_wav_many", "wrnn_score_wav_many_host", "wrnn_griffinlim_many",
+           "wrnn_griffinlim_many_host")
 LIVE_RUNNING, LIVE_DONE, LIVE_CANCELLED = 0, 1, 2
 
 _fp = C.POINTER(C.c_float)
@@ -108,6 +109,10 @@ class WrnnScoreWavUtt(C.Structure):
     _fields_ = [("y", C.c_void_p), ("n", C.c_int64), ("nll", C.c_void_p)]
 
 
+class WrnnGlUtt(C.Structure):
+    _fields_ = [("mel", C.c_void_p), ("T", C.c_int64), ("phase_seed", C.c_uint64), ("wav", C.c_void_p)]
+
+
 def mel_cfg(*, sample_rate=22050, n_fft=2048, hop_length=275, win_length=1100, n_mels=80, fmin=40.0,
             min_level_db=-100.0) -> WrnnMelCfg:
     """A wrnn_mel_cfg; the defaults are the reference's hparams."""
@@ -120,6 +125,13 @@ def ptr_n_ptr_array(struct, items):
     the array and its length (an empty list gives a NULL array)."""
     arr = (struct * max(len(items), 1))(*[struct(a or None, int(n), b or None) for a, n, b in items])
     return (arr if items else None), len(items)
+
+
+def gl_utts(utts):
+    """A wrnn_gl_utt array over `utts`, a list of (mel address, T, phase_seed, wav address) (0 = NULL).  Returns the
+    array and its length (an empty list gives a NULL array)."""
+    arr = (WrnnGlUtt * max(len(utts), 1))(*[WrnnGlUtt(m or None, int(T), int(s), w or None) for m, T, s, w in utts])
+    return (arr if utts else None), len(utts)
 
 
 def score_utts(utts):
@@ -236,6 +248,15 @@ def load() -> C.CDLL:
     lib.wrnn_score_wav_many_host.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(WrnnScoreWavUtt), C.c_int32, C.c_int32,
                                              C.c_int32]
     # test hooks (not declared in the header)
+    lib.wrnn_griffinlim_many.restype = C.c_int
+    lib.wrnn_griffinlim_many.argtypes = [C.c_void_p, C.POINTER(WrnnGlUtt), C.c_int32, C.c_int32, C.c_void_p]
+    lib.wrnn_griffinlim_many_host.restype = C.c_int
+    lib.wrnn_griffinlim_many_host.argtypes = [C.c_void_p, C.POINTER(WrnnGlUtt), C.c_int32, C.c_int32]
+    lib.wrnn_debug_griffinlim_plan.restype = C.c_int
+    lib.wrnn_debug_griffinlim_plan.argtypes = [C.POINTER(WrnnMelCfg), C.POINTER(WrnnGlUtt), C.c_int32, C.c_int32, C.c_void_p]
+    lib.wrnn_debug_griffinlim.restype = C.c_int
+    lib.wrnn_debug_griffinlim.argtypes = [C.POINTER(WrnnMelCfg), C.c_void_p, C.c_int64, C.c_uint64, C.c_int32, C.c_void_p,
+                                          C.c_void_p]
     lib.wrnn_debug_mel_tables.restype = C.c_int
     lib.wrnn_debug_mel_tables.argtypes = [C.POINTER(WrnnMelCfg), C.c_void_p, C.c_void_p, C.c_void_p]
     lib.wrnn_debug_mel_plan.restype = C.c_int
@@ -577,6 +598,29 @@ class MelAnalysis:
         arr, n = ptr_n_ptr_array(WrnnMelUtt, [(y.ctypes.data, y.size, m.ctypes.data) for y, m in zip(ys, mels)])
         _check(self.lib, self.lib.wrnn_melspectrogram_many_host(self._m, arr, n))
         return mels
+
+    def samples(self, T: int) -> int:
+        """Samples of the Griffin-Lim reconstruction of T frames: hop_length * (T - 1)."""
+        return self.cfg.hop_length * (int(T) - 1)
+
+    def griffinlim_many(self, *, mels, Ts, seeds, wavs, n_iter: int = 32, stream: int = 0):
+        """wrnn_griffinlim_many with raw device addresses: mels[i] [n_mels, Ts[i]] fp32 -> wavs[i] [samples(Ts[i])]
+        fp32, the initial phases keyed by seeds[i].  Asynchronous."""
+        arr, n = gl_utts(list(zip(mels, Ts, seeds, wavs)))
+        _check(self.lib, self.lib.wrnn_griffinlim_many(self._m, arr, n, int(n_iter), C.c_void_p(stream or None)))
+
+    def griffinlim_many_host(self, mels, n_iter: int = 32, seeds=None):
+        """wrnn_griffinlim_many_host: a list of numpy mels [n_mels, T_i] and one phase seed per mel (default i) -> the
+        list of float32 waveforms [hop_length * (T_i - 1)]."""
+        import numpy as np
+        mels = [np.ascontiguousarray(m, dtype=np.float32) for m in mels]
+        seeds = list(range(len(mels))) if seeds is None else list(seeds)
+        if len(seeds) != len(mels):
+            raise ValueError("one seed per mel")
+        wavs = [np.empty(max(self.samples(m.shape[-1]), 0), dtype=np.float32) for m in mels]
+        arr, n = gl_utts([(m.ctypes.data, m.shape[-1], s, w.ctypes.data) for m, s, w in zip(mels, seeds, wavs)])
+        _check(self.lib, self.lib.wrnn_griffinlim_many_host(self._m, arr, n, int(n_iter)))
+        return wavs
 
     def close(self):
         if self._m:

@@ -85,12 +85,22 @@ __device__ __forceinline__ float gru_unit(float gi_r, float gi_z, float gi_n, fl
 // Philox4x32-10 (Salmon et al. 2011), counter-based: (seed) x (step, fold, lane, offset)
 // -------------------------------------------------------------------------------------
 struct Philox4 { unsigned x, y, z, w; };
-__device__ __forceinline__ Philox4 philox4x32_10(unsigned c0, unsigned c1, unsigned c2, unsigned c3,
-                                                  unsigned k0, unsigned k1) {
+__host__ __device__ __forceinline__ unsigned umulhi32(unsigned a, unsigned b) {
+#ifdef __CUDA_ARCH__
+  return __umulhi(a, b);
+#else
+  return (unsigned)(((unsigned long long)a * b) >> 32);
+#endif
+}
+// host and device (wrnn_debug_griffinlim runs the Griffin-Lim phase draws on the host)
+__host__ __device__ __forceinline__ Philox4 philox4x32_10(unsigned c0, unsigned c1, unsigned c2, unsigned c3,
+                                                           unsigned k0, unsigned k1) {
+#ifdef __CUDA_ARCH__
 #pragma unroll
+#endif
   for (int i = 0; i < 10; ++i) {
-    const unsigned hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-    const unsigned hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
+    const unsigned hi0 = umulhi32(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
+    const unsigned hi1 = umulhi32(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
     const unsigned n0 = hi1 ^ c1 ^ k0, n1 = lo1, n2 = hi0 ^ c3 ^ k1, n3 = lo0;
     c0 = n0; c1 = n1; c2 = n2; c3 = n3;
     k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
@@ -99,7 +109,7 @@ __device__ __forceinline__ Philox4 philox4x32_10(unsigned c0, unsigned c1, unsig
 }
 // 24 random bits -> [2^-25, 1].  Closed at 1: above 2^23 the float sum (m + 0.5f) rounds to nearest even, so
 // x >> 8 == 0xffffff gives exactly 1.0f (once per 2^24 words).
-__device__ __forceinline__ float u01(unsigned x) { return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f); }
+__host__ __device__ __forceinline__ float u01(unsigned x) { return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f); }
 // u01 clamped into the open interval (0, 1): the RAW head's Exp(1) draws -logf(u) must be > 0 (at u = 1 they were -0.0,
 // which forced the class in the persistent engine and excluded it in the SIMT engine).  Every other word maps as u01.
 __device__ __forceinline__ float u01_open(unsigned x) { return fminf(u01(x), 0x1.fffffep-1f); }
