@@ -522,6 +522,36 @@ int wrnn_griffinlim_many(const wrnn_mel_t *m, const wrnn_gl_utt *u, int32_t n_ut
 /* The same with HOST mel / wav: copies in, runs, copies out and synchronises. */
 int wrnn_griffinlim_many_host(const wrnn_mel_t *m, const wrnn_gl_utt *u, int32_t n_utts, int32_t n_iter);
 
+/* Resampling: the reference's load_wav (utils/dsp.py: librosa.load(path, sr=hp.sample_rate), librosa 0.6.3) after
+ * decoding and mixing to mono, on the device: resampy's `kaiser_best` band-limited interpolation to the analysis
+ * object's sample_rate, then librosa's fix_length.  Per utterance, with ratio = (double)sample_rate_out / sample_rate:
+ *   1. int(n * ratio) samples of resampy's resample_f with the kaiser_best half-window (64 zero crossings, Kaiser
+ *      beta 14.769656459379492, rolloff 0.9475937167399596, 2^16 table entries per zero crossing), scaled by ratio
+ *      when it is below 1; output t reads the time register t * (1 / ratio), and each tap's weighted sample is added
+ *      in float64 and the sum rounded to float32 (DESIGN.md §3.10);
+ *   2. zero padding to wrnn_resample_length(n, sample_rate, sample_rate_out) = ceil(n * ratio) samples.
+ * Equal rates copy x, as librosa does not resample them.  The result feeds wrnn_melspectrogram_many,
+ * wrnn_score_wav_many and wrnn_vocode built for the same sample_rate.
+ * Contracts: a batch gives the same bits as each utterance resampled alone; the _host entry point gives the same bits
+ * as the device one; nothing is written past wrnn_resample_length samples of y.
+ * The filter table (33.6 MB of float64) is uploaded once per analysis object, by its first resampling call. */
+typedef struct {
+  const float *x;        /* [n] the decoded mono recording, float32                                  */
+  int64_t n;             /* samples, >= 1                                                             */
+  int32_t sample_rate;   /* its rate, > 0; each utterance of a batch may have its own                 */
+  int32_t pad;
+  float *y;              /* [wrnn_resample_length(n, sample_rate, m's sample_rate)]                   */
+} wrnn_resample_utt;
+/* ceil(n * ((double)sr_out / sr_in)): the samples librosa.load returns; -1 if n < 0 or a rate is <= 0. */
+int64_t wrnn_resample_length(int64_t n, int32_t sr_in, int32_t sr_out);
+/* Every output sample of every utterance in one kernel launch.  Refused (WRNN_E_INVALID; the message names i): a null
+ * m or u, n_utts < 1, a null x or y, sample_rate <= 0, n < 1, int(n * ratio) < 1 (resampy refuses it too), a ratio
+ * below 2^-16 (the filter would have no taps), a batch of 2^31 output samples or more.  DEVICE x / y; asynchronous on
+ * `stream` (the first call on an object also uploads the table, synchronously). */
+int wrnn_resample_many(const wrnn_mel_t *m, const wrnn_resample_utt *u, int32_t n_utts, void *stream);
+/* The same with HOST x / y: copies in, runs, copies out and synchronises. */
+int wrnn_resample_many_host(const wrnn_mel_t *m, const wrnn_resample_utt *u, int32_t n_utts);
+
 /* Scoring a recording from its audio alone: what preprocess.py:36-47 and utils/dataset.py:86-91 do, on the device.
  *   1. y /= max|y| (float32) when peak_norm is set or the peak exceeds 1;
  *   2. mel = the analysis of that y by `m` (T = 1 + n / hop frames, so T * hop >= n);

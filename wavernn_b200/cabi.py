@@ -28,7 +28,7 @@ EXPORTS = ("wrnn_abi_version", "wrnn_last_error", "wrnn_create", "wrnn_destroy",
            "wrnn_vocode_many_live_poll", "wrnn_live_open", "wrnn_live_submit", "wrnn_live_cancel", "wrnn_live_poll",
            "wrnn_live_close", "wrnn_mel_create", "wrnn_mel_destroy", "wrnn_melspectrogram_many",
            "wrnn_melspectrogram_many_host", "wrnn_score_wav_many", "wrnn_score_wav_many_host", "wrnn_griffinlim_many",
-           "wrnn_griffinlim_many_host")
+           "wrnn_griffinlim_many_host", "wrnn_resample_length", "wrnn_resample_many", "wrnn_resample_many_host")
 LIVE_RUNNING, LIVE_DONE, LIVE_CANCELLED = 0, 1, 2
 
 _fp = C.POINTER(C.c_float)
@@ -111,6 +111,18 @@ class WrnnScoreWavUtt(C.Structure):
 
 class WrnnGlUtt(C.Structure):
     _fields_ = [("mel", C.c_void_p), ("T", C.c_int64), ("phase_seed", C.c_uint64), ("wav", C.c_void_p)]
+
+
+class WrnnResampleUtt(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("n", C.c_int64), ("sample_rate", C.c_int32), ("pad", C.c_int32), ("y", C.c_void_p)]
+
+
+def resample_utts(utts):
+    """A wrnn_resample_utt array over `utts`, a list of (x address, n, sample_rate, y address) (0 = NULL).  Returns the
+    array and its length (an empty list gives a NULL array)."""
+    arr = (WrnnResampleUtt * max(len(utts), 1))(*[WrnnResampleUtt(x or None, int(n), int(sr), 0, y or None)
+                                                  for x, n, sr, y in utts])
+    return (arr if utts else None), len(utts)
 
 
 def mel_cfg(*, sample_rate=22050, n_fft=2048, hop_length=275, win_length=1100, n_mels=80, fmin=40.0,
@@ -247,11 +259,21 @@ def load() -> C.CDLL:
     lib.wrnn_score_wav_many_host.restype = C.c_int
     lib.wrnn_score_wav_many_host.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(WrnnScoreWavUtt), C.c_int32, C.c_int32,
                                              C.c_int32]
-    # test hooks (not declared in the header)
+    lib.wrnn_resample_length.restype = C.c_int64
+    lib.wrnn_resample_length.argtypes = [C.c_int64, C.c_int32, C.c_int32]
+    lib.wrnn_resample_many.restype = C.c_int
+    lib.wrnn_resample_many.argtypes = [C.c_void_p, C.POINTER(WrnnResampleUtt), C.c_int32, C.c_void_p]
+    lib.wrnn_resample_many_host.restype = C.c_int
+    lib.wrnn_resample_many_host.argtypes = [C.c_void_p, C.POINTER(WrnnResampleUtt), C.c_int32]
     lib.wrnn_griffinlim_many.restype = C.c_int
     lib.wrnn_griffinlim_many.argtypes = [C.c_void_p, C.POINTER(WrnnGlUtt), C.c_int32, C.c_int32, C.c_void_p]
     lib.wrnn_griffinlim_many_host.restype = C.c_int
     lib.wrnn_griffinlim_many_host.argtypes = [C.c_void_p, C.POINTER(WrnnGlUtt), C.c_int32, C.c_int32]
+    # test hooks (not declared in the header)
+    lib.wrnn_debug_resample_table.restype = C.c_int64
+    lib.wrnn_debug_resample_table.argtypes = [C.c_void_p]
+    lib.wrnn_debug_resample.restype = C.c_int
+    lib.wrnn_debug_resample.argtypes = [C.POINTER(WrnnResampleUtt), C.c_int32, C.c_int32]
     lib.wrnn_debug_griffinlim_plan.restype = C.c_int
     lib.wrnn_debug_griffinlim_plan.argtypes = [C.POINTER(WrnnMelCfg), C.POINTER(WrnnGlUtt), C.c_int32, C.c_int32, C.c_void_p]
     lib.wrnn_debug_griffinlim.restype = C.c_int
@@ -621,6 +643,30 @@ class MelAnalysis:
         arr, n = gl_utts([(m.ctypes.data, m.shape[-1], s, w.ctypes.data) for m, s, w in zip(mels, seeds, wavs)])
         _check(self.lib, self.lib.wrnn_griffinlim_many_host(self._m, arr, n, int(n_iter)))
         return wavs
+
+    def resample_length(self, n: int, sample_rate: int) -> int:
+        """Samples of a recording of n samples at sample_rate resampled to this object's rate (wrnn_resample_length):
+        ceil(n * ratio), what librosa.load returns."""
+        return int(self.lib.wrnn_resample_length(int(n), int(sample_rate), self.cfg.sample_rate))
+
+    def resample_many(self, *, xs, ns, rates, ys, stream: int = 0):
+        """wrnn_resample_many with raw device addresses: xs[i] [ns[i]] fp32 at rates[i] Hz -> ys[i]
+        [resample_length(ns[i], rates[i])] at this object's sample_rate.  Asynchronous."""
+        arr, n = resample_utts(list(zip(xs, ns, rates, ys)))
+        _check(self.lib, self.lib.wrnn_resample_many(self._m, arr, n, C.c_void_p(stream or None)))
+
+    def resample_many_host(self, xs, rates):
+        """wrnn_resample_many_host: a list of numpy recordings and their sample rates -> the list of float32 recordings
+        at this object's sample_rate, what librosa.load(..., sr=sample_rate) makes of them after decoding."""
+        import numpy as np
+        xs = [np.ascontiguousarray(x, dtype=np.float32).reshape(-1) for x in xs]
+        rates = [int(r) for r in rates]
+        if len(rates) != len(xs):
+            raise ValueError("one sample rate per recording")
+        ys = [np.empty(max(self.resample_length(x.size, r), 0), dtype=np.float32) for x, r in zip(xs, rates)]
+        arr, n = resample_utts([(x.ctypes.data, x.size, r, y.ctypes.data) for x, r, y in zip(xs, rates, ys)])
+        _check(self.lib, self.lib.wrnn_resample_many_host(self._m, arr, n))
+        return ys
 
     def close(self):
         if self._m:

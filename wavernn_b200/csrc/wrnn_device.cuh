@@ -81,6 +81,30 @@ __device__ __forceinline__ float gru_unit(float gi_r, float gi_z, float gi_n, fl
   return (1.0f - z) * n + z * h;
 }
 
+// float32 / float64 arithmetic rounded step by step, as numpy evaluates it (no fused multiply-add on the device); the
+// host hooks of wrnn_mel.cu and wrnn_resample.cu run the same source on the CPU
+__host__ __device__ inline float fmul_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+__host__ __device__ inline double dmul_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+__host__ __device__ inline double dadd_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+
 // -------------------------------------------------------------------------------------
 // Philox4x32-10 (Salmon et al. 2011), counter-based: (seed) x (step, fold, lane, offset)
 // -------------------------------------------------------------------------------------

@@ -319,22 +319,6 @@ static void build_gl(const wrnn_mel_cfg& c, const HostTabs& t, HostGL& g) {
   g.step = hi > 0 ? 1.0 / hi : 0.0;
 }
 
-// float32 / float64 arithmetic rounded step by step, as numpy evaluates it (no fused multiply-add on the device)
-__host__ __device__ inline float fmul_rn(float a, float b) {
-#ifdef __CUDA_ARCH__
-  return __fmul_rn(a, b);
-#else
-  return a * b;
-#endif
-}
-__host__ __device__ inline double dmul_rn(double a, double b) {
-#ifdef __CUDA_ARCH__
-  return __dmul_rn(a, b);
-#else
-  return a * b;
-#endif
-}
-
 // ---- the solve, step by step ----
 // b_m = db_to_amp(denormalize(mel)) in float32: (clip(v, 0, 1) * -L + L) * 0.05, then 10^x rounded once.  NaN stays NaN.
 __host__ __device__ inline double nnls_rhs(const Tabs& tb, float v) {
@@ -682,9 +666,10 @@ int wrnn_mel_create(wrnn_mel_t** out, const wrnn_mel_cfg* cfg, int device) {
 
 void wrnn_mel_destroy(wrnn_mel_t* m) {
   if (!m) return;
-  if (m->d_tabs) {
+  if (m->d_tabs || m->d_rs_win) {
     cudaSetDevice(m->device);
     cudaFree(m->d_tabs);
+    cudaFree(m->d_rs_win);
   }
   delete m;
 }

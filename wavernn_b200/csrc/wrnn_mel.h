@@ -1,6 +1,7 @@
 // wrnn_mel.h -- the mel analysis object of wrnn_mel_create and its host-side checks (wrnn_mel.cu).
 #pragma once
 #include <cstdint>
+#include <mutex>
 #include <vector>
 
 #include "../../include/wavernn_b200.h"
@@ -13,6 +14,9 @@ struct wrnn_mel_plan {
   long long n_basis = 0;    // nonzero filterbank weights
   long long gl_off = 0;     // offset of basis32 in d_tabs, in doubles
   double gl_step = 0.0;     // 1 / lambda_max(A A^T) of the float32 filterbank A
+  // the resampling filter's half-window (wrnn_resample.cu), uploaded by the first wrnn_resample_many on this object
+  mutable std::mutex rs_mu;
+  mutable double* d_rs_win = nullptr;
 };
 
 namespace wrnn {
