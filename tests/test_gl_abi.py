@@ -173,7 +173,7 @@ def gl_plan(lib, Ts, n_iter=32, null=None, **cfg):
     if null is not None:
         i, field = null
         items[i] = (0 if field == "mel" else FAKE, Ts[i], 0, 0 if field == "wav" else FAKE)
-    arr, n = cabi.gl_utts(items)
+    arr, n = cabi.utt_array(cabi.WrnnGlUtt, items)
     f0 = np.zeros(max(n, 1) + 1, dtype=np.int64)
     rc = lib.wrnn_debug_griffinlim_plan(ctypes.byref(cabi.mel_cfg(**cfg)), arr, n, n_iter, f0.ctypes.data)
     return rc, lib.wrnn_last_error().decode() if rc else "", f0
@@ -214,7 +214,7 @@ def test_griffinlim_refusals(lib, kw, msg):
 
 
 def test_null_analysis_object_is_refused(lib):
-    arr, n = cabi.gl_utts([(FAKE, 300, 0, FAKE)])
+    arr, n = cabi.utt_array(cabi.WrnnGlUtt, [(FAKE, 300, 0, FAKE)])
     assert lib.wrnn_griffinlim_many(None, arr, n, 32, None) == cabi.WRNN_E_INVALID
     assert lib.wrnn_griffinlim_many_host(None, arr, n, 32) == cabi.WRNN_E_INVALID
     assert "null analysis object" in lib.wrnn_last_error().decode()

@@ -139,7 +139,7 @@ def mel_plan(lib, ns, null=None, **cfg):
     if null is not None:
         i, field = null
         items[i] = (0 if field == "y" else FAKE, ns[i], 0 if field == "mel" else FAKE)
-    arr, n = cabi.ptr_n_ptr_array(cabi.WrnnMelUtt, items)
+    arr, n = cabi.utt_array(cabi.WrnnMelUtt, items)
     f0 = np.zeros(max(n, 1) + 1, dtype=np.int64)
     rc = lib.wrnn_debug_mel_plan(ctypes.byref(cabi.mel_cfg(**cfg)), arr, n, f0.ctypes.data)
     return rc, lib.wrnn_last_error().decode() if rc else "", f0
@@ -176,11 +176,11 @@ def test_melspectrogram_refusals(lib, kw, msg):
 
 
 def test_null_analysis_object_is_refused(lib):
-    arr, n = cabi.ptr_n_ptr_array(cabi.WrnnMelUtt, [(FAKE, 5000, FAKE)])
+    arr, n = cabi.utt_array(cabi.WrnnMelUtt, [(FAKE, 5000, FAKE)])
     assert lib.wrnn_melspectrogram_many(None, arr, n, None) == cabi.WRNN_E_INVALID
     assert lib.wrnn_melspectrogram_many_host(None, arr, n) == cabi.WRNN_E_INVALID
     assert "null analysis object" in lib.wrnn_last_error().decode()
-    sarr, n = cabi.ptr_n_ptr_array(cabi.WrnnScoreWavUtt, [(FAKE, 5000, FAKE)])
+    sarr, n = cabi.utt_array(cabi.WrnnScoreWavUtt, [(FAKE, 5000, FAKE)])
     assert lib.wrnn_score_wav_many(None, None, sarr, n, 0, 0, None) == cabi.WRNN_E_INVALID
     assert lib.wrnn_score_wav_many_host(None, None, sarr, n, 0, 0) == cabi.WRNN_E_INVALID
     assert "null handle" in lib.wrnn_last_error().decode()
@@ -191,7 +191,7 @@ def wav_plan(lib, ns, feat=80, hop=275, null=None, **cfg):
     if null is not None:
         i, field = null
         items[i] = (0 if field == "y" else FAKE, ns[i], 0 if field == "nll" else FAKE)
-    arr, n = cabi.ptr_n_ptr_array(cabi.WrnnScoreWavUtt, items)
+    arr, n = cabi.utt_array(cabi.WrnnScoreWavUtt, items)
     T = np.zeros(max(n, 1), dtype=np.int64)
     rc = lib.wrnn_debug_score_wav_plan(feat, hop, ctypes.byref(cabi.mel_cfg(**cfg)), arr, n, T.ctypes.data)
     return rc, lib.wrnn_last_error().decode() if rc else "", T

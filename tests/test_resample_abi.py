@@ -32,7 +32,8 @@ def host(lib, xs, rates, sr_out=SR):
     """wrnn_debug_resample on a batch: the list of outputs, each followed in memory by a sentinel that must survive."""
     xs = [np.ascontiguousarray(x, dtype=np.float32) for x in xs]
     bufs = [np.full(lib.wrnn_resample_length(x.size, r, sr_out) + 1, 7.0, dtype=np.float32) for x, r in zip(xs, rates)]
-    arr, n = cabi.resample_utts([(x.ctypes.data, x.size, r, b.ctypes.data) for x, r, b in zip(xs, rates, bufs)])
+    arr, n = cabi.utt_array(cabi.WrnnResampleUtt,
+                            [(x.ctypes.data, x.size, r, b.ctypes.data) for x, r, b in zip(xs, rates, bufs)])
     rc = lib.wrnn_debug_resample(arr, n, sr_out)
     assert rc == 0, lib.wrnn_last_error()
     assert all(b[-1] == 7.0 for b in bufs), "written past wrnn_resample_length"
@@ -180,7 +181,7 @@ def test_struct_layout():
 
 
 def refusal(lib, utts, n=None, sr_out=SR):
-    arr, k = cabi.resample_utts(utts)
+    arr, k = cabi.utt_array(cabi.WrnnResampleUtt, utts)
     rc = lib.wrnn_debug_resample(arr, k if n is None else n, sr_out)
     return rc, (lib.wrnn_last_error() or b"").decode()
 
@@ -213,7 +214,7 @@ def test_refusals(lib):
 
 def test_null_analysis_object(lib):
     x = np.zeros(10, np.float32)
-    arr, n = cabi.resample_utts([(x.ctypes.data, 10, 44100, x.ctypes.data)])
+    arr, n = cabi.utt_array(cabi.WrnnResampleUtt, [(x.ctypes.data, 10, 44100, x.ctypes.data)])
     assert lib.wrnn_resample_many(None, arr, n, None) == cabi.WRNN_E_INVALID
     assert lib.wrnn_resample_many_host(None, arr, n) == cabi.WRNN_E_INVALID
     assert "null analysis object" in lib.wrnn_last_error().decode()

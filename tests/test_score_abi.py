@@ -108,7 +108,7 @@ def _plan(lib, Ts, ns, hop=HOP, null=None):
         i, field = null
         m, T, x, n, o = utts[i]
         utts[i] = (0 if field == "mel" else m, T, 0 if field == "x" else x, n, 0 if field == "nll" else o)
-    arr, count = cabi.score_utts(utts)
+    arr, count = cabi.utt_array(cabi.WrnnScoreUtt, utts)
     geo = np.zeros(5, dtype=np.int64)
     rc = lib.wrnn_debug_score_many_plan(hop, arr, count, geo.ctypes.data, None)
     if rc != 0:

@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+from functools import partial
 from pathlib import Path
 
 LIB_NAME = "libwavernn_b200.so"
@@ -117,14 +118,6 @@ class WrnnResampleUtt(C.Structure):
     _fields_ = [("x", C.c_void_p), ("n", C.c_int64), ("sample_rate", C.c_int32), ("pad", C.c_int32), ("y", C.c_void_p)]
 
 
-def resample_utts(utts):
-    """A wrnn_resample_utt array over `utts`, a list of (x address, n, sample_rate, y address) (0 = NULL).  Returns the
-    array and its length (an empty list gives a NULL array)."""
-    arr = (WrnnResampleUtt * max(len(utts), 1))(*[WrnnResampleUtt(x or None, int(n), int(sr), 0, y or None)
-                                                  for x, n, sr, y in utts])
-    return (arr if utts else None), len(utts)
-
-
 def mel_cfg(*, sample_rate=22050, n_fft=2048, hop_length=275, win_length=1100, n_mels=80, fmin=40.0,
             min_level_db=-100.0) -> WrnnMelCfg:
     """A wrnn_mel_cfg; the defaults are the reference's hparams."""
@@ -132,34 +125,28 @@ def mel_cfg(*, sample_rate=22050, n_fft=2048, hop_length=275, win_length=1100, n
                       float(min_level_db))
 
 
-def ptr_n_ptr_array(struct, items):
-    """A wrnn_mel_utt or wrnn_score_wav_utt array over `items`, a list of (address, n, address) (0 = NULL).  Returns
-    the array and its length (an empty list gives a NULL array)."""
-    arr = (struct * max(len(items), 1))(*[struct(a or None, int(n), b or None) for a, n, b in items])
-    return (arr if items else None), len(items)
+def utt_array(struct, rows):
+    """A ctypes array of `struct` (WrnnUtterance, WrnnScoreUtt, WrnnMelUtt, WrnnScoreWavUtt, WrnnGlUtt or
+    WrnnResampleUtt) over `rows`, each a tuple of the struct's fields in order, `pad` left out (addresses as integers,
+    0 = NULL).  Returns the array and its length (an empty list gives a NULL array)."""
+    fields = [(name, t) for name, t in struct._fields_ if name != "pad"]
+    arr = (struct * max(len(rows), 1))(*[struct(**{name: (v or None) if t is C.c_void_p else int(v)
+                                                   for (name, t), v in zip(fields, row, strict=True)}) for row in rows])
+    return (arr if rows else None), len(rows)
 
 
-def gl_utts(utts):
-    """A wrnn_gl_utt array over `utts`, a list of (mel address, T, phase_seed, wav address) (0 = NULL).  Returns the
-    array and its length (an empty list gives a NULL array)."""
-    arr = (WrnnGlUtt * max(len(utts), 1))(*[WrnnGlUtt(m or None, int(T), int(s), w or None) for m, T, s, w in utts])
-    return (arr if utts else None), len(utts)
-
-
-def score_utts(utts):
-    """A wrnn_score_utt array over `utts`, a list of (mel address, T, x address, n, nll address) (0 = NULL).  Returns
-    the array and its length (an empty list gives a NULL array)."""
-    arr = (WrnnScoreUtt * max(len(utts), 1))(*[WrnnScoreUtt(m or None, int(T), x or None, int(n), o or None)
-                                               for m, T, x, n, o in utts])
-    return (arr if utts else None), len(utts)
+# The per-struct builders of earlier versions of this module, kept so that callers written against them still run.
+ptr_n_ptr_array = utt_array
+gl_utts = partial(utt_array, WrnnGlUtt)
+score_utts = partial(utt_array, WrnnScoreUtt)
+resample_utts = partial(utt_array, WrnnResampleUtt)
 
 
 def vocode_batch(utts, *, batched=True, target=11000, overlap=550, mu_law=False):
     """A wrnn_vocode_batch over `utts`, a list of (mel address, T, philox_seed, wav address) (0 = NULL).  Returns the
     struct and the utterance array it points to (keep both alive for the call)."""
-    arr = (WrnnUtterance * max(len(utts), 1))(*[WrnnUtterance(m or None, int(T), int(s), w or None) for m, T, s, w in utts])
-    b = WrnnVocodeBatch(arr if utts else None, len(utts), int(bool(batched)), int(target), int(overlap), int(bool(mu_law)))
-    return b, arr
+    arr, n = utt_array(WrnnUtterance, utts)
+    return WrnnVocodeBatch(arr, n, int(bool(batched)), int(target), int(overlap), int(bool(mu_law))), arr
 
 
 _lib = None
@@ -541,7 +528,7 @@ class Engine:
     def score_many(self, *, mels, Ts, xs, ns, nlls, stream: int = 0):
         """wrnn_score_many with raw device addresses: utterance i is mels[i] [80, Ts[i]] and its waveform xs[i] [ns[i]]
         -> nlls[i] [ns[i]] fp32, each scored unbatched (one fold).  One job for the whole batch.  Asynchronous."""
-        arr, n = score_utts(list(zip(mels, Ts, xs, ns, nlls)))
+        arr, n = utt_array(WrnnScoreUtt, list(zip(mels, Ts, xs, ns, nlls)))
         _check(self.lib, self.lib.wrnn_score_many(self._h, arr, n, C.c_void_p(stream or None)))
 
     def score_many_host(self, mels, xs):
@@ -553,8 +540,8 @@ class Engine:
         if len(xs) != len(mels):
             raise ValueError("one waveform per mel")
         nlls = [np.empty(x.size, dtype=np.float32) for x in xs]
-        arr, n = score_utts([(m.ctypes.data, m.shape[-1], x.ctypes.data, x.size, o.ctypes.data)
-                             for m, x, o in zip(mels, xs, nlls)])
+        arr, n = utt_array(WrnnScoreUtt, [(m.ctypes.data, m.shape[-1], x.ctypes.data, x.size, o.ctypes.data)
+                                          for m, x, o in zip(mels, xs, nlls)])
         _check(self.lib, self.lib.wrnn_score_many_host(self._h, arr, n))
         return nlls
 
@@ -562,7 +549,7 @@ class Engine:
                        stream: int = 0):
         """wrnn_score_wav_many with raw device addresses: recording i is ys[i] [ns[i]] fp32 -> nlls[i] [ns[i]], its mel
         made by `analysis` and its targets quantised as preprocess.py stores them.  Asynchronous."""
-        arr, n = ptr_n_ptr_array(WrnnScoreWavUtt, list(zip(ys, ns, nlls)))
+        arr, n = utt_array(WrnnScoreWavUtt, list(zip(ys, ns, nlls)))
         _check(self.lib, self.lib.wrnn_score_wav_many(self._h, analysis._m, arr, n, int(bool(peak_norm)), int(bool(mu_law)),
                                                       C.c_void_p(stream or None)))
 
@@ -572,7 +559,7 @@ class Engine:
         import numpy as np
         ys = [np.ascontiguousarray(y, dtype=np.float32).reshape(-1) for y in ys]
         nlls = [np.empty(y.size, dtype=np.float32) for y in ys]
-        arr, n = ptr_n_ptr_array(WrnnScoreWavUtt, [(y.ctypes.data, y.size, o.ctypes.data) for y, o in zip(ys, nlls)])
+        arr, n = utt_array(WrnnScoreWavUtt, [(y.ctypes.data, y.size, o.ctypes.data) for y, o in zip(ys, nlls)])
         _check(self.lib, self.lib.wrnn_score_wav_many_host(self._h, analysis._m, arr, n, int(bool(peak_norm)),
                                                            int(bool(mu_law))))
         return nlls
@@ -609,7 +596,7 @@ class MelAnalysis:
     def melspectrogram_many(self, *, ys, ns, mels, stream: int = 0):
         """wrnn_melspectrogram_many with raw device addresses: ys[i] [ns[i]] fp32 -> mels[i] [n_mels, frames(ns[i])].
         Asynchronous."""
-        arr, n = ptr_n_ptr_array(WrnnMelUtt, list(zip(ys, ns, mels)))
+        arr, n = utt_array(WrnnMelUtt, list(zip(ys, ns, mels)))
         _check(self.lib, self.lib.wrnn_melspectrogram_many(self._m, arr, n, C.c_void_p(stream or None)))
 
     def melspectrogram_many_host(self, ys):
@@ -617,7 +604,7 @@ class MelAnalysis:
         import numpy as np
         ys = [np.ascontiguousarray(y, dtype=np.float32).reshape(-1) for y in ys]
         mels = [np.empty((self.cfg.n_mels, self.frames(y.size)), dtype=np.float32) for y in ys]
-        arr, n = ptr_n_ptr_array(WrnnMelUtt, [(y.ctypes.data, y.size, m.ctypes.data) for y, m in zip(ys, mels)])
+        arr, n = utt_array(WrnnMelUtt, [(y.ctypes.data, y.size, m.ctypes.data) for y, m in zip(ys, mels)])
         _check(self.lib, self.lib.wrnn_melspectrogram_many_host(self._m, arr, n))
         return mels
 
@@ -628,7 +615,7 @@ class MelAnalysis:
     def griffinlim_many(self, *, mels, Ts, seeds, wavs, n_iter: int = 32, stream: int = 0):
         """wrnn_griffinlim_many with raw device addresses: mels[i] [n_mels, Ts[i]] fp32 -> wavs[i] [samples(Ts[i])]
         fp32, the initial phases keyed by seeds[i].  Asynchronous."""
-        arr, n = gl_utts(list(zip(mels, Ts, seeds, wavs)))
+        arr, n = utt_array(WrnnGlUtt, list(zip(mels, Ts, seeds, wavs)))
         _check(self.lib, self.lib.wrnn_griffinlim_many(self._m, arr, n, int(n_iter), C.c_void_p(stream or None)))
 
     def griffinlim_many_host(self, mels, n_iter: int = 32, seeds=None):
@@ -640,7 +627,7 @@ class MelAnalysis:
         if len(seeds) != len(mels):
             raise ValueError("one seed per mel")
         wavs = [np.empty(max(self.samples(m.shape[-1]), 0), dtype=np.float32) for m in mels]
-        arr, n = gl_utts([(m.ctypes.data, m.shape[-1], s, w.ctypes.data) for m, s, w in zip(mels, seeds, wavs)])
+        arr, n = utt_array(WrnnGlUtt, [(m.ctypes.data, m.shape[-1], s, w.ctypes.data) for m, s, w in zip(mels, seeds, wavs)])
         _check(self.lib, self.lib.wrnn_griffinlim_many_host(self._m, arr, n, int(n_iter)))
         return wavs
 
@@ -652,7 +639,7 @@ class MelAnalysis:
     def resample_many(self, *, xs, ns, rates, ys, stream: int = 0):
         """wrnn_resample_many with raw device addresses: xs[i] [ns[i]] fp32 at rates[i] Hz -> ys[i]
         [resample_length(ns[i], rates[i])] at this object's sample_rate.  Asynchronous."""
-        arr, n = resample_utts(list(zip(xs, ns, rates, ys)))
+        arr, n = utt_array(WrnnResampleUtt, list(zip(xs, ns, rates, ys)))
         _check(self.lib, self.lib.wrnn_resample_many(self._m, arr, n, C.c_void_p(stream or None)))
 
     def resample_many_host(self, xs, rates):
@@ -664,7 +651,7 @@ class MelAnalysis:
         if len(rates) != len(xs):
             raise ValueError("one sample rate per recording")
         ys = [np.empty(max(self.resample_length(x.size, r), 0), dtype=np.float32) for x, r in zip(xs, rates)]
-        arr, n = resample_utts([(x.ctypes.data, x.size, r, y.ctypes.data) for x, r, y in zip(xs, rates, ys)])
+        arr, n = utt_array(WrnnResampleUtt, [(x.ctypes.data, x.size, r, y.ctypes.data) for x, r, y in zip(xs, rates, ys)])
         _check(self.lib, self.lib.wrnn_resample_many_host(self._m, arr, n))
         return ys
 

@@ -77,36 +77,18 @@ static int grow_mapped(void** host, void** dev, size_t* bytes, size_t want) {
   return WRNN_OK;
 }
 
-// Staging of the host-memory entry points.  stage places each item at a 256-B-aligned offset of the handle's one device
-// staging buffer and copies it there on st (cudaMemcpyDefault: src may be host or device memory; src NULL: a region the
-// job writes); dev[k] is item k's device address, NULL for an empty item.  unstage, their common end, copies the results
-// back, synchronises and returns the engine's check().
-struct Staged { const void* src; size_t bytes; };
-struct Unstaged { void* dst; const void* src; size_t bytes; };
-static size_t align256(size_t bytes) { return (bytes + 255) & ~size_t(255); }
-
+// Staging of the handle's host-memory entry points (place / copy_back, wrnn_engine.h) in its one device staging buffer,
+// grown as needed.  unstage, their common end, copies the results back, synchronises and returns the engine's check().
 static int stage(wrnn_t* h, const std::vector<Staged>& items, cudaStream_t st, std::vector<void*>& dev) {
-  size_t total = 0;
-  for (const Staged& it : items) total += align256(it.bytes);
   WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
-  const int rc = grow(&h->d_stage, &h->stage_bytes, total);
+  const int rc = grow(&h->d_stage, &h->stage_bytes, staged_bytes(items));
   if (rc != WRNN_OK) return rc;
-  char* d = static_cast<char*>(h->d_stage);
-  dev.assign(items.size(), nullptr);
-  for (size_t k = 0; k < items.size(); ++k) {
-    if (!items[k].bytes) continue;
-    dev[k] = d;
-    if (items[k].src) WRNN_CUDA_OK(cudaMemcpyAsync(d, items[k].src, items[k].bytes, cudaMemcpyDefault, st));
-    d += align256(items[k].bytes);
-  }
-  return WRNN_OK;
+  return place(h->d_stage, items, st, dev);
 }
 
 static int unstage(wrnn_t* h, const std::vector<Unstaged>& items) {
-  for (const Unstaged& it : items)
-    if (it.bytes) WRNN_CUDA_OK(cudaMemcpyAsync(it.dst, it.src, it.bytes, cudaMemcpyDeviceToHost, 0));
-  WRNN_CUDA_OK(cudaStreamSynchronize(0));
-  return h->last->check();
+  const int rc = copy_back(items);
+  return rc != WRNN_OK ? rc : h->last->check();
 }
 
 // The host epilogue's tables (wrnn_vocode's unbatched geometry): mu is empty unless mu-law applies, which it does on a
@@ -903,21 +885,21 @@ static int validate_score_wav(const wrnn_t* h, const wrnn_mel_t* m, const wrnn_s
 static int score_wav_many(wrnn_t* h, const wrnn_mel_t* m, const wrnn_score_wav_utt* u, int n, int peak_norm, int mu_law,
                           const cond::BatchPlan& pl, const std::vector<int64_t>& frame0, cudaStream_t st) {
   const int nm = m->cfg.n_mels;
-  std::vector<size_t> off(3 * n + 3, 0);
-  off[1] = align256(n * sizeof(WavUtt));
-  off[2] = off[1] + align256(n * sizeof(float));
+  std::vector<Staged> items(3 * n + 2);
+  items[0].bytes = n * sizeof(WavUtt);
+  items[1].bytes = n * sizeof(float);
   long long max_n = 0;
-  for (int k = 0; k < 3 * n; ++k) {
-    const int i = k % n;
-    const size_t floats = k / n == 1 ? (size_t)nm * (frame0[i + 1] - frame0[i]) : (size_t)u[i].n;
-    off[k + 3] = off[k + 2] + align256(floats * sizeof(float));
+  for (int i = 0; i < n; ++i) {
+    items[2 + i].bytes = items[2 + 2 * n + i].bytes = (size_t)u[i].n * sizeof(float);
+    items[2 + n + i].bytes = (size_t)nm * (frame0[i + 1] - frame0[i]) * sizeof(float);
     max_n = std::max<long long>(max_n, u[i].n);
   }
   WRNN_CUDA_OK(cudaSetDevice(h->engine->device));
-  int rc = grow(&h->d_audio, &h->audio_bytes, off[3 * n + 2]);
+  int rc = grow(&h->d_audio, &h->audio_bytes, staged_bytes(items));
   if (rc != WRNN_OK) return rc;
-  char* d = static_cast<char*>(h->d_audio);
-  auto region = [&](int kind, int i) { return reinterpret_cast<float*>(d + off[2 + kind * n + i]); };
+  std::vector<void*> d;
+  if ((rc = place(h->d_audio, items, st, d)) != WRNN_OK) return rc;
+  auto region = [&](int kind, int i) { return static_cast<float*>(d[2 + kind * n + i]); };
   std::vector<WavUtt> wu(n);
   std::vector<wrnn_mel_utt> mu(n);
   std::vector<wrnn_score_utt> su(n);
@@ -926,9 +908,9 @@ static int score_wav_many(wrnn_t* h, const wrnn_mel_t* m, const wrnn_score_wav_u
     mu[i] = wrnn_mel_utt{region(0, i), u[i].n, region(1, i)};
     su[i] = wrnn_score_utt{region(1, i), frame0[i + 1] - frame0[i], region(2, i), u[i].n, u[i].nll};
   }
-  WRNN_CUDA_OK(cudaMemcpyAsync(d, wu.data(), n * sizeof(WavUtt), cudaMemcpyHostToDevice, st));
+  WRNN_CUDA_OK(cudaMemcpyAsync(d[0], wu.data(), n * sizeof(WavUtt), cudaMemcpyHostToDevice, st));
   const wrnn_cfg& c = h->engine->cfg;
-  if ((rc = wav_targets(reinterpret_cast<const WavUtt*>(d), n, max_n, reinterpret_cast<float*>(d + off[1]), peak_norm, c.mode,
+  if ((rc = wav_targets(static_cast<const WavUtt*>(d[0]), n, max_n, static_cast<float*>(d[1]), peak_norm, c.mode,
                         c.n_classes, mu_law, st)) != WRNN_OK)
     return rc;
   if ((rc = wrnn_melspectrogram_many(m, mu.data(), n, st)) != WRNN_OK) return rc;
@@ -999,13 +981,9 @@ int wrnn_debug_score_wav_targets(const float* y, int64_t n, int32_t mode, int32_
                                  int32_t mu_law, float* yn, float* x, float* peak, void* stream) {
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   const WavUtt w{y, n, yn, x};
-  void* d = nullptr;
-  WRNN_CUDA_OK(cudaMallocAsync(&d, sizeof(WavUtt), st));
-  WRNN_CUDA_OK(cudaMemcpyAsync(d, &w, sizeof(WavUtt), cudaMemcpyHostToDevice, st));
-  const int rc = wav_targets(static_cast<const WavUtt*>(d), 1, n, peak, peak_norm, mode, n_classes, mu_law, st);
-  if (rc != WRNN_OK) return rc;
-  WRNN_CUDA_OK(cudaFreeAsync(d, st));
-  return WRNN_OK;
+  return with_device_table(&w, 1, st, [&](const WavUtt* d) {
+    return wav_targets(d, 1, n, peak, peak_norm, mode, n_classes, mu_law, st);
+  });
 }
 
 }  // extern "C"

@@ -105,6 +105,18 @@ __host__ __device__ inline double dadd_rn(double a, double b) {
 #endif
 }
 
+// The utterance of a batch that owns `key` (a frame, sample or block of the launch): the last of utts[0 .. n) whose
+// `first` (its first frame, sample, ...; ascending, utts[0]'s <= key) is <= key.
+template <class U>
+__device__ __forceinline__ int find_utt(const U* utts, int n, long long key, long long U::*first) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (utts[mid].*first <= key) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
 // -------------------------------------------------------------------------------------
 // Philox4x32-10 (Salmon et al. 2011), counter-based: (seed) x (step, fold, lane, offset)
 // -------------------------------------------------------------------------------------

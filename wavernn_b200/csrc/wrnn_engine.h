@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <string>
+#include <vector>
 
 #include "../../include/wavernn_b200.h"
 #include "wrnn_fold.h"
@@ -27,6 +28,70 @@ inline int grid_stride_blocks(long long blocks) {
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   const long long cap = 8ll * (n_sm > 0 ? n_sm : 1);
   return (int)(blocks < cap ? blocks : cap);
+}
+
+// Staging of the host-memory entry points.  place puts each item at a 256-B-aligned offset of the device buffer d
+// (staged_bytes(items) long) and copies it there on st (cudaMemcpyDefault: src may be host or device memory; src NULL:
+// a region the job writes); dev[k] is item k's device address, NULL for an empty item.  copy_back copies results back
+// (host or device destinations) on stream 0 and synchronises.  Static, so that none is exported by the library.
+struct Staged { const void* src; size_t bytes; };
+struct Unstaged { void* dst; const void* src; size_t bytes; };
+static inline size_t align256(size_t bytes) { return (bytes + 255) & ~size_t(255); }
+
+static inline size_t staged_bytes(const std::vector<Staged>& items) {
+  size_t total = 0;
+  for (const Staged& it : items) total += align256(it.bytes);
+  return total;
+}
+
+static inline int place(void* d, const std::vector<Staged>& items, cudaStream_t st, std::vector<void*>& dev) {
+  char* p = static_cast<char*>(d);
+  dev.assign(items.size(), nullptr);
+  for (size_t k = 0; k < items.size(); ++k) {
+    if (!items[k].bytes) continue;
+    dev[k] = p;
+    if (items[k].src) WRNN_CUDA_OK(cudaMemcpyAsync(p, items[k].src, items[k].bytes, cudaMemcpyDefault, st));
+    p += align256(items[k].bytes);
+  }
+  return WRNN_OK;
+}
+
+static inline int copy_back(const std::vector<Unstaged>& items) {
+  for (const Unstaged& it : items)
+    if (it.bytes) WRNN_CUDA_OK(cudaMemcpyAsync(it.dst, it.src, it.bytes, cudaMemcpyDefault, 0));
+  WRNN_CUDA_OK(cudaStreamSynchronize(0));
+  return WRNN_OK;
+}
+
+// A host-memory entry point of the analysis object (wrnn_mel_t): the items staged in one device allocation of this
+// call alone, so that calls on any streams share the object, and freed on every path.  run(dev, out) launches on
+// stream 0 with the items' device addresses and sets out[k] for each item k whose region copy_back returns.
+template <class F>
+int with_staging(int device, const std::vector<Staged>& items, F run) {
+  WRNN_CUDA_OK(cudaSetDevice(device));
+  void* d = nullptr;
+  WRNN_CUDA_OK(cudaMalloc(&d, staged_bytes(items)));
+  std::vector<void*> dev;
+  std::vector<Unstaged> out(items.size(), Unstaged{nullptr, nullptr, 0});
+  int rc = place(d, items, 0, dev);
+  if (rc == WRNN_OK) rc = run(dev, out);
+  if (rc == WRNN_OK) rc = copy_back(out);
+  cudaFree(d);
+  return rc;
+}
+
+// A launch whose table of n utterances lives on the device for that launch only, allocated and freed in stream order
+// on st, so that calls on any streams share one analysis object.  launch(d_tab) enqueues on st.
+template <class T, class F>
+int with_device_table(const T* tab, size_t n, cudaStream_t st, F launch) {
+  const size_t bytes = n * sizeof(T);
+  void* d = nullptr;
+  WRNN_CUDA_OK(cudaMallocAsync(&d, bytes, st));
+  WRNN_CUDA_OK(cudaMemcpyAsync(d, tab, bytes, cudaMemcpyHostToDevice, st));
+  const int rc = launch(static_cast<const T*>(d));
+  if (rc != WRNN_OK) return rc;
+  WRNN_CUDA_OK(cudaFreeAsync(d, st));
+  return WRNN_OK;
 }
 
 // ---- live session (wrnn_live_open / _submit / _cancel / _poll / _close; DESIGN §3.7) ------------------------------------

@@ -174,12 +174,7 @@ struct FrameUtt {          // one entry of the frame table: utterance i owns fra
 __global__ void __launch_bounds__(THREADS) mel_frames_kernel(Tabs tb, const FrameUtt* __restrict__ utts, int n_utts) {
   extern __shared__ double2 sm[];   // [2][n_fft / 2]; the magnitudes reuse the free half
   const long long f = blockIdx.x;
-  int lo = 0, hi = n_utts - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (utts[mid].frame0 <= f) lo = mid; else hi = mid - 1;
-  }
-  const FrameUtt u = utts[lo];
+  const FrameUtt u = utts[find_utt(utts, n_utts, f, &FrameUtt::frame0)];
   const long long t = f - u.frame0;
   const int H = tb.n_fft / 2;
   double2 *in = sm, *out = sm + H;
@@ -239,14 +234,11 @@ static int launch(const wrnn_mel_plan& m, const wrnn_mel_utt* u, int n, const st
   std::vector<FrameUtt> tab(n);
   for (int i = 0; i < n; ++i) tab[i] = FrameUtt{u[i].y, u[i].n, u[i].mel, frame0[i + 1] - frame0[i], frame0[i]};
   WRNN_CUDA_OK(cudaSetDevice(m.device));
-  // the table lives for this launch only, so that calls on any streams share the analysis object
-  void* d = nullptr;
-  WRNN_CUDA_OK(cudaMallocAsync(&d, tab.size() * sizeof(FrameUtt), st));
-  WRNN_CUDA_OK(cudaMemcpyAsync(d, tab.data(), tab.size() * sizeof(FrameUtt), cudaMemcpyHostToDevice, st));
-  mel_frames_kernel<<<(unsigned)frame0[n], THREADS, smem_bytes(m.cfg.n_fft), st>>>(device_view(m), static_cast<FrameUtt*>(d), n);
-  WRNN_CUDA_OK(cudaGetLastError());
-  WRNN_CUDA_OK(cudaFreeAsync(d, st));
-  return WRNN_OK;
+  return with_device_table(tab.data(), tab.size(), st, [&](const FrameUtt* d) {
+    mel_frames_kernel<<<(unsigned)frame0[n], THREADS, smem_bytes(m.cfg.n_fft), st>>>(device_view(m), d, n);
+    WRNN_CUDA_OK(cudaGetLastError());
+    return WRNN_OK;
+  });
 }
 
 // ---- Griffin-Lim: the inverse of the analysis (DESIGN.md §3.9) -------------------------------------------------------
@@ -440,22 +432,13 @@ struct GLScratch {          // per frame of a launch batch, indexed by frame - t
   double* frames;           // [n_fft], the windowed inverse transform
 };
 
-__device__ inline int find_utt(const GLUtt* utts, int n, long long f, bool by_sample) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if ((by_sample ? utts[mid].sample0 : utts[mid].frame0) <= f) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
 __global__ void __launch_bounds__(THREADS) gl_nnls_kernel(Tabs tb, GLTabs g, const GLUtt* __restrict__ utts, int n,
                                                           float* __restrict__ S) {
   extern __shared__ double sd[];   // b [M] | z [M] | r [M] | x [nb] | y [nb]
   const int M = tb.n_mels, nb = tb.n_fft / 2 + 1;
   double *b = sd, *z = b + M, *r = z + M, *x = r + M, *y = x + nb;
   const long long f = utts[0].frame0 + blockIdx.x;
-  const GLUtt u = utts[find_utt(utts, n, f, false)];
+  const GLUtt u = utts[find_utt(utts, n, f, &GLUtt::frame0)];
   const long long t = f - u.frame0;
   for (int m = threadIdx.x; m < M; m += THREADS) b[m] = nnls_rhs(tb, u.mel[(long long)m * u.T + t]);
   __syncthreads();
@@ -482,7 +465,7 @@ __global__ void __launch_bounds__(THREADS) gl_frames_kernel(Tabs tb, const GLUtt
   extern __shared__ double2 sm[];   // [2][n_fft / 2]; the products S * angles (complex64) reuse the free half
   const int H = tb.n_fft / 2, nb = H + 1;
   const long long f = utts[0].frame0 + blockIdx.x;
-  const GLUtt u = utts[find_utt(utts, n, f, false)];
+  const GLUtt u = utts[find_utt(utts, n, f, &GLUtt::frame0)];
   const long long t = f - u.frame0;
   const float* S = s.S + (size_t)blockIdx.x * nb;
   double2 *in = sm, *out = sm + H;
@@ -519,7 +502,7 @@ __global__ void __launch_bounds__(THREADS) gl_ola_kernel(Tabs tb, const GLUtt* _
                                                          long long n_samples) {
   const long long j = utts[0].sample0 + (long long)blockIdx.x * THREADS + threadIdx.x;
   if (j >= utts[0].sample0 + n_samples) return;
-  const GLUtt u = utts[find_utt(utts, n, j, true)];
+  const GLUtt u = utts[find_utt(utts, n, j, &GLUtt::sample0)];
   const double* fr = frames + (size_t)(u.frame0 - utts[0].frame0) * tb.n_fft;
   u.wav[j - u.sample0] = gl_ola(tb, fr, u.T, j - u.sample0 + tb.n_fft / 2);
 }
@@ -527,7 +510,7 @@ __global__ void __launch_bounds__(THREADS) gl_ola_kernel(Tabs tb, const GLUtt* _
 static size_t nnls_smem(const wrnn_mel_cfg& c) { return (size_t)(3 * c.n_mels + 2 * (c.n_fft / 2 + 1)) * sizeof(double); }
 static size_t gl_frame_bytes(int n_fft) {
   const size_t nb = n_fft / 2 + 1;
-  return ((nb * sizeof(float) + 255) & ~size_t(255)) + ((nb * sizeof(float2) + 255) & ~size_t(255)) + n_fft * sizeof(double);
+  return align256(nb * sizeof(float)) + align256(nb * sizeof(float2)) + n_fft * sizeof(double);
 }
 
 static GLTabs gl_device_view(const wrnn_mel_plan& m) {
@@ -574,8 +557,8 @@ static int gl_launch(const wrnn_mel_plan& m, const wrnn_gl_utt* u, int n, int n_
     biggest = std::max<long long>(biggest, frame0[i + 1] - frame0[first.back()]);
   }
   first.push_back(n);
-  const size_t tab_bytes = (n * sizeof(GLUtt) + 255) & ~size_t(255);
-  const size_t S_bytes = (nb * sizeof(float) + 255) & ~size_t(255), P_bytes = (nb * sizeof(float2) + 255) & ~size_t(255);
+  const size_t tab_bytes = align256(n * sizeof(GLUtt));
+  const size_t S_bytes = align256(nb * sizeof(float)), P_bytes = align256(nb * sizeof(float2));
   WRNN_CUDA_OK(cudaSetDevice(m.device));
   char* d = nullptr;
   if (cudaMallocAsync(reinterpret_cast<void**>(&d), tab_bytes + (size_t)biggest * per_frame, st) != cudaSuccess) {
@@ -688,31 +671,20 @@ int wrnn_melspectrogram_many_host(const wrnn_mel_t* m, const wrnn_mel_utt* u, in
   int rc = mel::plan(m->cfg, u, n_utts, frame0);
   if (rc != WRNN_OK) return rc;
   const int n = n_utts;
-  // one device block [y_0 | .. | y_{n-1} | mel_0 | ..], each region 256-B aligned
-  std::vector<size_t> off(2 * n + 1, 0);
-  for (int i = 0; i < 2 * n; ++i) {
-    const size_t bytes = i < n ? (size_t)u[i].n * sizeof(float) : (size_t)m->cfg.n_mels * (frame0[i - n + 1] - frame0[i - n]) * sizeof(float);
-    off[i + 1] = off[i] + ((bytes + 255) & ~size_t(255));
+  std::vector<Staged> in(2 * n);                       // [recordings | mels]
+  for (int i = 0; i < n; ++i) {
+    in[i] = {u[i].y, (size_t)u[i].n * sizeof(float)};
+    in[n + i] = {nullptr, (size_t)m->cfg.n_mels * (frame0[i + 1] - frame0[i]) * sizeof(float)};
   }
-  WRNN_CUDA_OK(cudaSetDevice(m->device));
-  char* d = nullptr;
-  WRNN_CUDA_OK(cudaMalloc(&d, off[2 * n]));
-  std::vector<wrnn_mel_utt> du(n);
-  cudaError_t e = cudaSuccess;
-  for (int i = 0; i < n && e == cudaSuccess; ++i) {
-    du[i] = wrnn_mel_utt{reinterpret_cast<float*>(d + off[i]), u[i].n, reinterpret_cast<float*>(d + off[n + i])};
-    e = cudaMemcpyAsync(d + off[i], u[i].y, (size_t)u[i].n * sizeof(float), cudaMemcpyDefault, 0);
-  }
-  if (e == cudaSuccess) {
-    rc = mel::launch(*m, du.data(), n, frame0, 0);
-    for (int i = 0; i < n && rc == WRNN_OK && e == cudaSuccess; ++i)
-      e = cudaMemcpyAsync(u[i].mel, du[i].mel, (size_t)m->cfg.n_mels * (frame0[i + 1] - frame0[i]) * sizeof(float),
-                          cudaMemcpyDefault, 0);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(0);
-  }
-  cudaFree(d);
-  if (e != cudaSuccess) { set_error(std::string("wrnn_melspectrogram_many_host: ") + cudaGetErrorString(e)); return WRNN_E_CUDA; }
-  return rc;
+  return with_staging(m->device, in, [&](const std::vector<void*>& d, std::vector<Unstaged>& out) {
+    std::vector<wrnn_mel_utt> du(u, u + n);
+    for (int i = 0; i < n; ++i) {
+      du[i].y = static_cast<float*>(d[i]);
+      du[i].mel = static_cast<float*>(d[n + i]);
+      out[n + i] = {u[i].mel, d[n + i], in[n + i].bytes};
+    }
+    return mel::launch(*m, du.data(), n, frame0, 0);
+  });
 }
 
 int wrnn_griffinlim_many(const wrnn_mel_t* m, const wrnn_gl_utt* u, int32_t n_utts, int32_t n_iter, void* stream) {
@@ -730,30 +702,20 @@ int wrnn_griffinlim_many_host(const wrnn_mel_t* m, const wrnn_gl_utt* u, int32_t
   if (rc != WRNN_OK) return rc;
   const int n = n_utts;
   const long long M = m->cfg.n_mels, hop = m->cfg.hop_length;
-  // one device block [mel_0 | .. | mel_{n-1} | wav_0 | ..], each region 256-B aligned
-  std::vector<size_t> off(2 * n + 1, 0);
-  for (int i = 0; i < 2 * n; ++i) {
-    const size_t bytes = (i < n ? (size_t)(M * u[i].T) : (size_t)(hop * (u[i - n].T - 1))) * sizeof(float);
-    off[i + 1] = off[i] + ((bytes + 255) & ~size_t(255));
+  std::vector<Staged> in(2 * n);                       // [mels | waveforms]
+  for (int i = 0; i < n; ++i) {
+    in[i] = {u[i].mel, (size_t)(M * u[i].T) * sizeof(float)};
+    in[n + i] = {nullptr, (size_t)(hop * (u[i].T - 1)) * sizeof(float)};
   }
-  WRNN_CUDA_OK(cudaSetDevice(m->device));
-  char* d = nullptr;
-  WRNN_CUDA_OK(cudaMalloc(&d, off[2 * n]));
-  std::vector<wrnn_gl_utt> du(n);
-  cudaError_t e = cudaSuccess;
-  for (int i = 0; i < n && e == cudaSuccess; ++i) {
-    du[i] = wrnn_gl_utt{reinterpret_cast<float*>(d + off[i]), u[i].T, u[i].phase_seed, reinterpret_cast<float*>(d + off[n + i])};
-    e = cudaMemcpyAsync(d + off[i], u[i].mel, (size_t)(M * u[i].T) * sizeof(float), cudaMemcpyDefault, 0);
-  }
-  if (e == cudaSuccess) {
-    rc = mel::gl_launch(*m, du.data(), n, n_iter, frame0, 0);
-    for (int i = 0; i < n && rc == WRNN_OK && e == cudaSuccess; ++i)
-      e = cudaMemcpyAsync(u[i].wav, du[i].wav, (size_t)(hop * (u[i].T - 1)) * sizeof(float), cudaMemcpyDefault, 0);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(0);
-  }
-  cudaFree(d);
-  if (e != cudaSuccess) { set_error(std::string("wrnn_griffinlim_many_host: ") + cudaGetErrorString(e)); return WRNN_E_CUDA; }
-  return rc;
+  return with_staging(m->device, in, [&](const std::vector<void*>& d, std::vector<Unstaged>& out) {
+    std::vector<wrnn_gl_utt> du(u, u + n);
+    for (int i = 0; i < n; ++i) {
+      du[i].mel = static_cast<float*>(d[i]);
+      du[i].wav = static_cast<float*>(d[n + i]);
+      out[n + i] = {u[i].wav, d[n + i], in[n + i].bytes};
+    }
+    return mel::gl_launch(*m, du.data(), n, n_iter, frame0, 0);
+  });
 }
 
 // ---- test hooks (not declared in the header) ------------------------------------------------------------------------

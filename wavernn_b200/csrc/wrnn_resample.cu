@@ -133,12 +133,7 @@ __global__ void __launch_bounds__(THREADS) resample_kernel(const double* __restr
                                                            int n_utts, int stage_cap) {
   extern __shared__ float xs[];
   const long long b = blockIdx.x;
-  int lo_u = 0, hi_u = n_utts - 1;
-  while (lo_u < hi_u) {
-    const int mid = (lo_u + hi_u + 1) >> 1;
-    if (utts[mid].block0 <= b) lo_u = mid; else hi_u = mid - 1;
-  }
-  const RsUtt u = utts[lo_u];
+  const RsUtt u = utts[find_utt(utts, n_utts, b, &RsUtt::block0)];
   const long long t0 = (b - u.block0) * THREADS, t = t0 + threadIdx.x;
   if (u.copy) {
     if (t < u.n_len) u.y[t] = u.x[t];
@@ -236,14 +231,11 @@ static int launch(const wrnn_mel_plan& m, std::vector<RsUtt> tab, cudaStream_t s
   const RsUtt& last = tab.back();
   const long long blocks = last.block0 + (last.n_len + THREADS - 1) / THREADS;
   const int cap = stage_cap(tab);
-  // the table lives for this launch only, so that calls on any streams share the analysis object
-  void* d = nullptr;
-  WRNN_CUDA_OK(cudaMallocAsync(&d, n * sizeof(RsUtt), st));
-  WRNN_CUDA_OK(cudaMemcpyAsync(d, tab.data(), n * sizeof(RsUtt), cudaMemcpyHostToDevice, st));
-  resample_kernel<<<(unsigned)blocks, THREADS, (size_t)cap * sizeof(float), st>>>(m.d_rs_win, static_cast<RsUtt*>(d), n, cap);
-  WRNN_CUDA_OK(cudaGetLastError());
-  WRNN_CUDA_OK(cudaFreeAsync(d, st));
-  return WRNN_OK;
+  return with_device_table(tab.data(), tab.size(), st, [&](const RsUtt* d) {
+    resample_kernel<<<(unsigned)blocks, THREADS, (size_t)cap * sizeof(float), st>>>(m.d_rs_win, d, n, cap);
+    WRNN_CUDA_OK(cudaGetLastError());
+    return WRNN_OK;
+  });
 }
 
 }  // namespace rs
@@ -273,31 +265,19 @@ int wrnn_resample_many_host(const wrnn_mel_t* m, const wrnn_resample_utt* u, int
   int rc = rs::plan(m->cfg.sample_rate, u, n_utts, tab);
   if (rc != WRNN_OK) return rc;
   const int n = n_utts;
-  // one device block [x_0 | .. | x_{n-1} | y_0 | ..], each region 256-B aligned
-  std::vector<size_t> off(2 * n + 1, 0);
-  for (int i = 0; i < 2 * n; ++i) {
-    const size_t bytes = (size_t)(i < n ? tab[i].n : tab[i - n].n_len) * sizeof(float);
-    off[i + 1] = off[i] + ((bytes + 255) & ~size_t(255));
+  std::vector<Staged> in(2 * n);                       // [recordings | outputs]
+  for (int i = 0; i < n; ++i) {
+    in[i] = {u[i].x, (size_t)tab[i].n * sizeof(float)};
+    in[n + i] = {nullptr, (size_t)tab[i].n_len * sizeof(float)};
   }
-  WRNN_CUDA_OK(cudaSetDevice(m->device));
-  char* d = nullptr;
-  WRNN_CUDA_OK(cudaMalloc(&d, off[2 * n]));
-  std::vector<rs::RsUtt> dtab = tab;
-  cudaError_t e = cudaSuccess;
-  for (int i = 0; i < n && e == cudaSuccess; ++i) {
-    dtab[i].x = reinterpret_cast<float*>(d + off[i]);
-    dtab[i].y = reinterpret_cast<float*>(d + off[n + i]);
-    e = cudaMemcpyAsync(d + off[i], u[i].x, (size_t)u[i].n * sizeof(float), cudaMemcpyDefault, 0);
-  }
-  if (e == cudaSuccess) {
-    rc = rs::launch(*m, dtab, 0);
-    for (int i = 0; i < n && rc == WRNN_OK && e == cudaSuccess; ++i)
-      e = cudaMemcpyAsync(u[i].y, dtab[i].y, (size_t)tab[i].n_len * sizeof(float), cudaMemcpyDefault, 0);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(0);
-  }
-  cudaFree(d);
-  if (e != cudaSuccess) { set_error(std::string("wrnn_resample_many_host: ") + cudaGetErrorString(e)); return WRNN_E_CUDA; }
-  return rc;
+  return with_staging(m->device, in, [&](const std::vector<void*>& d, std::vector<Unstaged>& out) {
+    for (int i = 0; i < n; ++i) {
+      tab[i].x = static_cast<float*>(d[i]);
+      tab[i].y = static_cast<float*>(d[n + i]);
+      out[n + i] = {u[i].y, d[n + i], in[n + i].bytes};
+    }
+    return rs::launch(*m, tab, 0);
+  });
 }
 
 // ---- test hooks (not declared in the header) ------------------------------------------------------------------------
