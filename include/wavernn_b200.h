@@ -405,7 +405,27 @@ int wrnn_live_open(wrnn_t *h, int32_t capacity, int64_t max_T, int32_t mu_law, v
  * every slot holds an utterance (there is no host queue): poll until one is released. */
 int wrnn_live_submit(wrnn_t *h, const wrnn_utterance *u, int64_t *ticket);
 
-/* Cancels a ticket: its slot stops at the next boundary and is released by a later poll (state CANCELLED). */
+/* Submits one utterance for BATCHED generation (wrnn_vocode_job with batched = 1, target, overlap): its n_seg folds
+ * (fold_with_overlap's geometry) each take a free slot of the session and are admitted into the running kernel, each at
+ * the next boundary it is seen (not necessarily the same one).  Fold b's draws are keyed by (philox_seed, b), as
+ * wrnn_vocode's are, and every fold runs target + 2 * overlap steps.
+ *
+ * Contract: the ticket's delivered wav is bit-identical to wrnn_vocode_host on the same handle with {mel, T, batched = 1,
+ * target, overlap, mu_law = the session's, philox_seed}, whatever its slots, the boundaries its folds were admitted at,
+ * the launches that served them and whatever else was in flight.  Sample n is final once every fold whose window
+ * [b * (target + overlap), + target + 2 * overlap) covers n has stored its sample for n; n_ready is the longest final
+ * prefix (fold 0's samples lead it, one per step, so the waveform starts to play as early as an unbatched ticket's).
+ * It never decreases and a delivered sample is never rewritten.  A batched ticket is ONE wrnn_live_ticket:
+ * wrnn_live_cancel cancels all its folds, and wrnn_live_poll releases all its slots together, once every fold has
+ * retired, and only then reports it DONE or CANCELLED.
+ *
+ * Refused (WRNN_E_INVALID, with a message; the handle and the session are unchanged): those of wrnn_live_submit;
+ * target <= 0 or overlap <= 0; more folds than the session's capacity (it could never be admitted); target + 2 * overlap
+ * > (max_T - 1) * hop (a fold's samples would not fit a slot's row).  WRNN_E_BUSY, taking no slot, while fewer slots
+ * are free than the utterance has folds: poll until enough are released. */
+int wrnn_live_submit_batched(wrnn_t *h, const wrnn_utterance *u, int32_t target, int32_t overlap, int64_t *ticket);
+
+/* Cancels a ticket: its slots stop at the next boundary and are released by a later poll (state CANCELLED). */
 int wrnn_live_cancel(wrnn_t *h, int64_t ticket);
 
 /* Waits up to wait_us for progress, writes every newly final sample into its ticket's wav and reports in out[0 ..

@@ -26,8 +26,8 @@ EXPORTS = ("wrnn_abi_version", "wrnn_last_error", "wrnn_create", "wrnn_destroy",
            "wrnn_attach_upsampler", "wrnn_conditioning_frames", "wrnn_vocode", "wrnn_vocode_host",
            "wrnn_vocode_many", "wrnn_vocode_many_host", "wrnn_score", "wrnn_score_many", "wrnn_score_many_host",
            "wrnn_vocode_live_start", "wrnn_vocode_live_poll", "wrnn_vocode_many_live_start",
-           "wrnn_vocode_many_live_poll", "wrnn_live_open", "wrnn_live_submit", "wrnn_live_cancel", "wrnn_live_poll",
-           "wrnn_live_close", "wrnn_mel_create", "wrnn_mel_destroy", "wrnn_melspectrogram_many",
+           "wrnn_vocode_many_live_poll", "wrnn_live_open", "wrnn_live_submit", "wrnn_live_submit_batched",
+           "wrnn_live_cancel", "wrnn_live_poll", "wrnn_live_close", "wrnn_mel_create", "wrnn_mel_destroy", "wrnn_melspectrogram_many",
            "wrnn_melspectrogram_many_host", "wrnn_score_wav_many", "wrnn_score_wav_many_host", "wrnn_griffinlim_many",
            "wrnn_griffinlim_many_host", "wrnn_resample_length", "wrnn_resample_many", "wrnn_resample_many_host")
 LIVE_RUNNING, LIVE_DONE, LIVE_CANCELLED = 0, 1, 2
@@ -226,6 +226,8 @@ def load() -> C.CDLL:
     lib.wrnn_live_open.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_void_p]
     lib.wrnn_live_submit.restype = C.c_int
     lib.wrnn_live_submit.argtypes = [C.c_void_p, C.POINTER(WrnnUtterance), C.POINTER(C.c_int64)]
+    lib.wrnn_live_submit_batched.restype = C.c_int
+    lib.wrnn_live_submit_batched.argtypes = [C.c_void_p, C.POINTER(WrnnUtterance), C.c_int32, C.c_int32, C.POINTER(C.c_int64)]
     lib.wrnn_live_cancel.restype = C.c_int
     lib.wrnn_live_cancel.argtypes = [C.c_void_p, C.c_int64]
     lib.wrnn_live_poll.restype = C.c_int
@@ -288,6 +290,19 @@ def load() -> C.CDLL:
     lib.wrnn_debug_live_session_slot.restype = C.c_int
     lib.wrnn_debug_live_session_slot.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.c_int32, C.c_uint32, C.c_uint32,
                                                  C.c_uint64, C.c_int64, C.c_void_p]
+    lib.wrnn_debug_live_batched_deliver.restype = C.c_int
+    lib.wrnn_debug_live_batched_deliver.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int64, C.c_int64,
+                                                    C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                                    C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.wrnn_debug_live_batched_relaunch.restype = C.c_int
+    lib.wrnn_debug_live_batched_relaunch.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32,
+                                                     C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                                     C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.wrnn_debug_live_post_limit.restype = C.c_int
+    lib.wrnn_debug_live_post_limit.argtypes = [C.c_void_p, C.c_int32]
+    lib.wrnn_debug_live_session_fold_slot.restype = C.c_int
+    lib.wrnn_debug_live_session_fold_slot.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.c_int32, C.c_uint32, C.c_uint32,
+                                                      C.c_uint64, C.c_int64, C.c_uint32, C.c_int32, C.c_int32, C.c_void_p]
     lib.wrnn_debug_live_many_deliver.restype = C.c_int
     lib.wrnn_debug_live_many_deliver.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
                                                  C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
@@ -668,10 +683,12 @@ class MelAnalysis:
 
 
 class LiveSession:
-    """wrnn_live_*: submit(mel, philox_seed) -> ticket at any time; poll() yields (ticket, slice) for each newly final
-    slice of a ticket's float64 waveform (views of one array per ticket; their concatenation is bit-identical to
-    vocode_host(mel, batched=False, mu_law=mu_law, philox_seed=philox_seed)); cancel(ticket); close().  `waves` maps
-    each ticket to its array, `states` to its last reported state (LIVE_*)."""
+    """wrnn_live_*: submit(mel, philox_seed) or submit_batched(mel, philox_seed, target, overlap) -> ticket at any time;
+    poll() yields (ticket, slice) for each newly final slice of a ticket's float64 waveform (views of one array per
+    ticket; their concatenation is bit-identical to vocode_host(mel, batched=False, mu_law=mu_law,
+    philox_seed=philox_seed), or for a batched ticket to vocode_host(mel, batched=True, target=target, overlap=overlap,
+    mu_law=mu_law, philox_seed=philox_seed)); cancel(ticket); close().  `waves` maps each ticket to its array, `states`
+    to its last reported state (LIVE_*)."""
 
     def __init__(self, engine: Engine, capacity: int, max_T: int, mu_law: bool = False):
         self.engine, self.lib, self.capacity = engine, engine.lib, int(capacity)
@@ -686,6 +703,17 @@ class LiveSession:
         u = WrnnUtterance(mel.ctypes.data, mel.shape[-1], int(philox_seed), wav.ctypes.data)
         tk = C.c_int64(0)
         _check(self.lib, self.lib.wrnn_live_submit(self.engine._h, C.byref(u), C.byref(tk)))
+        t = int(tk.value)
+        self.waves[t], self._mels[t], self._prev[t], self.states[t] = wav, mel, 0, LIVE_RUNNING
+        return t
+
+    def submit_batched(self, mel, *, philox_seed: int, target: int = 11000, overlap: int = 550) -> int:
+        """Submits mel (80, T) numpy for batched generation: each of its folds takes a free slot.  Returns its ticket.
+        Raises EngineError(WRNN_E_BUSY) when fewer slots are free than it has folds."""
+        mel, wav = self.engine._mel_and_wav(mel)
+        u = WrnnUtterance(mel.ctypes.data, mel.shape[-1], int(philox_seed), wav.ctypes.data)
+        tk = C.c_int64(0)
+        _check(self.lib, self.lib.wrnn_live_submit_batched(self.engine._h, C.byref(u), int(target), int(overlap), C.byref(tk)))
         t = int(tk.value)
         self.waves[t], self._mels[t], self._prev[t], self.states[t] = wav, mel, 0, LIVE_RUNNING
         return t

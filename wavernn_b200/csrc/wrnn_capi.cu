@@ -1,6 +1,7 @@
 // wrnn_capi.cu -- the extern "C" surface declared in include/wavernn_b200.h.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <cstdlib>
@@ -91,19 +92,19 @@ static int unstage(wrnn_t* h, const std::vector<Unstaged>& items) {
   return rc != WRNN_OK ? rc : h->last->check();
 }
 
-// The host epilogue's tables (wrnn_vocode's unbatched geometry): mu is empty unless mu-law applies, which it does on a
-// RAW head only.
+// The host epilogue's tables (wrnn_vocode's geometry: unbatched with overlap 0, else batched): mu is empty unless mu-law
+// applies, which it does on a RAW head only.
 struct LiveTables {
-  std::vector<double> mu, tail;
+  std::vector<double> mu, tail, fade_in, fade_out;
   long long tail_len = 0;
-  int n_classes = 0;
+  int n_classes = 0, overlap = 0;
 };
-static LiveTables live_tables(int mode, bool mu_law, int n_classes, int hop) {
+static LiveTables live_tables(int mode, bool mu_law, int n_classes, int hop, int overlap = 0) {
   LiveTables t;
-  std::vector<double> fade_in, fade_out;
-  cond::epilogue_tables(0, mu_law && mode == WRNN_MODE_RAW, n_classes, hop, fade_in, fade_out, t.mu, t.tail);
+  cond::epilogue_tables(overlap, mu_law && mode == WRNN_MODE_RAW, n_classes, hop, t.fade_in, t.fade_out, t.mu, t.tail);
   t.tail_len = 20ll * hop;
   t.n_classes = n_classes;
+  t.overlap = overlap;
   return t;
 }
 
@@ -994,19 +995,31 @@ int wrnn_debug_score_wav_targets(const float* y, int64_t n, int32_t mode, int32_
 // wrnn_vocode_many_live_start / _poll: the same for an unbatched wrnn_vocode_many of up to 64 utterances, one fold each,
 // in one tile; each fold publishes its own progress.
 // ---------------------------------------------------------------------------------------------------------------------
-// wrnn_epilogue_kernel in the unbatched geometry, on the host: samples [n0, n1) of x -> wav.  The same operations in the
-// same order: the mu-law label recovered in fp32 and rounded half to even (saturating, NaN -> 0, then clamped), 0.0 + y
-// (a -0.0 sample becomes +0.0), then the fade-out over the last tail_len samples.
-static void live_epilogue(const LiveTables& t, const float* x, long long n0, long long n1, long long wave_len, double* wav) {
-  const int nc = t.n_classes;
-  for (long long n = n0; n < n1; ++n) {
-    const float xf = x[n];
+// wrnn_epilogue_kernel on the host: samples [n0, n1) of a waveform of wave_len samples unfolded from x[0 .. n_seg), fold
+// b's seg_len samples starting at waveform sample b * stride (unbatched: one fold, stride = seg_len >= wave_len).  The
+// same operations in the same order: per fold sample, the mu-law label recovered in fp32 and rounded half to even
+// (saturating, NaN -> 0, then clamped), times fade_in on the fold's first overlap samples and fade_out on its last; per
+// waveform sample 0.0 + the earlier fold's sample + the later one's (a -0.0 sample becomes +0.0), then the fade-out over
+// the last tail_len samples.
+static void live_epilogue(const LiveTables& t, const float* const* x, int n_seg, long long seg_len, long long stride, long long n0,
+                          long long n1, long long wave_len, double* wav) {
+  const int nc = t.n_classes, ov = t.overlap;
+  auto value = [&](long long i, long long k) {
+    const float xf = x[i][k];
     double y = (double)xf;
     if (!t.mu.empty()) {
       const float r = std::nearbyint((xf + 1.0f) * (0.5f * (float)(nc - 1)));
       y = t.mu[!(r > 0.f) ? 0 : (r >= (float)(nc - 1) ? nc - 1 : (int)r)];
     }
-    double v = 0.0 + y;
+    if (k < ov) y *= t.fade_in[k];
+    if (k >= seg_len - ov) y *= t.fade_out[k - (seg_len - ov)];
+    return y;
+  };
+  for (long long n = n0; n < n1; ++n) {
+    const long long i = std::min(n / stride, (long long)n_seg - 1), k = n - i * stride;
+    double v = 0.0;
+    if (i >= 1 && k + stride < seg_len) v += value(i - 1, k + stride);
+    if (k < seg_len) v += value(i, k);
     if (n >= wave_len - t.tail_len) v *= t.tail[n - (wave_len - t.tail_len)];
     wav[n] = v;
   }
@@ -1018,7 +1031,7 @@ static bool live_deliver_one(const LiveTables& t, const float* x, long long coun
                              double* wav) {
   const long long ready = count < wave_len ? count : wave_len;
   if (ready <= delivered) return false;
-  live_epilogue(t, x, delivered, ready, wave_len, wav);
+  live_epilogue(t, &x, 1, wave_len, wave_len, delivered, ready, wave_len, wav);
   delivered = ready;
   return true;
 }
@@ -1196,7 +1209,7 @@ int wrnn_debug_live_epilogue(const float* x, int64_t n, int64_t wave_len, int32_
   if (!x || !wav || hop <= 0 || n < 0 || n > wave_len || wave_len < 20ll * hop || (mu_law && n_classes < 2)) {
     set_error("bad argument"); return WRNN_E_INVALID;
   }
-  live_epilogue(live_tables(WRNN_MODE_RAW, mu_law != 0, n_classes, hop), x, 0, n, wave_len, wav);
+  live_epilogue(live_tables(WRNN_MODE_RAW, mu_law != 0, n_classes, hop), &x, 1, wave_len, wave_len, 0, n, wave_len, wav);
   return WRNN_OK;
 }
 
@@ -1278,10 +1291,11 @@ int wrnn_debug_stream_plan(const wrnn_cfg* cfg, const wrnn_weights* w, uint8_t* 
 
 // ---------------------------------------------------------------------------------------------------------------------
 // wrnn_live_open .. wrnn_live_close: a live session.  Slot s of the persistent tile owns region s of the frame arena, row
-// s of the pinned sample block, progress word s and mailbox s.  The host picks a free slot, writes the utterance's
-// conditioning frames into its region on a side stream and, once they are complete, posts the request to the mailbox; CTA
-// 0 admits it at the next boundary (DESIGN §3.7).  A launch that has exited is relaunched with the posted requests
-// admitted at its step 0.
+// s of the pinned sample block, progress word s and mailbox s.  A ticket holds one slot per fold: an unbatched one a single
+// fold, a batched one the n_seg folds of fold_with_overlap.  The host picks free slots, writes the utterance's conditioning
+// frames into the region of the ticket's first slot on a side stream and, once they are complete, posts each fold's
+// request to its slot's mailbox; CTA 0 admits each at the next boundary it sees it (DESIGN §3.7).  A launch that has
+// exited is relaunched with the posted requests admitted at its step 0.
 // ---------------------------------------------------------------------------------------------------------------------
 namespace wrnn {
 struct LiveSession {
@@ -1290,15 +1304,20 @@ struct LiveSession {
   static constexpr size_t SAMPLES_OFF = 4096;     // [progress words | mailboxes | pad | samples [C][max_steps]]
   static_assert(MAIL_OFF + MAX_SLOTS * sizeof(SesMail) <= SAMPLES_OFF, "pinned layout");
   enum { FREE, PREP, POSTED };
-  struct Slot {
+  // A ticket, kept at the index of its first slot.  Fold b runs seg_len steps from arena row row0 + b * stride (rows
+  // past `rows` read as zeros), covers waveform samples [b * stride, + seg_len) and is held by slot slot[b].
+  struct Ticket {
     int state = FREE;
     long long ticket = 0;
     unsigned tag = 0;
     unsigned long long seed = 0;
     long long wave_len = 0, delivered = 0;
+    long long seg_len = 0, stride = 0, row0 = 0, rows = 0;
+    std::vector<int> slot;
+    int posted = 0;                  // folds 0 .. posted - 1 have their request in their slot's mailbox
+    LiveTables tabs;                 // the session's, or a batched ticket's own (its overlap's fade tables)
     double* wav = nullptr;
     bool cancelled = false;
-    cudaEvent_t ready = nullptr;     // the slot's conditioning frames are complete
   };
   int C = 0, hop = 0;
   long long max_T = 0, max_steps = 0;
@@ -1313,42 +1332,87 @@ struct LiveSession {
   size_t stage_pitch = 0;
   cudaEvent_t done = nullptr;                        // recorded after the running launch
   bool running = false;
-  std::vector<Slot> slots;
+  std::vector<Ticket> tickets;                       // [C]: the ticket whose first slot is s, if any
+  std::vector<int> owner;                            // [C]: the first slot of the ticket holding slot s, or -1
+  std::vector<cudaEvent_t> ready;                    // [C]: the frames of the ticket whose first slot is s are complete
   std::vector<SesEntry> tab;                         // host image of the table for a launch: [2][64], version -1 in buffer 1
   long long next_ticket = 1;
-  std::vector<wrnn_live_ticket> released;            // tickets whose slot was released since the last poll
+  int post_limit = MAX_SLOTS;                        // folds posted by one pump at most (wrnn_debug_live_post_limit)
+  std::vector<wrnn_live_ticket> released;            // tickets whose slots were released since the last poll
   unsigned long long* progress() const { return static_cast<unsigned long long*>(host); }
   SesMail* mail() const { return reinterpret_cast<SesMail*>(static_cast<char*>(host) + MAIL_OFF); }
   const float* samples(int s) const {
     return reinterpret_cast<const float*>(static_cast<const char*>(host) + SAMPLES_OFF) + (size_t)s * max_steps;
   }
-  void release(Slot& sl) {
-    released.push_back(wrnn_live_ticket{sl.ticket, sl.delivered,
-                                        (!sl.cancelled && sl.delivered == sl.wave_len) ? WRNN_LIVE_DONE : WRNN_LIVE_CANCELLED, 0});
-    const cudaEvent_t ev = sl.ready;
-    sl = Slot();
-    sl.ready = ev;
+  // Releases all of a ticket's slots at once: a retired fold's samples stay in its slot's row until the prefix has
+  // passed them.
+  void release(Ticket& tk) {
+    released.push_back(wrnn_live_ticket{tk.ticket, tk.delivered,
+                                        (!tk.cancelled && tk.delivered == tk.wave_len) ? WRNN_LIVE_DONE : WRNN_LIVE_CANCELLED, 0});
+    for (const int s : tk.slot) owner[s] = -1;
+    tk = Ticket();
   }
 };
 
-// Delivers, per posted slot, the samples its occupant has published (words of an earlier occupant of the slot carry
-// another tag and are ignored) and releases the slots whose occupant CTA 0 retired.  Returns whether anything changed.
+// Delivers, per posted ticket, the longest prefix of its waveform whose every sample each covering fold has published
+// (words of an earlier occupant of a slot carry another tag and count as nothing published), and releases the tickets
+// whose every fold CTA 0 retired (a cancelled ticket: every fold it posted).  Returns whether anything changed.
 static bool session_deliver(LiveSession& ss) {
   bool more = false;
-  for (int s = 0; s < ss.C; ++s) {
-    LiveSession::Slot& sl = ss.slots[s];
-    if (sl.state != LiveSession::POSTED) continue;
-    const unsigned long long w = __atomic_load_n(ss.progress() + s, __ATOMIC_ACQUIRE);
-    if ((unsigned)(w >> 32) != sl.tag) continue;
-    const long long count = (long long)(w & (SES_RETIRED - 1u));
-    if (!sl.cancelled && live_deliver_one(ss.tabs, ss.samples(s), count, sl.wave_len, sl.delivered, sl.wav)) more = true;
-    if (w & SES_RETIRED) { ss.release(sl); more = true; }
+  for (LiveSession::Ticket& tk : ss.tickets) {
+    if (tk.state != LiveSession::POSTED) continue;
+    const int n_seg = (int)tk.slot.size();
+    long long ready = tk.wave_len;
+    bool retired = tk.posted == n_seg || tk.cancelled;
+    const float* x[LiveSession::MAX_SLOTS];
+    for (int b = 0; b < n_seg; ++b) {
+      const unsigned long long w = __atomic_load_n(ss.progress() + tk.slot[b], __ATOMIC_ACQUIRE);
+      const bool mine = (unsigned)(w >> 32) == tk.tag;
+      const long long count = mine ? (long long)(w & (SES_RETIRED - 1u)) : 0;
+      if (b < tk.posted) retired = retired && mine && (w & SES_RETIRED);
+      if (count < tk.seg_len) ready = std::min(ready, b * tk.stride + count);
+      x[b] = ss.samples(tk.slot[b]);
+    }
+    if (!tk.cancelled && ready > tk.delivered) {
+      live_epilogue(tk.tabs, x, n_seg, tk.seg_len, tk.stride, tk.delivered, ready, tk.wave_len, tk.wav);
+      tk.delivered = ready;
+      more = true;
+    }
+    if (retired) { ss.release(tk); more = true; }
   }
   return more;
 }
 
-// Posts the slots whose frames are complete, and relaunches the kernel when the last launch has exited and a posted
-// request was not admitted by it.
+// A relaunch's decision for one posted ticket (no launch runs, so every fold a launch admitted has retired).  Each posted
+// fold whose slot carries the ticket's tag has finished, whatever launch served it; the others were never admitted.
+// Those go into version -1 of the table, admitted at step 0 with the ticket's tag written to their progress words, or
+// are withdrawn if the ticket is cancelled, which then releases it.  Its folds may so be served by several launches: a
+// launch exits at a boundary where no slot is held, which can fall between two folds' posts.  Sets `launch` when a
+// fold was admitted; WRNN_E_CUDA if a fold with the ticket's tag is not retired.
+static int relaunch_ticket(LiveSession& ss, LiveSession::Ticket& tk, bool& launch) {
+  for (int b = 0; b < tk.posted; ++b) {
+    const int s = tk.slot[b];
+    const unsigned long long w = __atomic_load_n(ss.progress() + s, __ATOMIC_ACQUIRE);
+    if ((unsigned)(w >> 32) == tk.tag) {
+      if (w & SES_RETIRED) continue;
+      set_error("live session: a launch exited with slot " + std::to_string(s) + " still held");
+      return WRNN_E_CUDA;
+    }
+    if (tk.cancelled) {
+      __atomic_store_n(&ss.mail()[s].req, w >> 32, __ATOMIC_RELEASE);
+      continue;
+    }
+    ss.tab[LiveSession::MAX_SLOTS + s] = SesEntry{0, (int)tk.seg_len, tk.seed, (unsigned)b, (int)(tk.row0 + b * tk.stride),
+                                                  (int)(tk.rows - b * tk.stride), 0};
+    __atomic_store_n(ss.progress() + s, (unsigned long long)tk.tag << 32, __ATOMIC_RELEASE);
+    launch = true;
+  }
+  if (tk.cancelled) ss.release(tk);
+  return WRNN_OK;
+}
+
+// Posts the folds of the tickets whose frames are complete (at most post_limit per call), and relaunches the kernel when
+// the last launch has exited and a posted request was not admitted by it.
 static int session_pump(LiveSession& ss) {
   if (ss.running) {
     const cudaError_t q = cudaEventQuery(ss.done);
@@ -1363,39 +1427,34 @@ static int session_pump(LiveSession& ss) {
     }
   }
   for (int s = 0; s < ss.C; ++s) {
-    LiveSession::Slot& sl = ss.slots[s];
-    if (sl.state != LiveSession::PREP) continue;
-    const cudaError_t q = cudaEventQuery(sl.ready);
+    LiveSession::Ticket& tk = ss.tickets[s];
+    if (tk.state != LiveSession::PREP) continue;
+    const cudaError_t q = cudaEventQuery(ss.ready[s]);
     if (q == cudaErrorNotReady) continue;
     if (q != cudaSuccess) { set_error(std::string("live session: conditioning: ") + cudaGetErrorString(q)); return WRNN_E_CUDA; }
-    if (sl.cancelled) { ss.release(sl); continue; }
-    SesMail& m = ss.mail()[s];
-    m.seed = sl.seed;
-    m.steps = sl.wave_len;
-    __atomic_store_n(&m.req, (unsigned long long)sl.tag, __ATOMIC_RELEASE);   // the body before the tag
-    sl.state = LiveSession::POSTED;
+    if (tk.cancelled) { ss.release(tk); continue; }
+    tk.state = LiveSession::POSTED;
+  }
+  int budget = ss.post_limit;
+  for (LiveSession::Ticket& tk : ss.tickets) {
+    for (; tk.state == LiveSession::POSTED && !tk.cancelled && tk.posted < (int)tk.slot.size() && budget > 0; ++tk.posted, --budget) {
+      const int b = tk.posted;
+      SesMail& m = ss.mail()[tk.slot[b]];
+      m.seed = tk.seed;
+      m.steps = tk.seg_len;
+      m.fold = (unsigned)b;
+      m.row0 = (int)(tk.row0 + b * tk.stride);
+      m.rows = (int)(tk.rows - b * tk.stride);
+      __atomic_store_n(&m.req, (unsigned long long)tk.tag, __ATOMIC_RELEASE);   // the body before the tag
+    }
   }
   if (ss.running) return WRNN_OK;
-  // No launch runs: every slot it admitted is retired and released.  A posted request it did not admit is admitted at
-  // step 0 of the next launch (version -1 of the table), or withdrawn if cancelled.
   bool launch = false;
-  for (int s = 0; s < LiveSession::MAX_SLOTS; ++s) ss.tab[LiveSession::MAX_SLOTS + s] = SesEntry{0, 0, 0ull};
-  for (int s = 0; s < ss.C; ++s) {
-    LiveSession::Slot& sl = ss.slots[s];
-    if (sl.state != LiveSession::POSTED) continue;
-    const unsigned long long w = __atomic_load_n(ss.progress() + s, __ATOMIC_ACQUIRE);
-    if ((unsigned)(w >> 32) == sl.tag) {
-      set_error("live session: a launch exited with slot " + std::to_string(s) + " still held");
-      return WRNN_E_CUDA;
-    }
-    if (sl.cancelled) {
-      __atomic_store_n(&ss.mail()[s].req, w >> 32, __ATOMIC_RELEASE);
-      ss.release(sl);
-      continue;
-    }
-    ss.tab[LiveSession::MAX_SLOTS + s] = SesEntry{0, (int)sl.wave_len, sl.seed};
-    __atomic_store_n(ss.progress() + s, (unsigned long long)sl.tag << 32, __ATOMIC_RELEASE);
-    launch = true;
+  for (int s = 0; s < LiveSession::MAX_SLOTS; ++s) ss.tab[LiveSession::MAX_SLOTS + s] = SesEntry{};
+  for (LiveSession::Ticket& tk : ss.tickets) {
+    if (tk.state != LiveSession::POSTED) continue;
+    const int rc = relaunch_ticket(ss, tk, launch);
+    if (rc != WRNN_OK) return rc;
   }
   if (!launch) return WRNN_OK;
   WRNN_CUDA_OK(cudaSetDevice(ss.e->device));
@@ -1420,11 +1479,66 @@ static int session_pump(LiveSession& ss) {
 static void session_free(LiveSession* ss) {
   if (ss->done) { cudaEventSynchronize(ss->done); cudaEventDestroy(ss->done); }
   if (ss->side) { cudaStreamSynchronize(ss->side); cudaStreamDestroy(ss->side); }
-  for (auto& sl : ss->slots) if (sl.ready) cudaEventDestroy(sl.ready);
+  for (const cudaEvent_t ev : ss->ready) if (ev) cudaEventDestroy(ev);
   if (ss->host) cudaFreeHost(ss->host);
   cudaFree(ss->d_ctl);
   cudaFree(ss->d_arena);
   delete ss;
+}
+
+// The refusals shared by both submits, then the open session of h (nullptr after a refusal).
+static LiveSession* submit_session(wrnn_t* h, const wrnn_utterance* u) {
+  if (!h || !h->engine) { set_error("null handle"); return nullptr; }
+  if (!h->session) { set_error("no live session is open on this handle (wrnn_live_open)"); return nullptr; }
+  if (u->T > h->session->max_T) { set_error("T exceeds the session's max_T (" + std::to_string(h->session->max_T) + ")"); return nullptr; }
+  return h->session;
+}
+
+// Both submits, after their refusals: g is the ticket's fold geometry (unbatched: one fold of wave_len steps).  Takes
+// g.n_seg free slots (none when fewer are free), runs the conditioning network into the first one's region on the side
+// stream and records that slot's ready event; session_pump posts the folds once it has completed.
+static int session_submit(wrnn_t* h, const wrnn_utterance* u, const cond::Geometry& g, LiveTables tabs, int64_t* ticket) {
+  LiveSession& ss = *h->session;
+  int rc = session_pump(ss);                           // releases what has finished, so that its slots can be reused
+  if (rc != WRNN_OK) return rc;
+  session_deliver(ss);
+  std::vector<int> slot;
+  for (int s = 0; s < ss.C && (long long)slot.size() < g.n_seg; ++s)
+    if (ss.owner[s] < 0) slot.push_back(s);
+  if ((long long)slot.size() < g.n_seg) {
+    set_error(g.n_seg == 1 ? "all " + std::to_string(ss.C) + " slots of the live session hold an utterance: poll until one is released"
+                           : std::to_string(slot.size()) + " of the live session's " + std::to_string(ss.C) + " slots are free and the utterance has " +
+                                 std::to_string(g.n_seg) + " folds: poll until enough are released");
+    return WRNN_E_BUSY;
+  }
+  WRNN_CUDA_OK(cudaSetDevice(ss.e->device));
+  const int s0 = slot[0];
+  float* stage = ss.mel_stage + (size_t)s0 * ss.stage_pitch;
+  const size_t frame0 = (size_t)s0 * (ss.max_T + 4);
+  WRNN_CUDA_OK(cudaMemcpyAsync(stage, u->mel, (size_t)u->T * FEAT * sizeof(float), cudaMemcpyDefault, ss.side));
+  if ((rc = conditioning_frames(*h->upsampler, stage, u->T, ss.mel_frames + frame0 * FEAT, ss.aux_frames + frame0 * cond::CD,
+                                nullptr, ss.side)) != WRNN_OK)
+    return rc;
+  WRNN_CUDA_OK(cudaEventRecord(ss.ready[s0], ss.side));
+  LiveSession::Ticket& tk = ss.tickets[s0];
+  tk.state = LiveSession::PREP;
+  tk.ticket = ss.next_ticket++;
+  tk.tag = ses_tag(tk.ticket);
+  tk.seed = u->philox_seed;
+  tk.wave_len = (u->T - 1) * ss.hop;
+  tk.delivered = 0;
+  tk.seg_len = g.seg_len;
+  tk.stride = g.seg_stride;
+  tk.row0 = (long long)frame0 * ss.hop;
+  tk.rows = u->T * ss.hop;
+  tk.slot = slot;
+  tk.posted = 0;
+  tk.tabs = std::move(tabs);
+  tk.wav = u->wav;
+  tk.cancelled = false;
+  for (const int s : slot) ss.owner[s] = s0;
+  *ticket = tk.ticket;
+  return session_pump(ss);
 }
 }  // namespace wrnn
 
@@ -1450,8 +1564,10 @@ int wrnn_live_open(wrnn_t* h, int32_t capacity, int64_t max_T, int32_t mu_law, v
   ss->C = capacity; ss->hop = hop; ss->max_T = max_T; ss->max_steps = (max_T - 1) * hop;
   ss->tabs = live_tables(h->engine->cfg.mode, mu_law != 0, h->engine->cfg.n_classes, hop);
   ss->e = h->engine; ss->st = static_cast<cudaStream_t>(stream); ss->taps = h->upsampler->d_taps;
-  ss->slots.resize(capacity);
-  ss->tab.assign(2 * LiveSession::MAX_SLOTS, SesEntry{0, 0, 0ull});
+  ss->tickets.resize(capacity);
+  ss->owner.assign(capacity, -1);
+  ss->ready.assign(capacity, nullptr);
+  ss->tab.assign(2 * LiveSession::MAX_SLOTS, SesEntry{});
   auto fail = [&](int code) { session_free(ss); return code; };
 #define SES_OK(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { set_error(std::string(#expr) + " failed: " + cudaGetErrorString(_e)); return fail(WRNN_E_CUDA); } } while (0)
   SES_OK(cudaSetDevice(h->engine->device));
@@ -1469,7 +1585,7 @@ int wrnn_live_open(wrnn_t* h, int32_t capacity, int64_t max_T, int32_t mu_law, v
   ss->mel_stage = ss->aux_frames + n_af;
   SES_OK(cudaStreamCreateWithFlags(&ss->side, cudaStreamNonBlocking));
   SES_OK(cudaEventCreateWithFlags(&ss->done, cudaEventDisableTiming));
-  for (auto& sl : ss->slots) SES_OK(cudaEventCreateWithFlags(&sl.ready, cudaEventDisableTiming));
+  for (auto& ev : ss->ready) SES_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
 #undef SES_OK
   h->session = ss;
   return WRNN_OK;
@@ -1477,52 +1593,46 @@ int wrnn_live_open(wrnn_t* h, int32_t capacity, int64_t max_T, int32_t mu_law, v
 
 int wrnn_live_submit(wrnn_t* h, const wrnn_utterance* u, int64_t* ticket) {
   if (!u || !ticket) { set_error("null utterance or ticket"); return WRNN_E_INVALID; }
-  int rc = check_utterance("", u->mel, u->wav, u->T);
+  const int rc = check_utterance("", u->mel, u->wav, u->T);
   if (rc != WRNN_OK) return rc;
-  if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
-  if (!h->session) { set_error("no live session is open on this handle (wrnn_live_open)"); return WRNN_E_INVALID; }
-  LiveSession& ss = *h->session;
-  if (u->T > ss.max_T) { set_error("T exceeds the session's max_T (" + std::to_string(ss.max_T) + ")"); return WRNN_E_INVALID; }
-  rc = session_pump(ss);                               // releases what has finished, so that its slot can be reused
+  LiveSession* ss = submit_session(h, u);
+  if (!ss) return WRNN_E_INVALID;
+  const long long wave_len = (u->T - 1) * ss->hop;
+  return session_submit(h, u, cond::Geometry{1, wave_len, wave_len, 0, wave_len}, ss->tabs, ticket);
+}
+
+int wrnn_live_submit_batched(wrnn_t* h, const wrnn_utterance* u, int32_t target, int32_t overlap, int64_t* ticket) {
+  if (!u || !ticket) { set_error("null utterance or ticket"); return WRNN_E_INVALID; }
+  const int rc = check_utterance("", u->mel, u->wav, u->T);
   if (rc != WRNN_OK) return rc;
-  session_deliver(ss);
-  int s = 0;
-  while (s < ss.C && ss.slots[s].state != LiveSession::FREE) ++s;
-  if (s == ss.C) {
-    set_error("all " + std::to_string(ss.C) + " slots of the live session hold an utterance: poll until one is released");
-    return WRNN_E_BUSY;
+  if (target <= 0 || overlap <= 0) { set_error("a batched ticket needs target > 0 and overlap > 0"); return WRNN_E_INVALID; }
+  LiveSession* ss = submit_session(h, u);
+  if (!ss) return WRNN_E_INVALID;
+  const cond::Geometry g = cond::fold_geometry(u->T * ss->hop, true, target, overlap);
+  if (g.n_seg < 1) { set_error("target / overlap give no fold"); return WRNN_E_INVALID; }
+  if (g.n_seg > ss->C) {
+    set_error("the utterance has " + std::to_string(g.n_seg) + " folds, more than the session's " + std::to_string(ss->C) +
+              " slots: it could never be admitted");
+    return WRNN_E_INVALID;
   }
-  WRNN_CUDA_OK(cudaSetDevice(ss.e->device));
-  float* stage = ss.mel_stage + (size_t)s * ss.stage_pitch;
-  const size_t frame0 = (size_t)s * (ss.max_T + 4);
-  WRNN_CUDA_OK(cudaMemcpyAsync(stage, u->mel, (size_t)u->T * FEAT * sizeof(float), cudaMemcpyDefault, ss.side));
-  if ((rc = conditioning_frames(*h->upsampler, stage, u->T, ss.mel_frames + frame0 * FEAT, ss.aux_frames + frame0 * cond::CD,
-                                nullptr, ss.side)) != WRNN_OK)
-    return rc;
-  LiveSession::Slot& sl = ss.slots[s];
-  WRNN_CUDA_OK(cudaEventRecord(sl.ready, ss.side));
-  sl.state = LiveSession::PREP;
-  sl.ticket = ss.next_ticket++;
-  sl.tag = ses_tag(sl.ticket);
-  sl.seed = u->philox_seed;
-  sl.wave_len = (u->T - 1) * ss.hop;
-  sl.delivered = 0;
-  sl.wav = u->wav;
-  sl.cancelled = false;
-  *ticket = sl.ticket;
-  return session_pump(ss);
+  if (g.seg_len > ss->max_steps) {
+    set_error("a fold's target + 2 * overlap = " + std::to_string(g.seg_len) + " samples exceed a slot's row of (max_T - 1) * hop = " +
+              std::to_string(ss->max_steps));
+    return WRNN_E_INVALID;
+  }
+  return session_submit(h, u, g, live_tables(ss->e->cfg.mode, !ss->tabs.mu.empty(), ss->e->cfg.n_classes, ss->hop, overlap),
+                        ticket);
 }
 
 int wrnn_live_cancel(wrnn_t* h, int64_t ticket) {
   if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
   if (!h->session) { set_error("no live session is open on this handle (wrnn_live_open)"); return WRNN_E_INVALID; }
   LiveSession& ss = *h->session;
-  for (int s = 0; s < ss.C; ++s) {
-    LiveSession::Slot& sl = ss.slots[s];
-    if (sl.state == LiveSession::FREE || sl.ticket != ticket) continue;
-    if (!sl.cancelled) {
-      sl.cancelled = true;
-      if (sl.state == LiveSession::POSTED) __atomic_store_n(&ss.mail()[s].cancel, (unsigned long long)sl.tag, __ATOMIC_RELEASE);
+  for (LiveSession::Ticket& tk : ss.tickets) {
+    if (tk.state == LiveSession::FREE || tk.ticket != ticket) continue;
+    if (!tk.cancelled) {
+      tk.cancelled = true;
+      for (int b = 0; b < tk.posted; ++b) __atomic_store_n(&ss.mail()[tk.slot[b]].cancel, (unsigned long long)tk.tag, __ATOMIC_RELEASE);
     }
     return WRNN_OK;
   }
@@ -1548,10 +1658,10 @@ int wrnn_live_poll(wrnn_t* h, int32_t wait_us, wrnn_live_ticket* out, int32_t ma
   size_t k = 0;
   for (; k < ss.released.size() && n < max_out - ss.C; ++k) out[n++] = ss.released[k];
   ss.released.erase(ss.released.begin(), ss.released.begin() + k);   // the rest: next poll
-  for (const auto& sl : ss.slots) {
-    if (sl.state == LiveSession::FREE) continue;
+  for (const auto& tk : ss.tickets) {
+    if (tk.state == LiveSession::FREE) continue;
     ++held;
-    out[n++] = wrnn_live_ticket{sl.ticket, sl.delivered, WRNN_LIVE_RUNNING, 0};
+    out[n++] = wrnn_live_ticket{tk.ticket, tk.delivered, WRNN_LIVE_RUNNING, 0};
   }
   *n_out = n;
   return held > 0 ? 1 : 0;
@@ -1561,16 +1671,14 @@ int wrnn_live_close(wrnn_t* h) {
   if (!h || !h->engine) { set_error("null handle"); return WRNN_E_INVALID; }
   if (!h->session) { set_error("no live session is open on this handle (wrnn_live_open)"); return WRNN_E_INVALID; }
   LiveSession* ss = h->session;
-  for (int s = 0; s < ss->C; ++s) {
-    LiveSession::Slot& sl = ss->slots[s];
-    if (sl.state != LiveSession::FREE && !sl.cancelled) wrnn_live_cancel(h, sl.ticket);
-  }
+  for (const auto& tk : ss->tickets)
+    if (tk.state != LiveSession::FREE && !tk.cancelled) wrnn_live_cancel(h, tk.ticket);
   const std::optional<int> rc = wait_for(-1, [&]() -> std::optional<int> {   // the launch stops once every cancelled slot is retired
     const int rc = session_pump(*ss);
     if (rc != WRNN_OK) return rc;
     session_deliver(*ss);
     bool held = false;
-    for (const auto& sl : ss->slots) held = held || sl.state != LiveSession::FREE;
+    for (const auto& tk : ss->tickets) held = held || tk.state != LiveSession::FREE;
     return (!held && !ss->running) ? std::optional<int>(WRNN_OK) : std::nullopt;
   });
   h->session = nullptr;
@@ -1599,24 +1707,128 @@ int wrnn_debug_live_session_deliver(const float* x, int64_t max_steps, const uin
   LiveSession ss;
   ss.host = buf.data();
   ss.C = C; ss.hop = hop; ss.max_steps = max_steps;
-  ss.tabs = live_tables(WRNN_MODE_RAW, mu_law != 0, n_classes, hop);
-  ss.slots.resize(C);
+  ss.tickets.resize(C);
+  ss.owner.assign(C, -1);
+  const LiveTables tabs = live_tables(WRNN_MODE_RAW, mu_law != 0, n_classes, hop);
   double* w = wav;
   for (int s = 0; s < C; ++s) {
     if (!ticket[s]) continue;
-    LiveSession::Slot& sl = ss.slots[s];
-    sl.state = LiveSession::POSTED; sl.ticket = ticket[s]; sl.tag = ses_tag(ticket[s]);
-    sl.wave_len = (T[s] - 1) * hop; sl.delivered = delivered[s]; sl.wav = w;
-    w += sl.wave_len;
+    LiveSession::Ticket& tk = ss.tickets[s];
+    tk.state = LiveSession::POSTED; tk.ticket = ticket[s]; tk.tag = ses_tag(ticket[s]);
+    tk.wave_len = (T[s] - 1) * hop; tk.seg_len = tk.stride = tk.wave_len; tk.delivered = delivered[s]; tk.wav = w;
+    tk.slot = {s}; tk.posted = 1; tk.tabs = tabs;
+    ss.owner[s] = s;
+    w += tk.wave_len;
   }
   session_deliver(ss);
   for (int s = 0; s < C; ++s) {
     released[s] = 0;
     if (!ticket[s]) continue;
     for (const auto& r : ss.released) if (r.ticket == ticket[s]) { released[s] = 1; delivered[s] = r.n_ready; }
-    if (!released[s]) delivered[s] = ss.slots[s].delivered;
+    if (!released[s]) delivered[s] = ss.tickets[s].delivered;
   }
   ss.host = nullptr;
+  return WRNN_OK;
+}
+
+// Test hook (CPU-only, no device needed): one delivery of wrnn_live_poll for ONE batched ticket (T frames, target,
+// overlap), on a host buffer laid out as the session's pinned one of C slots: fold b is held by slot slot[b] (n_seg
+// entries, fold_with_overlap's count), its samples are row slot[b] of x [C][max_steps] and its published word
+// progress[slot[b]].  *delivered holds what earlier polls delivered and receives what this one did; *released whether the
+// ticket was released, and free_slots [C] whether each slot is free afterwards.  Checked in tests/test_live_batched_abi.py.
+int wrnn_debug_live_batched_deliver(const float* x, int64_t max_steps, const uint64_t* progress, int32_t C, int64_t ticket,
+                                    int64_t T, int32_t target, int32_t overlap, const int32_t* slot, int32_t n_seg, int32_t hop,
+                                    int32_t mu_law, int32_t n_classes, int64_t* delivered, int32_t* released,
+                                    int32_t* free_slots, double* wav) {
+  if (!x || !progress || !slot || !delivered || !released || !free_slots || !wav || max_steps <= 0 || hop <= 0 || C < 1 ||
+      C > LiveSession::MAX_SLOTS || T < 21 || target <= 0 || overlap <= 0 || (mu_law && n_classes < 2)) {
+    set_error("bad argument"); return WRNN_E_INVALID;
+  }
+  const cond::Geometry g = cond::fold_geometry(T * hop, true, target, overlap);
+  if (g.n_seg != n_seg || g.seg_len > max_steps || *delivered < 0 || *delivered > (T - 1) * hop) { set_error("bad argument"); return WRNN_E_INVALID; }
+  std::vector<int> owner(C, -1);
+  for (int b = 0; b < n_seg; ++b) {
+    if (slot[b] < 0 || slot[b] >= C || owner[slot[b]] >= 0) { set_error("bad argument"); return WRNN_E_INVALID; }
+    owner[slot[b]] = slot[0];
+  }
+  std::vector<unsigned char> buf(LiveSession::SAMPLES_OFF + (size_t)C * max_steps * sizeof(float));
+  std::memcpy(buf.data(), progress, (size_t)C * sizeof(uint64_t));
+  std::memcpy(buf.data() + LiveSession::SAMPLES_OFF, x, (size_t)C * max_steps * sizeof(float));
+  LiveSession ss;
+  ss.host = buf.data();
+  ss.C = C; ss.hop = hop; ss.max_steps = max_steps;
+  ss.tickets.resize(C);
+  ss.owner = owner;
+  LiveSession::Ticket& tk = ss.tickets[slot[0]];
+  tk.state = LiveSession::POSTED; tk.ticket = ticket; tk.tag = ses_tag(ticket);
+  tk.wave_len = (T - 1) * hop; tk.seg_len = g.seg_len; tk.stride = g.seg_stride; tk.delivered = *delivered; tk.wav = wav;
+  tk.slot.assign(slot, slot + n_seg);
+  tk.posted = n_seg;
+  tk.tabs = live_tables(WRNN_MODE_RAW, mu_law != 0, n_classes, hop, overlap);
+  session_deliver(ss);
+  *released = ss.released.empty() ? 0 : 1;
+  *delivered = ss.released.empty() ? tk.delivered : ss.released[0].n_ready;
+  for (int s = 0; s < C; ++s) free_slots[s] = ss.owner[s] < 0 ? 1 : 0;
+  ss.host = nullptr;
+  return WRNN_OK;
+}
+
+// Test hook (CPU-only, no device needed): a relaunch's decision for ONE posted batched ticket (T frames, target, overlap;
+// cancelled or not) on a session of C slots whose launch has exited: fold b is held by slot slot[b] (n_seg entries) and
+// folds 0 .. posted - 1 were posted.  progress [C] holds each slot's word and receives what the host wrote; req [C]
+// receives each slot's mailbox tag (0 where nothing was posted or withdrawn); entry [C][4] the version -1 table entry of
+// each slot (steps, fold, row0 - the ticket's first row, rows; steps 0: not admitted); *launch whether a launch is
+// needed, *released whether the ticket was released.  Returns the decision's code (WRNN_E_CUDA: a fold still held).
+// Checked in tests/test_live_batched_abi.py.
+int wrnn_debug_live_batched_relaunch(uint64_t* progress, int32_t C, int64_t ticket, int64_t T, int32_t target, int32_t overlap,
+                                     const int32_t* slot, int32_t n_seg, int32_t posted, int32_t cancelled, int32_t hop,
+                                     uint64_t* req, int64_t* entry, int32_t* launch, int32_t* released) {
+  if (!progress || !slot || !req || !entry || !launch || !released || C < 1 || C > LiveSession::MAX_SLOTS || T < 21 ||
+      target <= 0 || overlap <= 0 || hop <= 0 || posted < 0 || posted > n_seg) {
+    set_error("bad argument"); return WRNN_E_INVALID;
+  }
+  const cond::Geometry g = cond::fold_geometry(T * hop, true, target, overlap);
+  if (g.n_seg != n_seg) { set_error("bad argument"); return WRNN_E_INVALID; }
+  std::vector<int> owner(C, -1);
+  for (int b = 0; b < n_seg; ++b) {
+    if (slot[b] < 0 || slot[b] >= C || owner[slot[b]] >= 0) { set_error("bad argument"); return WRNN_E_INVALID; }
+    owner[slot[b]] = slot[0];
+  }
+  std::vector<unsigned char> buf(LiveSession::SAMPLES_OFF, 0);
+  std::memcpy(buf.data(), progress, (size_t)C * sizeof(uint64_t));
+  LiveSession ss;
+  ss.host = buf.data();
+  ss.C = C; ss.hop = hop;
+  ss.tickets.resize(C);
+  ss.owner = owner;
+  ss.tab.assign(2 * LiveSession::MAX_SLOTS, SesEntry{});
+  for (int b = 0; b < posted; ++b) ss.mail()[slot[b]].req = ses_tag(ticket);
+  LiveSession::Ticket& tk = ss.tickets[slot[0]];
+  tk.state = LiveSession::POSTED; tk.ticket = ticket; tk.tag = ses_tag(ticket);
+  tk.wave_len = (T - 1) * hop; tk.seg_len = g.seg_len; tk.stride = g.seg_stride; tk.rows = T * hop;
+  tk.slot.assign(slot, slot + n_seg);
+  tk.posted = posted;
+  tk.cancelled = cancelled != 0;
+  bool go = false;
+  const int rc = relaunch_ticket(ss, tk, go);
+  std::memcpy(progress, buf.data(), (size_t)C * sizeof(uint64_t));
+  for (int s = 0; s < C; ++s) {
+    const SesEntry& e = ss.tab[LiveSession::MAX_SLOTS + s];
+    req[s] = ss.mail()[s].req;
+    entry[4 * s] = e.e - e.a; entry[4 * s + 1] = e.fold; entry[4 * s + 2] = e.row0; entry[4 * s + 3] = e.rows;
+  }
+  *launch = go ? 1 : 0;
+  *released = ss.released.empty() ? 0 : 1;
+  ss.host = nullptr;
+  return rc;
+}
+
+// Test hook (device tests): at most n folds are posted per pass of the open session's host loop on h (a submit makes one,
+// a poll one per 100 us of its wait, one with wait_us <= 0), so that a ticket's folds reach the kernel at different
+// boundaries or launches.  The default is 64.
+int wrnn_debug_live_post_limit(wrnn_t* h, int32_t n) {
+  if (!h || !h->session || n < 1) { set_error("bad argument: an open live session and n >= 1"); return WRNN_E_INVALID; }
+  h->session->post_limit = n;
   return WRNN_OK;
 }
 
@@ -1631,8 +1843,28 @@ int wrnn_debug_live_session_slot(int64_t* state, uint64_t* seed, int32_t b, uint
   SesSlot s{(unsigned)state[0], (int)state[1], (int)state[2], *seed, state[3] != 0};
   words[0] = ses_retire_cancel(s, b, cancel_tag);
   words[1] = 0;
-  if (ses_admits(s, b, req_tag)) words[1] = ses_admit(s, b, req_tag, req_seed, req_steps);
+  if (ses_admits(s, b, req_tag)) words[1] = ses_admit(s, b, req_tag, req_seed, req_steps, 0u, 0, (int)req_steps);
   state[0] = s.tag; state[1] = s.a; state[2] = s.e; state[3] = s.retired ? 1 : 0;
+  *seed = s.seed;
+  return WRNN_OK;
+}
+
+// Test hook (CPU-only): the same decision for a slot whose occupant (and request) is a fold of a batched utterance.
+// state = {tag, a, e, retired, fold, row0, rows}; the request's fold, first row and row count are req_fold, req_row0 and
+// req_rows.
+int wrnn_debug_live_session_fold_slot(int64_t* state, uint64_t* seed, int32_t b, uint32_t req_tag, uint32_t cancel_tag,
+                                      uint64_t req_seed, int64_t req_steps, uint32_t req_fold, int32_t req_row0, int32_t req_rows,
+                                      uint64_t* words) {
+  if (!state || !seed || !words || b < 0 || b % SES_PERIOD || req_steps < 1 || req_steps > SES_MAX_STEPS || req_row0 < 0 ||
+      req_rows < 1) {
+    set_error("bad argument"); return WRNN_E_INVALID;
+  }
+  SesSlot s{(unsigned)state[0], (int)state[1], (int)state[2], *seed, state[3] != 0, (unsigned)state[4], (int)state[5], (int)state[6]};
+  words[0] = ses_retire_cancel(s, b, cancel_tag);
+  words[1] = 0;
+  if (ses_admits(s, b, req_tag)) words[1] = ses_admit(s, b, req_tag, req_seed, req_steps, req_fold, req_row0, req_rows);
+  state[0] = s.tag; state[1] = s.a; state[2] = s.e; state[3] = s.retired ? 1 : 0;
+  state[4] = s.fold; state[5] = s.row0; state[6] = s.rows;
   *seed = s.seed;
   return WRNN_OK;
 }

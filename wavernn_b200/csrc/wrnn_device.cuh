@@ -163,9 +163,9 @@ __device__ __forceinline__ FoldPhilox fold_philox(const FoldKey* keys, int f, in
   }
   return FoldPhilox{(unsigned)(seg_first + f), (unsigned)seed, (unsigned)(seed >> 32)};
 }
-// the key of a live-session slot: its occupant's seed, counter fold 0
-__device__ __forceinline__ FoldPhilox slot_philox(unsigned long long seed) {
-  return FoldPhilox{0u, (unsigned)seed, (unsigned)(seed >> 32)};
+// the key of a live-session slot: its occupant's seed and fold, as wrnn_vocode keys fold `fold` of an utterance
+__device__ __forceinline__ FoldPhilox slot_philox(unsigned fold, unsigned long long seed) {
+  return FoldPhilox{fold, (unsigned)seed, (unsigned)(seed >> 32)};
 }
 // The in-kernel draws of one step of a fold, the same on every tensor-core engine.  MoL: words 0-9 (mixture) and 10
 // (logistic) of Philox blocks 0-2 at counter (step, fold, block, offset), each mapped by u_ref_range.

@@ -103,16 +103,22 @@ constexpr int SES_DRAIN = 4;                        // a slot is retired at the 
 constexpr int SES_ADMIT_LIMIT = 1 << 27;            // no admission at a boundary from here on: every step index stays below 2^28
 constexpr long long SES_MAX_STEPS = 1ll << 27;      // samples of one utterance: (T - 1) * hop <= 2^27
 constexpr unsigned SES_RETIRED = 1u << 31;          // progress word: (tag << 32) | [retired bit] | samples stored
-// Slot table entry (device, [2 versions][64]): version k is written at boundary k * SES_PERIOD.
+// Slot table entry (device, [2 versions][64]): version k is written at boundary k * SES_PERIOD.  The occupant is fold
+// `fold` of its utterance (the Philox counter fold of its draws); local step ts reads arena row row0 + ts, or zeros from
+// ts = rows on (an unbatched occupant: fold 0, its region's first row, rows its steps never reach).
 struct SesEntry {
   int a, e;
   unsigned long long seed;
+  unsigned fold;
+  int row0, rows, pad;
 };
 // One slot's mailbox (mapped host memory, written by the host only): the tag of the latest request and of the latest
-// cancellation, and the request's Philox seed and step count (written before `req`).
+// cancellation, and the request's Philox seed, step count, fold and rows (written before `req`).
 struct SesMail {
   unsigned long long req, cancel, seed;
   long long steps;
+  unsigned fold;
+  int row0, rows, pad;
 };
 // A ticket's 32-bit tag in the progress word and the mailbox: never 0 (the tag of a slot that never held a request).
 inline unsigned ses_tag(long long ticket) { return (unsigned)((unsigned long long)(ticket - 1) % 0xffffffffull) + 1u; }
@@ -122,6 +128,8 @@ struct SesSlot {
   int a, e;
   unsigned long long seed;
   bool retired;
+  unsigned fold;
+  int row0, rows;
 };
 // Retirement (returns the progress word to publish, or 0) and cancellation at boundary b.
 __host__ __device__ inline unsigned long long ses_retire_cancel(SesSlot& s, int b, unsigned cancel_tag) {
@@ -137,8 +145,10 @@ __host__ __device__ inline bool ses_admits(const SesSlot& s, int b, unsigned req
   return s.retired && req_tag != s.tag && b < SES_ADMIT_LIMIT;
 }
 // Admission at boundary b: the utterance runs steps [b + SES_PERIOD, + steps).  Returns the progress word to publish.
-__host__ __device__ inline unsigned long long ses_admit(SesSlot& s, int b, unsigned req_tag, unsigned long long seed, long long steps) {
+__host__ __device__ inline unsigned long long ses_admit(SesSlot& s, int b, unsigned req_tag, unsigned long long seed, long long steps,
+                                                     unsigned fold, int row0, int rows) {
   s.tag = req_tag; s.a = b + SES_PERIOD; s.e = s.a + (int)steps; s.seed = seed; s.retired = false;
+  s.fold = fold; s.row0 = row0; s.rows = rows;
   return (unsigned long long)req_tag << 32;
 }
 struct SesCtl {
@@ -167,8 +177,8 @@ class Engine {
     set_error(live_refusal());
     return WRNN_E_INVALID;
   }
-  // One launch of a live session (same refusal): job.n_seg slots, slot f's conditioning rows from f * job.seg_stride of the
-  // frame tensors, its samples at job.out + f * job.seg_len (mapped host memory).
+  // One launch of a live session (same refusal): job.n_seg slots, slot f's conditioning rows from its table entry's row0 of
+  // the frame tensors, its samples at job.out + f * job.seg_len (mapped host memory).
   virtual int generate_session(const wrnn_job& job, cudaStream_t stream, const SesCtl& c) {
     (void)job; (void)stream; (void)c;
     set_error(live_refusal());

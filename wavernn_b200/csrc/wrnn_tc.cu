@@ -93,8 +93,8 @@ constexpr int OFF_ACC = OFF_VEC + NVEC * 4;
 constexpr int OFF_BAR = OFF_ACC + AC_COLS * ACP * 4;      // 3 mbarriers
 constexpr int SMEM_BYTES = OFF_BAR + 64;
 static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
-constexpr int OFF_SES = SMEM_BYTES;                       // SES: the staging's window (a, e) of each slot
-constexpr int SMEM_SES = OFF_SES + MT * 8;
+constexpr int OFF_SES = SMEM_BYTES;                       // SES: the staging's window of each slot (see ses_windows)
+constexpr int SMEM_SES = OFF_SES + MT * 16;
 static_assert(SMEM_SES <= 227 * 1024, "shared memory budget");
 
 struct TcParams {
@@ -184,8 +184,9 @@ __device__ __forceinline__ bool named_bar_or(int id, int nthreads, bool pred) {
   return r != 0;
 }
 __device__ __forceinline__ SesEntry ld_ses_entry(const SesEntry* e) {   // L2, never a stale L1 line of an earlier version
-  const int2 w = __ldcg(reinterpret_cast<const int2*>(e));
-  return SesEntry{w.x, w.y, __ldcg(&e->seed)};
+  static_assert(sizeof(SesEntry) == 32, "two 16-byte loads");
+  const int4 w = __ldcg(reinterpret_cast<const int4*>(e)), v = __ldcg(reinterpret_cast<const int4*>(e) + 1);
+  return SesEntry{w.x, w.y, ((unsigned long long)(unsigned)w.w << 32) | (unsigned)w.z, (unsigned)v.x, v.y, v.z, 0};
 }
 __device__ __forceinline__ void ses_publish(unsigned long long* progress, unsigned tag, int ts, int steps) {
   if ((ts + 1) % LIVE_PERIOD == 0 || ts + 1 == steps) st_release_sys_u64(progress, ((unsigned long long)tag << 32) | (unsigned)(ts + 1));
@@ -304,14 +305,16 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
     // decision state of it, held by the thread that stores the slot's samples.  The mailbox words are read one step
     // before each boundary, so that their PCIe round trip overlaps the fc3 wait.
     int sa = 0, se = 0;
+    unsigned sfold = 0;
     unsigned long long sseed = 0;
     const bool decider = SES && cta == 0 && owns_fold && slot == 0;
     SesSlot ds{0u, 0, 0, 0ull, true};
     unsigned long long m_req = 0, m_can = 0;
     if constexpr (SES) {
-      if (owns_fold) { const SesEntry en = ld_ses_entry(p.ses_tab + MT + fold); sa = en.a; se = en.e; sseed = en.seed; }
+      SesEntry en{};
+      if (owns_fold) { en = ld_ses_entry(p.ses_tab + MT + fold); sa = en.a; se = en.e; sseed = en.seed; sfold = en.fold; }
       if (decider) {
-        ds = SesSlot{(unsigned)(ld_volatile_u64(p.progress + fold) >> 32), sa, se, sseed, se <= 0};
+        ds = SesSlot{(unsigned)(ld_volatile_u64(p.progress + fold) >> 32), sa, se, sseed, se <= 0, en.fold, en.row0, en.rows};
         m_req = ld_volatile_u64(&p.ses_mail[fold].req); m_can = ld_volatile_u64(&p.ses_mail[fold].cancel);
       }
     }
@@ -331,10 +334,12 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
               asm volatile("fence.acq_rel.sys;" ::: "memory");      // the request's body after its tag
               const unsigned long long seed = ld_volatile_u64(&p.ses_mail[fold].seed);
               const long long steps = (long long)ld_volatile_u64(reinterpret_cast<const unsigned long long*>(&p.ses_mail[fold].steps));
-              st_release_sys_u64(p.progress + fold, ses_admit(ds, t, (unsigned)m_req, seed, steps));
+              const unsigned long long fr = ld_volatile_u64(reinterpret_cast<const unsigned long long*>(&p.ses_mail[fold].fold));
+              const int rows = (int)ld_volatile_u64(reinterpret_cast<const unsigned long long*>(&p.ses_mail[fold].rows));
+              st_release_sys_u64(p.progress + fold, ses_admit(ds, t, (unsigned)m_req, seed, steps, (unsigned)fr, (int)(fr >> 32), rows));
             }
             busy = !ds.retired;
-            const SesEntry en{ds.a, ds.e, ds.seed};
+            const SesEntry en{ds.a, ds.e, ds.seed, ds.fold, ds.row0, ds.rows, 0};
             p.ses_tab[((t / SES_PERIOD) & 1) * MT + fold] = en;
           }
           if (cta == 0) {
@@ -395,7 +400,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
 #pragma unroll
                 for (int i = 0; i < UT; ++i) ex[i] = __ldg(p.expo + ((size_t)t * p.n_total + p.f0 + fold) * NCLS + u0 + j0 + i);
               } else {                                        // this thread's classes share one block: 16 + cta
-                const FoldPhilox k = SES ? slot_philox(sseed) : fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
+                const FoldPhilox k = SES ? slot_philox(sfold, sseed) : fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed);
                 const Philox4 r = raw_block(k, (unsigned)ts, (unsigned)cta, (unsigned)p.offset);
 #pragma unroll
                 for (int i = 0; i < UT; ++i) ex[i] = raw_exp(r, (unsigned)(j0 + i));
@@ -422,7 +427,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
               ur[10] = __ldg(u + 10 * p.n_total + p.f0 + fold);
             }
           } else if (owns_fold) {
-            mol_uniforms(SES ? slot_philox(sseed) : fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed), (unsigned)ts, (unsigned)p.offset, ur);
+            mol_uniforms(SES ? slot_philox(sfold, sseed) : fold_philox(p.keys, p.f0 + fold, p.seg_first, p.seed), (unsigned)ts, (unsigned)p.offset, ur);
           }
           if constexpr (RAW) {
 #pragma unroll
@@ -493,7 +498,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
             // of that boundary, released by CTA 0 after it wrote the version.
             const int v = (t / SES_PERIOD) & 1;
             counter_wait(p.counters + 0, (unsigned)P * (unsigned)(t + 2 - SES_PERIOD), p.abort_flag);
-            if (owns_fold) { const SesEntry en = ld_ses_entry(p.ses_tab + v * MT + fold); sa = en.a; se = en.e; sseed = en.seed; }
+            if (owns_fold) { const SesEntry en = ld_ses_entry(p.ses_tab + v * MT + fold); sa = en.a; se = en.e; sseed = en.seed; sfold = en.fold; }
             S = __ldcg(p.ses_stop + v);
             if (decider) { m_req = ld_volatile_u64(&p.ses_mail[fold].req); m_can = ld_volatile_u64(&p.ses_mail[fold].cancel); }
           }
@@ -801,8 +806,7 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
     float4 creg[COND_TASKS][2];
     // conditioning window of fold f of this tile: the strided fold, or the caller's tables (several utterances in one job)
     // strided windows: streams are indexed from the job's first fold, frame tensors from the stream's first sample
-    int2* ses_win = reinterpret_cast<int2*>(smem + OFF_SES);
-    const unsigned ses_frames = SES ? (unsigned)(p.seg_stride / p.hop) : 0u;   // frames of a slot's region
+    int4* ses_win = reinterpret_cast<int4*>(smem + OFF_SES);
     auto row0_of = [&](int f) -> long long {
       return p.fold_row0 ? __ldg(p.fold_row0 + p.f0 + f) : (long long)(p.f0 + f + (FRAMES ? p.seg_first : 0)) * p.seg_stride - p.row_base;
     };
@@ -817,9 +821,9 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
       a = make_float4(0.f, 0.f, 0.f, 0.f); b = a;
       long long row;
       if constexpr (SES) {                                 // slot f's window in the version the staging uses
-        const int2 w = ses_win[f];
+        const int4 w = ses_win[f];
         if (n < w.x || n >= w.y) return;
-        row = (long long)f * p.seg_stride + (n - w.x);
+        row = (long long)w.z * p.hop + w.w + (n - w.x);
       } else {
         row = row0_of(f) + n;
         if (row >= end_of(f)) return;
@@ -866,16 +870,16 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
     auto cond_fetch = [&](int n) {
       if (!deferred) return;
       if constexpr (SES) {
-        // The window changes with admissions.  A slot's rows start on a frame boundary of its region, and every step's
-        // rows are fetched in order, so (frame, phase) restarts at the admission step and advances as above: no division.
+        // The window changes with admissions.  Every step's rows are fetched in order, so (frame, phase) restarts from
+        // the occupant's first row at its admission step and advances as above: no division.
 #pragma unroll
         for (int j = 0; j < COND_TASKS; ++j) {
           const int task = st + j * 128;
           creg[j][0] = make_float4(0.f, 0.f, 0.f, 0.f); creg[j][1] = creg[j][0];
           if (task < n_tasks) {
             const int f = task / KQ, c8 = task - f * KQ;
-            const int2 w = ses_win[f];
-            if (n == w.x) { tk_frame[j] = (unsigned)f * ses_frames; tk_phase[j] = 0; }
+            const int4 w = ses_win[f];
+            if (n == w.x) { tk_frame[j] = (unsigned)w.z; tk_phase[j] = (unsigned)w.w; }
             if (n >= w.x && n < w.y) {
               if (c8 >= FEAT / 8) {
                 const float4* s = reinterpret_cast<const float4*>(p.aux_frames + (size_t)tk_frame[j] * (4 * AUXD) + (c8 - FEAT / 8) * 8);
@@ -960,9 +964,15 @@ __global__ void __launch_bounds__(NT, 1) wrnn_tc_kernel(const TcParams p) {
     // only ever do ONE of {store an image, issue the chain} and neither sits in front of a gather they could already
     // have launched.
     // SES: the staging's windows of version `v` of the slot table (version -1 = buffer 1, before the loop), written
-    // between two barriers of the issuer warpgroup so that no staging thread reads a torn (a, e)
+    // between two barriers of the issuer warpgroup so that no staging thread reads a torn window.  Slot f's window is
+    // (a, the end of its rows: min(e, a + rows), frame and phase of its first row): one division per slot every 64 steps,
+    // none in the staging's step.
     auto ses_windows = [&](int v) {
-      if (it < B) { const SesEntry en = ld_ses_entry(p.ses_tab + v * MT + it); ses_win[it] = make_int2(en.a, en.e); }
+      if (it < B) {
+        const SesEntry en = ld_ses_entry(p.ses_tab + v * MT + it);
+        const unsigned fr = (unsigned)en.row0 / (unsigned)p.hop;
+        ses_win[it] = make_int4(en.a, (int)min((long long)en.e, (long long)en.a + en.rows), (int)fr, (int)((unsigned)en.row0 - fr * (unsigned)p.hop));
+      }
       named_bar_sync(3, 128);
     };
     if constexpr (SES) ses_windows(1);
